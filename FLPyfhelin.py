@@ -1,5 +1,5 @@
 """``from FLPyfhelin import *`` keeps working (notebook N:21): thin re-export of
-hefl_b200.compat.FLPyfhelin, the B200-native counterpart of /root/reference/FLPyfhelin.py."""
+hefl_b200.compat.FLPyfhelin, the H100-native counterpart of /root/reference/FLPyfhelin.py."""
 from hefl_b200.compat.FLPyfhelin import *  # noqa: F401,F403
 from hefl_b200.compat import FLPyfhelin as _impl
 

@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Headline benchmark: encrypted-FedAvg rounds on N B200 clients (BASELINE.json).
+"""Headline benchmark: encrypted-FedAvg rounds on N GPU clients (BASELINE.json).
 
 A *step* is one federated round of the reference's notebook cell 3 (N:233-272) for the medical
 CNN (FLPyfhelin.py:118-136): every client (one per GPU) runs ``local_epochs`` x
@@ -15,6 +15,7 @@ run is 2 client-rounds in 6583.64 s on an unnamed CPU (BASELINE.md).
   python -m torch.distributed.run --nproc-per-node 8 ... bench.py --gpus 8 --steps 5 --warmup 3
   python bench.py --impl reference    # the unmodified reference, if it can be installed
   python bench.py --impl baseline     # same pipeline on NCCL + cuDNN/cuBLAS (the bar to beat)
+  python bench.py --dump-outputs DIR  # also write the last timed round's results as DIR/<name>.npy
 """
 import argparse
 import json
@@ -37,8 +38,8 @@ def reference_arm(args):
 
         missing = [m for m in ("tensorflow", "Pyfhel", "kerastuner") if importlib.util.find_spec(m) is None]
         if missing:
-            why = ("reference needs " + ", ".join(missing) + " (FLPyfhelin.py:3-27); not installed and not in "
-                   "/opt/wheelhouse; the reference has no setup.py/pyproject so pip cannot install it either")
+            why = ("reference needs " + ", ".join(missing) + " (FLPyfhelin.py:3-27), which are not installed; "
+                   "the reference has no setup.py/pyproject so pip cannot install it either")
         elif not os.path.exists(os.path.join(ref_dir, "FLPyfhelin.py")):
             why = "baseline/_ref/FLPyfhelin.py missing"
     except Exception as e:  # noqa: BLE001
@@ -47,6 +48,28 @@ def reference_arm(args):
         why = "reference importable but no dataset folders image/Train, image/Test offline"
     print(json.dumps({"impl": "reference", "unavailable": why}))
     return 0
+
+
+DUMP_MAX_ELEMS = 4 << 20     # 16 MB of float32 per array; larger outputs are sampled at fixed, seeded indices
+
+
+def dump_outputs(out_dir, run):
+    """Write what the last timed round handed its caller: the global model after FedAvg (the flat parameter
+    vector every client installs) and the round's training loss / accuracy."""
+    import numpy as np
+    import torch
+
+    os.makedirs(out_dir, exist_ok=True)
+    rec = run.history[-1]
+    flat = run.pack.flat.detach().float().cpu()
+    if flat.numel() > DUMP_MAX_ELEMS:
+        idx = torch.randperm(flat.numel(), generator=torch.Generator().manual_seed(0))[:DUMP_MAX_ELEMS].sort().values
+        np.save(os.path.join(out_dir, "global_weights_sample_idx.npy"), idx.numpy().astype(np.float64))
+        flat = flat[idx]
+    np.save(os.path.join(out_dir, "global_weights.npy"), flat.numpy().astype(np.float32))
+    for key in ("loss", "accuracy"):
+        if rec.get(key) is not None:
+            np.save(os.path.join(out_dir, f"{key}.npy"), np.asarray([rec[key]], dtype=np.float64))
 
 
 def main():
@@ -67,6 +90,9 @@ def main():
                     help="skip the NCCL + cuDNN arm that the ours arm also times and reports as own_baseline")
     ap.add_argument("--dtype", default="bf16", choices=["bf16", "fp8"],
                     help="fp8: e4m3 1x1 convolutions for the ResNets (BASELINE configs[4]); the headline config is bf16")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed rounds, write what the last one computed (global weights, loss, accuracy) "
+                         "as DIR/<name>.npy; inputs are seeded, so two builds can be compared output for output")
     args = ap.parse_args()
     if args.impl == "reference":
         return reference_arm(args)
@@ -136,9 +162,13 @@ def main():
             except Exception:  # noqa: BLE001
                 nn_backend = "cudnn"
         transport = "nccl" if impl == "baseline" else (args.transport or "fused")
+        # deterministic_crypto: the key pair and the encryption randomness come from the seeded config instead of OS
+        # entropy (the same kernels, the same work), so that with the same arguments every run computes the same
+        # outputs and two builds can be compared output for output
         cfg = FLConfig(model=args.model, he_preset=args.he_preset, local_epochs=args.local_epochs,
                        steps_per_epoch=args.steps_per_epoch, val_steps=args.val_steps, clients=world,
-                       nn_backend=nn_backend, transport=transport, device="cuda", dtype=args.dtype)
+                       nn_backend=nn_backend, transport=transport, device="cuda", dtype=args.dtype,
+                       deterministic_crypto=True)
         if args.model.startswith("resnet"):
             cfg.image_size, cfg.num_classes = 224, 1000
         run = FederatedRunner(cfg, rank=rank, world=world, device=device)
@@ -191,6 +221,8 @@ def main():
         res["stage"] = run.history[-1]["stage_ms"]
         res["dev_ms"], res["dev_wall"] = dev_ms, dev_wall
         res["value"] = world * steps / (dev_ms / 1e3)
+        if args.dump_outputs and impl == args.impl and rank == 0:
+            dump_outputs(args.dump_outputs, run)
         res["shard_mb"] = (per - nval) * cfg.image_size * cfg.image_size * cfg.in_channels / 1e6
         return res
 

@@ -3,7 +3,7 @@
 kernel. Device-timed (CUDA events, warm-up, max over ranks). Launch with torchrun.
 
 Reports, per (n, L, algo): time, algorithm bandwidth S/t, bus bandwidth 2(P-1)/P * S/t and the
-fraction of the measured 770 GB/s per-direction NVLink peer bandwidth (B200_PROFILING.md).
+fraction of the nominal 450 GB/s per-direction NVLink 4 bandwidth of an H100 SXM.
 """
 import argparse
 import json
@@ -17,7 +17,7 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from hefl_b200.he.context import CKKSContext  # noqa: E402
 from hefl_b200.parallel import CollectiveTransport, FusedTransport  # noqa: E402
 
-NVLINK_GBS = 770.0
+NVLINK_GBS = 450.0                 # H100 SXM, NVLink 4, per direction (data sheet: 900 GB/s bidirectional)
 
 
 def timed(fn, iters, warmup, device):
@@ -82,8 +82,7 @@ def main():
             row["best_fused_ms"] = best
             row["speedup_vs_nccl"] = row["nccl_ms"] / best
             row["busbw_gbs"] = 2 * (world - 1) / world * nbytes / best / 1e6
-            row["frac_nvlink"] = row["busbw_gbs"] / NVLINK_GBS            # of the measured 770 GB/s peer copy
-            row["frac_nvlink_nominal"] = row["busbw_gbs"] / 900.0         # of the nominal 900 GB/s per direction
+            row["frac_nvlink_nominal"] = row["busbw_gbs"] / NVLINK_GBS
             row["best_algo"] = min((v, k[:-3]) for k, v in row.items() if k.endswith("_ms") and not k.startswith(("nccl", "best")))[1]
             results.append(row)
             if rank == 0:
@@ -92,7 +91,7 @@ def main():
             torch.cuda.empty_cache()
     if rank == 0:
         os.makedirs(os.path.dirname(args.out), exist_ok=True)
-        json.dump({"world": world, "nvlink_gbs_measured_peer_copy": NVLINK_GBS, "nvlink_gbs_nominal": 900.0,
+        json.dump({"world": world, "nvlink_gbs_nominal": NVLINK_GBS,
                    "rows": results}, open(args.out, "w"), indent=1)
     dist.destroy_process_group()
 

@@ -51,7 +51,7 @@ def launches(path):
 
 def main():
     os.makedirs(OUT, exist_ok=True)
-    md = ["# ncu captures (`--set full --clock-control none --import-source on`, one B200)\n",
+    md = ["# ncu captures (`--set full --clock-control none --import-source on`, one GPU)\n",
           f"Roofline denominators (MEASURED_PEAKS.json): HBM copy {PEAKS.get('hbm_gbs')} GB/s, cuBLAS bf16 "
           f"{PEAKS.get('bf16_tflops')} TFLOP/s burst.\n"]
     reports = []

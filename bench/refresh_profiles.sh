@@ -1,7 +1,6 @@
 #!/bin/bash
-# One GPU call that regenerates every single-GPU artefact under gpurun_out/ (about 6 GPU-minutes on a B200):
-#   /usr/local/graft/bin/gpurun --timeout 1500 -- 'bash bench/refresh_profiles.sh'
-# then, back on the CPU box:
+# Regenerates every single-GPU artefact (run from the repository root on the GPU machine);
+# then:
 #   python bench/make_profiles.py && python bench/roofline.py && python bench/make_sass.py
 # (multi-GPU artefacts: bash bench/run_mgpu.sh N and bash bench/run_pipe.sh N under gpurun --gpus N).
 set -u

@@ -7,8 +7,8 @@ import os
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
-HBM = float(peaks.get("hbm_gbs", peaks.get("hbm_copy_gbs", 6567.0)))           # GB/s
-TF = float(peaks.get("bf16_tflops", peaks.get("cublas_bf16_tflops", 1679.0)))    # TFLOP/s
+HBM = float(peaks.get("hbm_gbs", peaks.get("hbm_copy_gbs", 3350.0)))           # GB/s (H100 SXM data sheet)
+TF = float(peaks.get("bf16_tflops", peaks.get("cublas_bf16_tflops", 989.0)))     # TFLOP/s (H100 SXM data sheet, dense)
 t = json.load(open(os.path.join(ROOT, "profiles", "nn_micro.json")))
 
 B = 32
@@ -51,7 +51,7 @@ add("conv1 wgrad (round-1 kernel: FP32-pipe gather, fallback)", "wgrad0(gather f
     B * 256 * 256 * 32 + P_pool * 32 * 3, 2.0 * P_pool * 32 * 27)
 add("Adam (222,722 parameters, bf16 shadow)", "adam", 222722 * (4 * 7 + 2), 0)
 
-out = ["# Roofline table — one training step of the medical CNN, batch 32, one B200\n",
+out = ["# Roofline table — one training step of the medical CNN, batch 32, one H100\n",
        f"Denominators (MEASURED_PEAKS.json): HBM copy {HBM:.0f} GB/s, cuBLAS bf16 {TF:.0f} TFLOP/s. Times are the",
        "stand-alone kernel times of `profiles/nn_micro.json` (CUDA events, warm-up, L2 flushed between iterations);",
        "bytes and FLOPs are the analytic minimum for the kernel (operands read once, results written once;",

@@ -1,4 +1,4 @@
-// Integer-pipe microbenchmark for the NTT butterfly (sm_100a): issue rates of IMAD, IMAD.WIDE.U32,
+// Integer-pipe microbenchmark for the NTT butterfly (sm_90a): issue rates of IMAD, IMAD.WIDE.U32,
 // IMAD.HI.U32, IADD3, DFMA, mixes of them, __umul64hi and a complete Shoup butterfly, at 4/8/16
 // warps per scheduler. Prints warp-instructions per cycle per SM. Build: see bench/ubench/build.sh.
 #include <cstdint>
@@ -57,7 +57,9 @@ __global__ void k(uint64_t* out, uint32_t seed, uint64_t q, uint64_t w, uint64_t
 template <int MODE>
 void run(const char* name, int per_iter, int threads) {
   uint64_t* out;
-  const int blocks = 148;
+  int dev = 0, blocks = 0;
+  cudaGetDevice(&dev);
+  cudaDeviceGetAttribute(&blocks, cudaDevAttrMultiProcessorCount, dev);   // one CTA per SM
   cudaMalloc(&out, (size_t)(blocks * threads + 1) * 8);
   k<MODE><<<blocks, threads>>>(out, 12345u, 18014398509404161ull, 123456789123ull, 987654321987654321ull);
   cudaDeviceSynchronize();

@@ -6,7 +6,7 @@
 // Buffer layout on every rank: [C][2][L][N] u64 residues (< q_l < 2^61), symmetric address
 // space (peer r's buffer is mapped at bufs[r]). Three algorithms:
 //   two_shot  : rank r owns chunk r. It pulls chunk r from all P peers with 32-byte loads
-//               (ld.global.v4.u64, two per peer in flight), adds, reduces mod q_l in registers
+//               (two 16-byte loads each, two per peer in flight), adds, reduces mod q_l in registers
 //               and pushes the result into chunk r of all P buffers (in place). With a key
 //               holder, that rank owns no chunk: it never reads un-aggregated ciphertext.
 //   one_shot  : every rank pulls everything and writes a private output (latency-optimal for
@@ -83,20 +83,20 @@ __device__ __forceinline__ bool block_barrier(const AllReduceArgs& a, int slot, 
   return ok_flag != 0;
 }
 
-// 32-byte peer accesses (sm_100: ld/st.global.v4.u64). Relaxed at system scope: ordering
+// 32-byte peer accesses as two 16-byte ld/st.global.v2.u64 (sm_90 has no 256-bit global accesses). Relaxed at system scope: ordering
 // against the other GPUs comes from the release/acquire flag barriers around the data phase.
 struct U64x4 {
   uint64_t v[4];
 };
 __device__ __forceinline__ U64x4 ld32(const uint64_t* p) {
   U64x4 r;
-  asm volatile("ld.global.relaxed.sys.v4.u64 {%0, %1, %2, %3}, [%4];"
-               : "=l"(r.v[0]), "=l"(r.v[1]), "=l"(r.v[2]), "=l"(r.v[3]) : "l"(p) : "memory");
+  asm volatile("ld.global.relaxed.sys.v2.u64 {%0, %1}, [%2];" : "=l"(r.v[0]), "=l"(r.v[1]) : "l"(p) : "memory");
+  asm volatile("ld.global.relaxed.sys.v2.u64 {%0, %1}, [%2];" : "=l"(r.v[2]), "=l"(r.v[3]) : "l"(p + 2) : "memory");
   return r;
 }
 __device__ __forceinline__ void st32(uint64_t* p, const U64x4& r) {
-  asm volatile("st.global.relaxed.sys.v4.u64 [%0], {%1, %2, %3, %4};"
-               :: "l"(p), "l"(r.v[0]), "l"(r.v[1]), "l"(r.v[2]), "l"(r.v[3]) : "memory");
+  asm volatile("st.global.relaxed.sys.v2.u64 [%0], {%1, %2};" ::"l"(p), "l"(r.v[0]), "l"(r.v[1]) : "memory");
+  asm volatile("st.global.relaxed.sys.v2.u64 [%0], {%1, %2};" ::"l"(p + 2), "l"(r.v[2]), "l"(r.v[3]) : "memory");
 }
 __device__ __forceinline__ uint64_t mm_ld_add(const uint64_t* mc) {
   uint64_t v;
@@ -289,7 +289,7 @@ pairwise_mask_kernel(uint64_t* __restrict__ data, int64_t numel, int L, int logn
 void pairwise_mask(uint64_t* data, int64_t numel, int L, int logn, const MaskArgs& m, cudaStream_t st) {
   if (numel == 0 || m.npeers == 0) return;
   int blocks = (int)(((numel >> 1) + 255) / 256);
-  if (blocks > 148 * 8) blocks = 148 * 8;
+  if (blocks > hefl::cuda::device_sm_count() * 8) blocks = hefl::cuda::device_sm_count() * 8;
   pairwise_mask_kernel<<<blocks, 256, 0, st>>>(data, numel, L, logn, m);
   hefl::cuda::note_launch();
 }
@@ -321,7 +321,7 @@ __global__ void local_sum_modq_kernel(const uint64_t* const* __restrict__ srcs, 
 void local_sum_modq(const uint64_t* const* srcs_dev, int K, uint64_t* out, int64_t numel, int logn,
                     int L, const uint64_t* consts, cudaStream_t st) {
   int blocks = (int)(((numel >> 1) + 255) / 256);
-  if (blocks > 148 * 8) blocks = 148 * 8;
+  if (blocks > hefl::cuda::device_sm_count() * 8) blocks = hefl::cuda::device_sm_count() * 8;
   if (blocks < 1) blocks = 1;
   local_sum_modq_kernel<<<blocks, 256, 0, st>>>(srcs_dev, K, out, numel, logn, L, consts);
   hefl::cuda::note_launch();

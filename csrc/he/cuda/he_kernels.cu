@@ -1,4 +1,4 @@
-// sm_100a HE kernels: NTT/INTT, pointwise modular ops, CKKS encode/decode (special FFT),
+// sm_90a HE kernels: NTT/INTT, pointwise modular ops, CKKS encode/decode (special FFT),
 // fused public-key encrypt, fused decrypt, CRT centring, BFV fractional codec.
 // SURVEY.md §2.4 K3-K9, K11. Every kernel has a CPU twin in ../host_math.cpp and is
 // tested bit-exact (integer kernels) or to 1 ulp-of-rounding (FFT) against it.
@@ -15,10 +15,19 @@
 namespace hefl {
 namespace cuda {
 
+int device_sm_count() {
+  static int counts[64] = {};
+  int dev = 0;
+  cudaGetDevice(&dev);
+  if (dev < 0 || dev >= 64) dev = 0;
+  if (!counts[dev]) cudaDeviceGetAttribute(&counts[dev], cudaDevAttrMultiProcessorCount, dev);
+  return counts[dev];
+}
+
 static std::atomic<uint64_t> g_launches{0};
 uint64_t launch_count() { return g_launches.load(); }
 // Called by every host launcher right after its launch(es): counts our kernels (bench.py gpu_launches) and
-// turns a failed launch (bad configuration, missing sm_100a image, sticky asynchronous error) into an exception
+// turns a failed launch (bad configuration, missing sm_90a image, sticky asynchronous error) into an exception
 // instead of a silent no-op — the ops must fail loudly.
 void note_launch(uint64_t n) {
   g_launches.fetch_add(n);
@@ -356,7 +365,7 @@ void crt_center(const uint64_t* res, int64_t C, int k, int n, uint64_t q0, uint6
   CrtParams p{q0, q1, q1_ratio_lo, q1_ratio_hi, q0_inv_q1, k};
   const int64_t total = C * n;
   int blocks = (int)((total + 255) / 256);
-  if (blocks > 148 * 16) blocks = 148 * 16;
+  if (blocks > device_sm_count() * 16) blocks = device_sm_count() * 16;
   crt_center_kernel<<<blocks, 256, 0, st>>>(res, C, n, p, out);
   note_launch();
 }
@@ -436,7 +445,7 @@ void coeff_encode(const float* vals, int64_t C, int64_t nvals_total, int n, doub
   if (C == 0) return;
   const int64_t total = C * n;
   int blocks = (int)((total + 255) / 256);
-  if (blocks > 148 * 16) blocks = 148 * 16;
+  if (blocks > device_sm_count() * 16) blocks = device_sm_count() * 16;
   coeff_encode_kernel<<<blocks, 256, 0, st>>>(vals, total, nvals_total, scale, msg);
   note_launch();
 }
@@ -723,7 +732,7 @@ void bfv_scale_round(const uint64_t* x, int64_t C, int n, uint64_t q, uint64_t p
   if (C == 0) return;
   const int64_t total = C * n;
   int blocks = (int)((total + 255) / 256);
-  if (blocks > 148 * 16) blocks = 148 * 16;
+  if (blocks > device_sm_count() * 16) blocks = device_sm_count() * 16;
   bfv_scale_round_kernel<<<blocks, 256, 0, st>>>(x, total, q, p, out);
   note_launch();
 }
@@ -740,7 +749,7 @@ void digit_extract(const uint64_t* x, int64_t rows, int n, int shift, int bits, 
   if (rows == 0) return;
   const int64_t total = rows * n;
   int blocks = (int)((total + 255) / 256);
-  if (blocks > 148 * 16) blocks = 148 * 16;
+  if (blocks > device_sm_count() * 16) blocks = device_sm_count() * 16;
   const uint64_t mask = bits >= 64 ? ~0ull : ((1ull << bits) - 1);
   digit_extract_kernel<<<blocks, 256, 0, st>>>(x, total, shift, mask, out);
   note_launch();

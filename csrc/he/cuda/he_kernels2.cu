@@ -1,4 +1,4 @@
-// Persistent, TMA-fed, cluster-shared-twiddle HE kernels for sm_100a (SURVEY.md K3, K4, K6, K7):
+// Persistent, TMA-fed, cluster-shared-twiddle HE kernels for sm_90a (SURVEY.md K3, K4, K6, K7):
 //
 //   ntt2_kernel      in-place NTT / INTT of rows [rows][N]; coefficients travel by TMA tensor
 //                    copies (SWIZZLE_128B) through a double-buffered shared-memory ring fed by a
@@ -280,9 +280,9 @@ __device__ __forceinline__ void enc_epilogue(uint32_t bufA, uint32_t bufU, const
       ldg256(pp + 8 * v, pk[0]);
       ldg256(pp + 8 * v + 4, pk[1]);
       if constexpr (USCR) {
-        asm volatile("ld.global.v4.u64 {%0, %1, %2, %3}, [%4];"
-                     : "=l"(uh[0]), "=l"(uh[1]), "=l"(uh[2]), "=l"(uh[3])
-                     : "l"(uscr + G.base + 4 * v)
+        asm volatile("ld.global.v2.u64 {%0, %1}, [%2];" : "=l"(uh[0]), "=l"(uh[1]) : "l"(uscr + G.base + 4 * v)
+                     : "memory");
+        asm volatile("ld.global.v2.u64 {%0, %1}, [%2];" : "=l"(uh[2]), "=l"(uh[3]) : "l"(uscr + G.base + 4 * v + 2)
                      : "memory");
       } else {
         lds128(bufU + row + (((ch0 + 2 * v) ^ rs) << 4), uh[0], uh[1]);
@@ -656,7 +656,7 @@ void launch_encrypt2(EncArgs a, cudaStream_t st) {
   set_smem(k, Smem<LOGN, NBUF>::kTotal);
   const int grid = grid_ctas(1);
   if (LOGN >= 14) {
-    // u_hat of the ciphertext in flight: one row per CTA, allocated once per device (19 MB for 148 CTAs), L2 resident
+    // u_hat of the ciphertext in flight: one row per CTA, allocated once per device (about 17 MB for 132 CTAs), L2 resident
     static uint64_t* scratch[16] = {nullptr};
     int dev = 0;
     cudaGetDevice(&dev);

@@ -1,4 +1,4 @@
-// Shared-memory negacyclic NTT / INTT device routines for sm_100a (SURVEY.md K3, K4).
+// Shared-memory negacyclic NTT / INTT device routines for sm_90a (SURVEY.md K3, K4).
 //
 // One CTA transforms one contiguous block of 2^logb coefficients held in shared
 // memory (the whole polynomial when logb == logn; N = 32768 is split into two

@@ -1,4 +1,4 @@
-// Second-generation negacyclic NTT device routines for sm_100a (SURVEY.md K3, K4).
+// Second-generation negacyclic NTT device routines for sm_90a (SURVEY.md K3, K4).
 //
 // What changed against ntt.cuh (which stays as the path for N = 32768 and primes >= 2^58):
 //
@@ -74,14 +74,14 @@ __device__ __forceinline__ void sts128(uint32_t a, uint64_t x, uint64_t y) {
 __device__ __forceinline__ void ldg128(const uint64_t* p, uint64_t& x, uint64_t& y) {
   asm volatile("ld.global.nc.v2.u64 {%0, %1}, [%2];" : "=l"(x), "=l"(y) : "l"(p));
 }
-// 32-byte global accesses (sm_100: ld/st.global.v4.u64)
+// 32 bytes of global memory as two 16-byte accesses (sm_90 has no 256-bit ld/st.global)
 __device__ __forceinline__ void ldg256(const uint64_t* p, uint64_t (&v)[4]) {
-  asm volatile("ld.global.nc.v4.u64 {%0, %1, %2, %3}, [%4];"
-               : "=l"(v[0]), "=l"(v[1]), "=l"(v[2]), "=l"(v[3])
-               : "l"(p));
+  ldg128(p, v[0], v[1]);
+  ldg128(p + 2, v[2], v[3]);
 }
 __device__ __forceinline__ void stg256(uint64_t* p, uint64_t a, uint64_t b, uint64_t c, uint64_t d) {
-  asm volatile("st.global.v4.u64 [%0], {%1, %2, %3, %4};" ::"l"(p), "l"(a), "l"(b), "l"(c), "l"(d) : "memory");
+  asm volatile("st.global.v2.u64 [%0], {%1, %2};" ::"l"(p), "l"(a), "l"(b) : "memory");
+  asm volatile("st.global.v2.u64 [%0], {%1, %2};" ::"l"(p + 2), "l"(c), "l"(d) : "memory");
 }
 
 // Per-limb state of a persistent CTA.

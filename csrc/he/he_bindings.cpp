@@ -1,5 +1,5 @@
 // torch.ops.hefl.* bindings for the HE core. Each op dispatches on the device of its
-// tensor arguments: CUDA tensors go to the sm_100a kernels (kernels.h), CPU tensors to the
+// tensor arguments: CUDA tensors go to the sm_90a kernels (kernels.h), CPU tensors to the
 // host implementation (host_math.h). u64 words travel as torch.int64 (same bits).
 #include <ATen/cuda/CUDAContext.h>
 #include <torch/library.h>

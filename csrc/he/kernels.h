@@ -1,4 +1,4 @@
-// Launchers of the sm_100a HE kernels (csrc/he/cuda/he_kernels.cu). Plain C++
+// Launchers of the sm_90a HE kernels (csrc/he/cuda/he_kernels.cu). Plain C++
 // signatures with raw device pointers so the .cu files compile without the
 // PyTorch headers (seconds, not minutes); csrc/bindings.cpp adapts tensors.
 //
@@ -87,6 +87,8 @@ void shoup_pairs(const uint64_t* x, uint64_t* out, int64_t rows, int L, int n, c
 // Number of kernels launched by this library since process start (bench.py's gpu_launches).
 uint64_t launch_count();
 void note_launch(uint64_t n = 1);
+// SM count of the current device (cached per device): grid caps of grid-stride kernels scale with it.
+int device_sm_count();
 
 }  // namespace cuda
 }  // namespace hefl

@@ -1,4 +1,4 @@
-// tcgen05 / TMEM / TMA implicit-GEMM 3x3 convolution for sm_100a (SURVEY.md K13-K15).
+// TMA-fed implicit-GEMM 3x3 convolution on the tensor cores for sm_90a (SURVEY.md K13-K15).
 //
 // Activations are NHWC bf16 viewed as a 2-D matrix [P = B*H*W pixels, C channels]. A 3x3 valid
 // convolution is then 9 "tap" GEMMs whose A operand is the SAME matrix shifted by
@@ -6,24 +6,20 @@
 // with h >= H-2 or w >= W-2 are garbage and masked). Each tap's A tile is therefore one plain
 // 2-D TMA box — no im2col buffer, no gather.
 //
-//   conv_fwd_pool : per CTA tile = 2 image rows x 128 columns (two TMEM accumulators) so that the
-//                   epilogue does bias + ReLU + 2x2 max-pool + argmax straight out of TMEM (vertical
+//   conv_fwd_pool : per CTA tile = 2 image rows x 128 columns (two accumulators) so that the
+//                   epilogue does bias + ReLU + 2x2 max-pool + argmax straight from the accumulators (vertical
 //                   max in-thread across the two accumulators, horizontal max by one shuffle) and
 //                   writes only the pooled tensor (4x less HBM traffic than the conv output).
 //   conv_dgrad    : dX[m,:] = sum_taps dY[m - off, :] * W[r,s]   (same kernel, negative offsets,
 //                   plain bf16 store).
 //   conv_wgrad    : dW[r,s] = sum_m X[m+off,:]^T dY[m,:]. Both operands are consumed in their
-//                   native [P, C] layout as MN-major UMMA operands (pixels = K), so no transposed
-//                   copies exist; taps are stacked along M (128/C tap atoms per MMA group), split-K
-//                   over pixels, fp32 vector-RED into a [9*C+1, Co] buffer whose extra row is the
-//                   bias gradient (an all-ones tap atom).
+//                   native [P, C] layout (ldmatrix.trans, pixels = K), so no transposed copies exist;
+//                   split-K over pixels and over filter rows, fp32 vector-RED into a [9*C+1, Co] buffer whose
+//                   extra row is the bias gradient.
 //
-// Warp roles: epilogue warps first (TMEM -> registers -> global; 8 in the tap-GEMM kernel, 4 in wgrad),
-// then the TMA producer warp, then the MMA issuer warp (+TMEM owner). The two single-thread roles get the highest
-// warp ids because the issue arbiter favours high warp ids (B300_MICROARCH.md): polling epilogue
-// warps must not starve them (measured: 1.8x on the layer-1 weight gradient). smem ring of halo tiles with full/empty
-// mbarriers; two TMEM tile buffers so the epilogue of tile i overlaps the MMAs of tile i+1.
-// Weights for all 9 taps stay resident in shared memory for the CTA's lifetime.
+// Warp roles: eight compute warps (mma.sync with fp32 accumulators in registers, then the epilogue), one TMA
+// producer warp; a smem ring of halo tiles with full/empty mbarriers lets TMA fill tile i+1 while tile i is
+// multiplied. Weights for all 9 taps stay resident in shared memory for the CTA's lifetime.
 #include <cuda_bf16.h>
 
 #include <cstdio>
@@ -96,9 +92,8 @@ static int num_sms() {
 // ------------------------------------------------------------------------------------------
 // G1: halo-tile tap-GEMM kernel (forward + pool epilogue, or dgrad with plain store)
 //
-// Measured on B200 (bench/probe_shift.py): a K-major swizzled tile written by TMA can be read by
-// tcgen05.mma starting at ANY row (descriptor start address + rows*row_bytes, base_offset 0) —
-// the swizzle is a function of absolute shared-memory address bits. So each input row segment
+// A K-major swizzled tile written by TMA can be read starting at ANY row: the swizzle is a function of
+// absolute shared-memory address bits (tc_common.cuh swz<>; umma_shift_probe checks it on the device). So each input row segment
 // is loaded ONCE per tile and all 9 taps address shifted windows of it:
 //   forward : tile = 2 image rows x 128 columns; 4 halo segments (rows h..h+3) of 130 pixels;
 //             accumulator j (row h+j), tap (r,s) reads segment j+r at row offset s.
@@ -153,45 +148,38 @@ struct TapGemmCfg {
   static constexpr int W_TAP = W_SUB * NKB;
   static constexpr int W_BYTES = NTAP * W_TAP;
   static constexpr int BAR_BYTES = 384;
-  static constexpr int BUDGET = 225 * 1024;
-  static constexpr int NBUF_RAW = (BUDGET - W_BYTES - BAR_BYTES - 1024) / HALO;
-  // ring depth beyond 3 and more than 2 TMEM tile buffers measured no gain; small footprints let a
-  // wgrad CTA and a dgrad/forward CTA share an SM (the backward pass runs them on two streams)
+  static constexpr int SCR_BYTES = 8 * 1024;              // 1 KB accumulator staging per compute warp
+  static constexpr int FIXED = W_BYTES + BAR_BYTES + SCR_BYTES + 1024;
+  static constexpr int NBUF_RAW = (kSmemMax - FIXED) / HALO;
+  // a ring deeper than 2 halo tiles measured no gain; the second tile overlaps TMA with the MMAs
   static constexpr int NBUF = NBUF_RAW > 2 ? 2 : NBUF_RAW;
-  static constexpr int SMEM = W_BYTES + NBUF * HALO + BAR_BYTES + 1024;
-  // TMEM tile buffers: the MMA -> epilogue -> MMA hand-off costs ~1500 cycles of mbarrier latency
-  // (measured with all work disabled: 750 cycles/tile with 2 buffers), so small-channel layers use
-  // up to 8 buffers to keep several tiles in flight.
-  static constexpr int NT_RAW = 512 / (NACC * CO);
-  static constexpr int NT = NT_RAW > 2 ? 2 : NT_RAW;
-  static constexpr int ACC_COLS = NT * NACC * CO;
-  static constexpr int TMEM_COLS = ACC_COLS <= 32 ? 32 : (ACC_COLS <= 64 ? 64 : (ACC_COLS <= 128 ? 128 : (ACC_COLS <= 256 ? 256 : 512)));
-  static_assert(NT >= 2, "need at least two TMEM tile buffers");
-  // two CTAs per SM when shared memory and TMEM allow: the kernels are latency-bound (issue, TMA,
-  // mbarrier hand-offs), so more independent pipelines on the same SM fill the bubbles
-  static constexpr int OCC = (3 * SMEM <= 226 * 1024 && 3 * TMEM_COLS <= 512) ? 3
-                             : ((2 * SMEM <= 226 * 1024 && 2 * TMEM_COLS <= 512) ? 2 : 1);
+  static constexpr int SMEM = FIXED + NBUF * HALO;
+  // 8-channel chunks per warp and pass: accumulators = NACC x NG x 2 m16 tiles x 4 floats = 64 registers or fewer
+  static constexpr int NG = (CO / 16) < (8 / NACC) ? (CO / 16) : (8 / NACC);
+  static constexpr int OCC = blocks_fit(SMEM, 2) ? 2 : 1;
   static_assert(NBUF >= 1, "halo tile does not fit in shared memory");
-  static_assert(ACC_COLS <= 512, "accumulators exceed TMEM");
+  static_assert(NG % 2 == 0 && (CO / 16) % NG == 0, "chunk groups");
   static_assert(CO % 32 == 0 && CO <= 128, "CO must be 32, 64, 96 or 128");
 };
 
+// Warp roles: warps 0..7 compute and run the epilogue (warp w owns GEMM rows 32*(w%4) .. +31 and the 8-channel
+// chunks w/4, w/4 + 2, ...), warp 8 is the TMA producer. Accumulators live in registers (mma.sync m16n8k16); the
+// halo ring of NBUF tiles lets TMA fill tile i+1 while tile i is multiplied.
 template <int CK, int CO, bool POOL, int TS>
-__global__ void __launch_bounds__(352, TapGemmCfg<CK, CO, POOL, TS>::OCC)
+__global__ void __launch_bounds__(288, TapGemmCfg<CK, CO, POOL, TS>::OCC)
 tap_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmW,
                 const TapGemmArgs a) {
   using Cfg = TapGemmCfg<CK, CO, POOL, TS>;
+  constexpr int RB = Cfg::ROW_BYTES;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* sW = smem;
   uint8_t* sA = smem + Cfg::W_BYTES;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(sA + Cfg::NBUF * Cfg::HALO);
+  float* scr_all = reinterpret_cast<float*>(sA + Cfg::NBUF * Cfg::HALO);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(reinterpret_cast<uint8_t*>(scr_all) + Cfg::SCR_BYTES);
   uint64_t* full = bars;                       // [NBUF]
   uint64_t* empty = bars + Cfg::NBUF;          // [NBUF]
   uint64_t* wfull = bars + 2 * Cfg::NBUF;      // [1]
-  uint64_t* tfull = wfull + 1;                 // [NT]
-  uint64_t* tempty = tfull + Cfg::NT;          // [NT]
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tempty + Cfg::NT);
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -199,17 +187,11 @@ tap_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
   if (warp == 8 && lane == 0) {
     prefetch_tmap(&tmA);
     prefetch_tmap(&tmW);
-    // POOL: two MMA-issuing warps (one per accumulator) => 2 commits per buffer / tile
-    for (int s = 0; s < Cfg::NBUF; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], Cfg::NACC); }
+    for (int s = 0; s < Cfg::NBUF; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 8); }
     mbar_init(wfull, 1);
-    for (int i = 0; i < Cfg::NT; ++i) { mbar_init(&tfull[i], Cfg::NACC); mbar_init(&tempty[i], 8); }
     fence_barrier_init();
   }
-  if (warp == 9) tmem_alloc<Cfg::TMEM_COLS>(tmem_slot);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
   // PDL: the set-up above and the weight tile (written only by the re-layout kernel, which never triggers its
   // dependents early — launch.cuh) overlap the previous kernel's tail; activations only after the wait.
   pdl_trigger();
@@ -258,178 +240,158 @@ tap_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
         if (++buf == Cfg::NBUF) { buf = 0; phase ^= 1; }
       }
     }
-  } else if (warp == 9 || warp == 10) {
-    // ===== MMA issuers: warp 9 owns accumulator 0, warp 10 accumulator 1 (the small-N MMAs of these
-    // layers are bound by per-thread issue cost, not by the tensor core, so two issuers run in parallel)
-    const int jme = warp - 9;
-    if (jme >= Cfg::NACC) goto done_roles;
-    constexpr uint32_t idesc = make_idesc_bf16(128, CO);
+  } else {
+    // ===== compute + epilogue warps (0..7): rows qd*32 .. +31, channel chunks grp, grp + 2, ...
+    const int qd = warp & 3;
+    const int grp = warp >> 2;
+    float* scr = scr_all + warp * 256;
+    const uint32_t w_base = smem_u32(sW);
     mbar_wait(wfull, 0);
-    tc_fence_after();
     int buf = 0;
     uint32_t phase = 0;
-    int tb = 0;
-    uint32_t tb_phase = 0;
     for (int t = blockIdx.x; t < a.num_tiles; t += gridDim.x) {
-      mbar_wait(&tempty[tb], tb_phase ^ 1);
       mbar_wait(&full[buf], phase);
-      tc_fence_after();
-      if (elect_one()) {
-        // descriptor low words: base + compile-time offsets (pure 32-bit adds per MMA)
-        const uint32_t a_lo = desc_lo(smem_u32(sA + buf * Cfg::HALO));
-        const uint32_t w_lo = desc_lo(smem_u32(sW));
-        constexpr uint32_t hi = desc_hi(8 * Cfg::ROW_BYTES, Cfg::ROW_BYTES);
+      const uint32_t a_base = smem_u32(sA + buf * Cfg::HALO);
+#pragma unroll 1
+      for (int g = 0; g < CO / 16 / Cfg::NG; ++g) {
+        float acc[Cfg::NACC][Cfg::NG][2][4];
 #pragma unroll
-        for (int j = 0; j < Cfg::NACC; ++j) {
+        for (int j = 0; j < Cfg::NACC; ++j)
+#pragma unroll
+          for (int i = 0; i < Cfg::NG; ++i)
+#pragma unroll
+            for (int mt = 0; mt < 2; ++mt)
+#pragma unroll
+              for (int q = 0; q < 4; ++q) acc[j][i][mt][q] = 0.f;
 #ifdef HEFL_CONV_DEBUG
-          if (a.dbg & 2) continue;
+        if (!(a.dbg & 2))
 #endif
-          if (j != jme) continue;
-          const uint32_t d_tmem = tmem_base + (tb * Cfg::NACC + j) * CO;
+#pragma unroll 1
+        for (int tap = 0; tap < Cfg::NTAP; ++tap) {
+          const int r = tap / TS, s = tap % TS;
+          const int shift = POOL ? s : (2 - s);
 #pragma unroll
-          for (int tap = 0; tap < Cfg::NTAP; ++tap) {
-            const int r = tap / TS, s = tap % TS;
-            const int seg = POOL ? (j + r) : r;
-            const int shift = POOL ? s : (2 - s);
+          for (int kb = 0; kb < Cfg::NKB; ++kb) {
 #pragma unroll
-            for (int kb = 0; kb < Cfg::NKB; ++kb) {
+            for (int k = 0; k < Cfg::KB / 16; ++k) {
+              uint32_t bf[Cfg::NG / 2][4];
 #pragma unroll
-              for (int k = 0; k < Cfg::KB / 16; ++k) {
-                const uint32_t ao = ((kb * Cfg::NSEG + seg) * Cfg::SEG_BYTES + shift * Cfg::ROW_BYTES + k * 32) >> 4;
-                const uint32_t wo = (tap * Cfg::W_TAP + kb * Cfg::W_SUB + k * 32) >> 4;
-                umma_bf16_lh(d_tmem, a_lo + ao, hi, w_lo + wo, hi, idesc, (tap | kb | k) != 0 ? 1u : 0u);
+              for (int i = 0; i < Cfg::NG; i += 2) {
+                const int c0 = grp + 2 * (g * Cfg::NG + i);
+                ld_b_kmajor<RB>(w_base + tap * Cfg::W_TAP + kb * Cfg::W_SUB, c0 * 8, (c0 + 2) * 8, k * 32, lane,
+                                bf[i / 2]);
               }
-            }
-          }
-        }
-        umma_commit(&empty[buf]);
-        umma_commit(&tfull[tb]);
-      }
-      __syncwarp();
-      if (++buf == Cfg::NBUF) { buf = 0; phase ^= 1; }
-      if (++tb == Cfg::NT) { tb = 0; tb_phase ^= 1; }
-    }
-  } else {
-    // ===== epilogue warps (0..7): quadrant = warp % 4, channel slice = warp / 4 (8 channels a time).
-    // (16 epilogue warps measured no faster than 8; 8 keeps the CTA small enough for 2 CTAs per SM.)
-    const int qd = warp & 3;                       // TMEM lane quadrant this warp may read
-    const int grp = warp >> 2;
-    const uint32_t lane_base = (uint32_t)(qd * 32) << 16;
-    int tb = 0;
-    uint32_t tb_phase = 0;
-    for (int t = blockIdx.x; t < a.num_tiles; t += gridDim.x) {
-      mbar_wait(&tfull[tb], tb_phase);
-      tc_fence_after();
-      if (POOL) {
-        const int per_img = a.Hp * a.tiles_w;
-        const int b = fast_div(t, per_img, a.magic_per_img);
-        const int rem = t - b * per_img;
-        const int hp = fast_div(rem, a.tiles_w, a.magic_tiles_w);
-        const int tw = rem - hp * a.tiles_w;
-        const int col = tw * 128 + qd * 32 + lane;           // conv-output column of this thread
-        const int wp = col >> 1;
-        const bool writer = wp < a.Wp;
-        const bool odd = (lane & 1) != 0;
-#pragma unroll 1
-#ifdef HEFL_CONV_DEBUG
-        const int ch_end = (a.dbg & 4) ? 0 : CO / 8;
-#else
-        constexpr int ch_end = CO / 8;
-#endif
-        for (int ch = grp; ch < ch_end; ch += 2) {
-          float v0[8], v1[8];
-          tmem_ld8_nowait(tmem_base + lane_base + (tb * 2 + 0) * CO + ch * 8, v0);
-          tmem_ld8_nowait(tmem_base + lane_base + (tb * 2 + 1) * CO + ch * 8, v1);
-          // the two lanes of a window split the 8 channels: even lane -> 0..3, odd lane -> 4..7 (the epilogue is
-          // issue-bound — ncu: 64 % issue active, 5 % tensor pipe — so no lane may do redundant work)
-          const float4 bq = __ldg(reinterpret_cast<const float4*>(a.bias + ch * 8 + (odd ? 4 : 0)));
-          const float bias4[4] = {bq.x, bq.y, bq.z, bq.w};
-          tmem_ld_wait();
-          // max over the two image rows on the raw accumulators (bias + ReLU commute with max)
-          uint32_t vbits = 0;                                 // 1 = lower image row wins
 #pragma unroll
-          for (int c = 0; c < 8; ++c) {
-            const bool lw = v1[c] > v0[c];
-            v0[c] = lw ? v1[c] : v0[c];
-            vbits |= lw ? (1u << c) : 0u;
-          }
-          const uint32_t pvbits = __shfl_xor_sync(0xffffffffu, vbits, 1);
-          const uint32_t mb = (vbits >> (odd ? 4 : 0)) & 15u;   // row bits of my column, my 4 channels
-          const uint32_t pb = (pvbits >> (odd ? 4 : 0)) & 15u;  // ... of the partner's column
-          float x[4];
-          uint32_t idx = 0u;
+              for (int j = 0; j < Cfg::NACC; ++j) {
+                const int seg = POOL ? (j + r) : r;
+                const uint32_t seg_base = a_base + (kb * Cfg::NSEG + seg) * Cfg::SEG_BYTES;
 #pragma unroll
-          for (int i = 0; i < 4; ++i) {
-            const float keep = odd ? v0[4 + i] : v0[i];
-            const float send = odd ? v0[i] : v0[4 + i];
-            const float recv = __shfl_xor_sync(0xffffffffu, send, 1);
-            const float left = odd ? recv : keep, right = odd ? keep : recv;
-            const bool rw = right > left;                       // right column wins only if strictly greater
-            const uint32_t rowbit = ((rw != odd) ? (pb >> i) : (mb >> i)) & 1u;
-            const float y = (rw ? right : left) + bias4[i];
-            // bits 0-1: arg-max position (row*2 + col) in the window, bit 2: unit active (ReLU mask)
-            idx |= ((rowbit << 1) | (rw ? 1u : 0u) | (y > 0.f ? 4u : 0u)) << (i * 8);
-            x[i] = y > 0.f ? y : 0.f;
-          }
-          if (writer) {
-            const size_t o = ((size_t)(b * a.Hp + hp) * a.Wp + wp) * CO + ch * 8 + (odd ? 4 : 0);
-            *reinterpret_cast<uint2*>(a.out + o) = make_uint2(pack_bf16x2(x[0], x[1]), pack_bf16x2(x[2], x[3]));
-            if (a.argmax) *reinterpret_cast<uint32_t*>(a.argmax + o) = idx;
-          }
-        }
-      } else {
-        const int m = t * 128 + qd * 32 + lane;
-        size_t up_base = 0;                                   // pixel index of the window's top-left position
-        if (a.up_amax && m < a.P) {
-          const int hw = a.H * a.W;
-          const int b = m / hw, rem = m - b * hw;
-          const int y = rem / a.W, x = rem - y * a.W;
-          up_base = ((size_t)b * a.up_W + 2 * y) * a.up_W + 2 * x;
-        }
-#pragma unroll 1
-        for (int ch = grp; ch < CO / 8; ch += 2) {
-          float v[8];
-          tmem_ld8_nowait(tmem_base + lane_base + tb * CO + ch * 8, v);
-          tmem_ld_wait();
-          if (m < a.P) {
-            const int c0 = blockIdx.y * CO + ch * 8;
-            const uint32_t pk[4] = {pack_bf16x2(v[0], v[1]), pack_bf16x2(v[2], v[3]), pack_bf16x2(v[4], v[5]),
-                                    pack_bf16x2(v[6], v[7])};
-            if (a.up_amax == nullptr) {
-              *reinterpret_cast<uint4*>(a.out + (size_t)m * a.co_total + c0) = make_uint4(pk[0], pk[1], pk[2], pk[3]);
-            } else {
-              const uint2 code = *reinterpret_cast<const uint2*>(a.up_amax + (size_t)m * a.co_total + c0);
-              const uint32_t cw[2] = {code.x, code.y};
+                for (int mt = 0; mt < 2; ++mt) {
+                  uint32_t af[4];
+                  ld_a_kmajor<RB>(seg_base, shift + qd * 32 + mt * 16, k * 32, lane, af);
 #pragma unroll
-              for (int q = 0; q < 4; ++q) {
-                uint32_t o[4];
-#pragma unroll
-                for (int i = 0; i < 4; ++i) {
-                  const uint32_t ca = (cw[i >> 1] >> ((i & 1) * 16)) & 0xFFu;          // channel 2i
-                  const uint32_t cb = (cw[i >> 1] >> ((i & 1) * 16 + 8)) & 0xFFu;      // channel 2i+1
-                  const uint32_t lo = (ca == (4u | q)) ? (pk[i] & 0xFFFFu) : 0u;
-                  const uint32_t hi = (cb == (4u | q)) ? (pk[i] & 0xFFFF0000u) : 0u;
-                  o[i] = lo | hi;
+                  for (int i = 0; i < Cfg::NG; ++i)
+                    mma_bf16(acc[j][i][mt], af, bf[i / 2][(i & 1) * 2], bf[i / 2][(i & 1) * 2 + 1]);
                 }
-                const size_t px = up_base + (size_t)(q >> 1) * a.up_W + (q & 1);
-                *reinterpret_cast<uint4*>(a.out + px * a.co_total + c0) = make_uint4(o[0], o[1], o[2], o[3]);
+              }
+            }
+          }
+        }
+        if (g == CO / 16 / Cfg::NG - 1) {
+          __syncwarp();
+          if (lane == 0) mbar_arrive(&empty[buf]);     // this warp's last read of the halo tile is done
+        }
+#pragma unroll
+        for (int i = 0; i < Cfg::NG; ++i) {
+          const int ch = grp + 2 * (g * Cfg::NG + i);
+#ifdef HEFL_CONV_DEBUG
+          if (a.dbg & 4) continue;
+#endif
+          if (POOL) {
+            const int per_img = a.Hp * a.tiles_w;
+            const int b = fast_div(t, per_img, a.magic_per_img);
+            const int rem = t - b * per_img;
+            const int hp = fast_div(rem, a.tiles_w, a.magic_tiles_w);
+            const int tw = rem - hp * a.tiles_w;
+            const int col = tw * 128 + qd * 32 + lane;           // conv-output column of this thread
+            const int wp = col >> 1;
+            const bool writer = wp < a.Wp;
+            const bool odd = (lane & 1) != 0;
+            float v0[8], v1[8];
+            frag_rows(scr, acc[0][i][0], acc[0][i][1], lane, v0);
+            frag_rows(scr, acc[Cfg::NACC - 1][i][0], acc[Cfg::NACC - 1][i][1], lane, v1);
+            // the two lanes of a window split the 8 channels: even lane -> 0..3, odd lane -> 4..7
+            const float4 bq = __ldg(reinterpret_cast<const float4*>(a.bias + ch * 8 + (odd ? 4 : 0)));
+            const float bias4[4] = {bq.x, bq.y, bq.z, bq.w};
+            // max over the two image rows on the raw accumulators (bias + ReLU commute with max)
+            uint32_t vbits = 0;                                 // 1 = lower image row wins
+#pragma unroll
+            for (int c = 0; c < 8; ++c) {
+              const bool lw = v1[c] > v0[c];
+              v0[c] = lw ? v1[c] : v0[c];
+              vbits |= lw ? (1u << c) : 0u;
+            }
+            const uint32_t pvbits = __shfl_xor_sync(0xffffffffu, vbits, 1);
+            const uint32_t mb = (vbits >> (odd ? 4 : 0)) & 15u;   // row bits of my column, my 4 channels
+            const uint32_t pb = (pvbits >> (odd ? 4 : 0)) & 15u;  // ... of the partner's column
+            float x[4];
+            uint32_t idx = 0u;
+#pragma unroll
+            for (int q = 0; q < 4; ++q) {
+              const float keep = odd ? v0[4 + q] : v0[q];
+              const float send = odd ? v0[q] : v0[4 + q];
+              const float recv = __shfl_xor_sync(0xffffffffu, send, 1);
+              const float left = odd ? recv : keep, right = odd ? keep : recv;
+              const bool rw = right > left;                       // right column wins only if strictly greater
+              const uint32_t rowbit = ((rw != odd) ? (pb >> q) : (mb >> q)) & 1u;
+              const float y = (rw ? right : left) + bias4[q];
+              // bits 0-1: arg-max position (row*2 + col) in the window, bit 2: unit active (ReLU mask)
+              idx |= ((rowbit << 1) | (rw ? 1u : 0u) | (y > 0.f ? 4u : 0u)) << (q * 8);
+              x[q] = y > 0.f ? y : 0.f;
+            }
+            if (writer) {
+              const size_t o = ((size_t)(b * a.Hp + hp) * a.Wp + wp) * CO + ch * 8 + (odd ? 4 : 0);
+              *reinterpret_cast<uint2*>(a.out + o) = make_uint2(pack_bf16x2(x[0], x[1]), pack_bf16x2(x[2], x[3]));
+              if (a.argmax) *reinterpret_cast<uint32_t*>(a.argmax + o) = idx;
+            }
+          } else {
+            const int m = t * 128 + qd * 32 + lane;
+            float v[8];
+            frag_rows(scr, acc[0][i][0], acc[0][i][1], lane, v);
+            if (m < a.P) {
+              const int c0 = blockIdx.y * CO + ch * 8;
+              const uint32_t pk[4] = {pack_bf16x2(v[0], v[1]), pack_bf16x2(v[2], v[3]), pack_bf16x2(v[4], v[5]),
+                                      pack_bf16x2(v[6], v[7])};
+              if (a.up_amax == nullptr) {
+                *reinterpret_cast<uint4*>(a.out + (size_t)m * a.co_total + c0) = make_uint4(pk[0], pk[1], pk[2], pk[3]);
+              } else {
+                const int hw = a.H * a.W;
+                const int b = m / hw, rem = m - b * hw;
+                const int y = rem / a.W, x = rem - y * a.W;
+                const size_t up_base = ((size_t)b * a.up_W + 2 * y) * a.up_W + 2 * x;   // window's top-left pixel
+                const uint2 code = *reinterpret_cast<const uint2*>(a.up_amax + (size_t)m * a.co_total + c0);
+                const uint32_t cw[2] = {code.x, code.y};
+#pragma unroll
+                for (int q = 0; q < 4; ++q) {
+                  uint32_t o[4];
+#pragma unroll
+                  for (int e = 0; e < 4; ++e) {
+                    const uint32_t ca = (cw[e >> 1] >> ((e & 1) * 16)) & 0xFFu;          // channel 2e
+                    const uint32_t cb = (cw[e >> 1] >> ((e & 1) * 16 + 8)) & 0xFFu;      // channel 2e+1
+                    const uint32_t lo = (ca == (4u | q)) ? (pk[e] & 0xFFFFu) : 0u;
+                    const uint32_t hi = (cb == (4u | q)) ? (pk[e] & 0xFFFF0000u) : 0u;
+                    o[e] = lo | hi;
+                  }
+                  const size_t px = up_base + (size_t)(q >> 1) * a.up_W + (q & 1);
+                  *reinterpret_cast<uint4*>(a.out + px * a.co_total + c0) = make_uint4(o[0], o[1], o[2], o[3]);
+                }
               }
             }
           }
         }
       }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&tempty[tb]);
-      if (++tb == Cfg::NT) { tb = 0; tb_phase ^= 1; }
+      if (++buf == Cfg::NBUF) { buf = 0; phase ^= 1; }
     }
-  }
-done_roles:
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 9) {
-    tc_fence_after();
-    tmem_dealloc<Cfg::TMEM_COLS>(tmem_base);
   }
 }
 
@@ -445,7 +407,7 @@ static void launch_tap_gemm(const __nv_bfloat16* A, const __nv_bfloat16* Wt, Tap
   int gx = a.num_tiles < slots ? a.num_tiles : slots;
   if (gx < 1) gx = 1;
   dim3 grid(gx, ny);
-  launch_pdl(kern, grid, dim3(352), Cfg::SMEM, st, tmA, tmW, a);
+  launch_pdl(kern, grid, dim3(288), Cfg::SMEM, st, tmA, tmW, a);
   hefl::cuda::note_launch();
 }
 
@@ -513,7 +475,7 @@ void conv_dgrad(const void* dY, const void* Wd, void* dX, int B, int H, int W, i
 
 // ------------------------------------------------------------------------------------------
 // G1b (layer 1 by default, HEFL_FWD_PAIR=0 / all to change): forward + pool with both columns of a pooling window in
-// the SAME TMEM lane.
+// the SAME thread.
 // Validated against G1 on hardware (tests/test_gpu_conv.py::test_conv_fwd_pool_pair_matches_plain_kernel: same
 // pooled values and arg-max codes); 33.7 vs 40.4 us on layer 1 (B=32, 256x256), slower on the small layers.
 //
@@ -529,7 +491,7 @@ void conv_dgrad(const void* dY, const void* Wd, void* dX, int B, int H, int W, i
 // 32-byte K steps inside a swizzle atom). Four accumulators (2 rows x 2 column parities), M = 128 windows.
 // The epilogue thread of window j then holds all four values of its window: max/arg-max in registers, no
 // shuffles, every lane stores a full 16-byte pooled pixel chunk. Restricted to CK <= 32 (one swizzle atom per
-// pair-row) and CO <= 64 (4 accumulators x 2 TMEM buffers).
+// pair-row) and CO <= 64 (4 accumulators in registers).
 // ------------------------------------------------------------------------------------------
 template <int CK, int CO>
 struct PairFwdCfg {
@@ -542,16 +504,15 @@ struct PairFwdCfg {
   static constexpr int W_TAP = CO * W_ROW;
   static constexpr int W_BYTES = 9 * W_TAP;
   static constexpr int BAR_BYTES = 384;
+  static constexpr int SCR_BYTES = 8 * 1024;
   static constexpr int NBUF = 2;
-  static constexpr int SMEM = W_BYTES + NBUF * HALO + BAR_BYTES + 1024;
+  static constexpr int SMEM = W_BYTES + NBUF * HALO + SCR_BYTES + BAR_BYTES + 1024;
   static constexpr int NACC = 4;
-  static constexpr int NT = 2;
-  static constexpr int ACC_COLS = NT * NACC * CO;
-  static constexpr int TMEM_COLS = ACC_COLS <= 256 ? 256 : 512;
-  static constexpr int OCC = (2 * SMEM <= 226 * 1024 && 2 * TMEM_COLS <= 512) ? 2 : 1;
+  static constexpr int NG = 2;                            // 8-channel chunks per warp and pass
+  static constexpr int OCC = blocks_fit(SMEM, 2) ? 2 : 1;
   static_assert(CK == 16 || CK == 32, "pair-row forward: one swizzle atom per pair-row");
-  static_assert(CO == 32 || CO == 64, "pair-row forward: 4 accumulators x 2 buffers must fit TMEM");
-  static_assert(SMEM <= 226 * 1024, "shared memory");
+  static_assert(CO == 32 || CO == 64, "pair-row forward: CO is 32 or 64");
+  static_assert(SMEM <= kSmemMax, "shared memory");
 };
 
 struct PairFwdArgs {
@@ -565,38 +526,35 @@ struct PairFwdArgs {
 
 // SP: s-packed layer-1 input (channels = pixels x, x+1, x+2): the three horizontal taps are already inside the 16
 // channels, so only the three filter rows remain — 3 MMAs per accumulator, column parity = K byte offset.
+// Warp roles as in G1: warps 0..7 compute + epilogue (lane = window, quadrant = warp % 4, chunks by warp / 4),
+// warp 8 is the TMA producer.
 template <int CK, int CO, bool SP>
-__global__ void __launch_bounds__(352, PairFwdCfg<CK, CO>::OCC)
+__global__ void __launch_bounds__(288, PairFwdCfg<CK, CO>::OCC)
 pair_fwd_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmW,
                 const PairFwdArgs a) {
   using Cfg = PairFwdCfg<CK, CO>;
+  constexpr int RB = Cfg::ROW_BYTES;
+  constexpr int WB = Cfg::W_ROW;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* sW = smem;
   uint8_t* sA = smem + Cfg::W_BYTES;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(sA + Cfg::NBUF * Cfg::HALO);
+  float* scr_all = reinterpret_cast<float*>(sA + Cfg::NBUF * Cfg::HALO);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(reinterpret_cast<uint8_t*>(scr_all) + Cfg::SCR_BYTES);
   uint64_t* full = bars;
   uint64_t* empty = bars + Cfg::NBUF;
   uint64_t* wfull = bars + 2 * Cfg::NBUF;
-  uint64_t* tfull = wfull + 1;
-  uint64_t* tempty = tfull + Cfg::NT;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tempty + Cfg::NT);
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
 
   if (warp == 8 && lane == 0) {
     prefetch_tmap(&tmA);
     prefetch_tmap(&tmW);
-    for (int s = 0; s < Cfg::NBUF; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 2); }   // two MMA issuers
+    for (int s = 0; s < Cfg::NBUF; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 8); }
     mbar_init(wfull, 1);
-    for (int i = 0; i < Cfg::NT; ++i) { mbar_init(&tfull[i], 2); mbar_init(&tempty[i], 8); }
     fence_barrier_init();
   }
-  if (warp == 9) tmem_alloc<Cfg::TMEM_COLS>(tmem_slot);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
   pdl_trigger();
   if (warp == 8 && elect_one()) {
     constexpr int NTAPW = SP ? 3 : 9;
@@ -621,114 +579,117 @@ pair_fwd_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
         if (++buf == Cfg::NBUF) { buf = 0; phase ^= 1; }
       }
     }
-  } else if (warp == 9 || warp == 10) {
-    // ===== MMA issuers: warp 9 -> accumulators (dy=0, dx=0/1), warp 10 -> (dy=1, dx=0/1) =====
-    const int dy = warp - 9;
-    constexpr uint32_t idesc = make_idesc_bf16(128, CO);
-    mbar_wait(wfull, 0);
-    tc_fence_after();
-    int buf = 0, tb = 0;
-    uint32_t phase = 0, tb_phase = 0;
-    for (int t = blockIdx.x; t < a.num_tiles; t += gridDim.x) {
-      mbar_wait(&tempty[tb], tb_phase ^ 1);
-      mbar_wait(&full[buf], phase);
-      tc_fence_after();
-      if (elect_one()) {
-        const uint32_t a_lo = desc_lo(smem_u32(sA + buf * Cfg::HALO));
-        const uint32_t w_lo = desc_lo(smem_u32(sW));
-        constexpr uint32_t a_hi = desc_hi(8 * Cfg::ROW_BYTES, Cfg::ROW_BYTES);
-        constexpr uint32_t w_hi = desc_hi(8 * Cfg::W_ROW, Cfg::W_ROW);
-#pragma unroll
-        for (int dx = 0; dx < 2; ++dx) {
-          const uint32_t d_tmem = tmem_base + (tb * Cfg::NACC + dy * 2 + dx) * CO;
-          if constexpr (SP) {
-#pragma unroll
-            for (int r = 0; r < 3; ++r) {
-              const uint32_t ao = ((dy + r) * Cfg::SEG_BYTES + dx * CK * 2) >> 4;
-              const uint32_t wo = (r * Cfg::W_TAP) >> 4;
-              umma_bf16_lh(d_tmem, a_lo + ao, a_hi, w_lo + wo, w_hi, idesc, r != 0 ? 1u : 0u);
-            }
-            continue;
-          }
-#pragma unroll
-          for (int tap = 0; tap < 9; ++tap) {
-            const int r = tap / 3, s = tap % 3;
-            const int e = dx + s;
-#pragma unroll
-            for (int k = 0; k < CK / 16; ++k) {
-              const uint32_t ao = ((dy + r) * Cfg::SEG_BYTES + (e >> 1) * Cfg::ROW_BYTES + (e & 1) * CK * 2 + k * 32) >> 4;
-              const uint32_t wo = (tap * Cfg::W_TAP + k * 32) >> 4;
-              umma_bf16_lh(d_tmem, a_lo + ao, a_hi, w_lo + wo, w_hi, idesc, (tap | k) != 0 ? 1u : 0u);
-            }
-          }
-        }
-        umma_commit(&empty[buf]);
-        umma_commit(&tfull[tb]);
-      }
-      __syncwarp();
-      if (++buf == Cfg::NBUF) { buf = 0; phase ^= 1; }
-      if (++tb == Cfg::NT) { tb = 0; tb_phase ^= 1; }
-    }
   } else {
-    // ===== epilogue warps 0..7: lane = window (quadrant = warp % 4), channel chunks interleaved by warp / 4 =====
+    // ===== compute + epilogue warps 0..7; accumulator (dy, dx) = acc[dy * 2 + dx] =====
     const int qd = warp & 3;
     const int grp = warp >> 2;
-    const uint32_t lane_base = (uint32_t)(qd * 32) << 16;
     const int j = qd * 32 + lane;                          // window index in the pooled row
-    int tb = 0;
-    uint32_t tb_phase = 0;
+    float* scr = scr_all + warp * 256;
+    const uint32_t w_base = smem_u32(sW);
+    mbar_wait(wfull, 0);
+    int buf = 0;
+    uint32_t phase = 0;
     for (int t = blockIdx.x; t < a.num_tiles; t += gridDim.x) {
-      mbar_wait(&tfull[tb], tb_phase);
-      tc_fence_after();
+      mbar_wait(&full[buf], phase);
+      const uint32_t a_base = smem_u32(sA + buf * Cfg::HALO);
       const size_t row_out = (size_t)t * a.Wp;             // t = b * Hp + hp
 #pragma unroll 1
-      for (int ch = grp; ch < CO / 8; ch += 2) {
-        float v00[8], v01[8], v10[8], v11[8];
-        const uint32_t tcol = tmem_base + lane_base + tb * Cfg::NACC * CO + ch * 8;
-        tmem_ld8_nowait(tcol + 0 * CO, v00);
-        tmem_ld8_nowait(tcol + 1 * CO, v01);
-        tmem_ld8_nowait(tcol + 2 * CO, v10);
-        tmem_ld8_nowait(tcol + 3 * CO, v11);
-        const float4 bA = __ldg(reinterpret_cast<const float4*>(a.bias + ch * 8));
-        const float4 bB = __ldg(reinterpret_cast<const float4*>(a.bias + ch * 8 + 4));
-        const float bias8[8] = {bA.x, bA.y, bA.z, bA.w, bB.x, bB.y, bB.z, bB.w};
-        tmem_ld_wait();
-        uint32_t packed[4], idx[2] = {0u, 0u};
+      for (int g = 0; g < CO / 16 / Cfg::NG; ++g) {
+        const int c0 = grp + 2 * g * Cfg::NG;              // chunks c0 and c0 + 2
+        float acc[4][2][2][4];
 #pragma unroll
-        for (int c = 0; c < 8; c += 2) {
-          float x[2];
+        for (int x = 0; x < 4; ++x)
 #pragma unroll
-          for (int i = 0; i < 2; ++i) {
-            // same tie-breaking as G1: lower row wins only if strictly greater, then right column likewise
-            const bool l0 = v10[c + i] > v00[c + i];
-            const bool l1 = v11[c + i] > v01[c + i];
-            const float m0 = l0 ? v10[c + i] : v00[c + i];
-            const float m1 = l1 ? v11[c + i] : v01[c + i];
-            const bool rw = m1 > m0;
-            const uint32_t rowbit = (rw ? l1 : l0) ? 1u : 0u;
-            const float y = (rw ? m1 : m0) + bias8[c + i];
-            idx[(c + i) >> 2] |= ((rowbit << 1) | (rw ? 1u : 0u) | (y > 0.f ? 4u : 0u)) << (((c + i) & 3) * 8);
-            x[i] = y > 0.f ? y : 0.f;
+          for (int i = 0; i < 2; ++i)
+#pragma unroll
+            for (int mt = 0; mt < 2; ++mt)
+#pragma unroll
+              for (int q = 0; q < 4; ++q) acc[x][i][mt][q] = 0.f;
+        if constexpr (SP) {
+#pragma unroll
+          for (int r = 0; r < 3; ++r) {
+            uint32_t bf[4];
+            ld_b_kmajor<WB>(w_base + r * Cfg::W_TAP, c0 * 8, (c0 + 2) * 8, 0, lane, bf);
+#pragma unroll
+            for (int dy = 0; dy < 2; ++dy)
+#pragma unroll
+              for (int dx = 0; dx < 2; ++dx)
+#pragma unroll
+                for (int mt = 0; mt < 2; ++mt) {
+                  uint32_t af[4];
+                  ld_a_kmajor<RB>(a_base + (dy + r) * Cfg::SEG_BYTES, qd * 32 + mt * 16, dx * CK * 2, lane, af);
+                  mma_bf16(acc[dy * 2 + dx][0][mt], af, bf[0], bf[1]);
+                  mma_bf16(acc[dy * 2 + dx][1][mt], af, bf[2], bf[3]);
+                }
           }
-          packed[c >> 1] = pack_bf16x2(x[0], x[1]);
+        } else {
+#pragma unroll 1
+          for (int tap = 0; tap < 9; ++tap) {
+            const int r = tap / 3, s = tap % 3;
+#pragma unroll
+            for (int k = 0; k < CK / 16; ++k) {
+              uint32_t bf[4];
+              ld_b_kmajor<WB>(w_base + tap * Cfg::W_TAP, c0 * 8, (c0 + 2) * 8, k * 32, lane, bf);
+#pragma unroll
+              for (int dy = 0; dy < 2; ++dy)
+#pragma unroll
+                for (int dx = 0; dx < 2; ++dx) {
+                  const int e = dx + s;
+#pragma unroll
+                  for (int mt = 0; mt < 2; ++mt) {
+                    uint32_t af[4];
+                    ld_a_kmajor<RB>(a_base + (dy + r) * Cfg::SEG_BYTES, (e >> 1) + qd * 32 + mt * 16,
+                                    (e & 1) * CK * 2 + k * 32, lane, af);
+                    mma_bf16(acc[dy * 2 + dx][0][mt], af, bf[0], bf[1]);
+                    mma_bf16(acc[dy * 2 + dx][1][mt], af, bf[2], bf[3]);
+                  }
+                }
+            }
+          }
         }
-        if (j < a.Wp) {
-          const size_t o = (row_out + j) * CO + ch * 8;
-          *reinterpret_cast<uint4*>(a.out + o) = make_uint4(packed[0], packed[1], packed[2], packed[3]);
-          if (a.argmax) *reinterpret_cast<uint2*>(a.argmax + o) = make_uint2(idx[0], idx[1]);
+        if (g == CO / 16 / Cfg::NG - 1) {
+          __syncwarp();
+          if (lane == 0) mbar_arrive(&empty[buf]);
+        }
+#pragma unroll
+        for (int i = 0; i < 2; ++i) {
+          const int ch = c0 + 2 * i;
+          float v00[8], v01[8], v10[8], v11[8];
+          frag_rows(scr, acc[0][i][0], acc[0][i][1], lane, v00);
+          frag_rows(scr, acc[1][i][0], acc[1][i][1], lane, v01);
+          frag_rows(scr, acc[2][i][0], acc[2][i][1], lane, v10);
+          frag_rows(scr, acc[3][i][0], acc[3][i][1], lane, v11);
+          const float4 bA = __ldg(reinterpret_cast<const float4*>(a.bias + ch * 8));
+          const float4 bB = __ldg(reinterpret_cast<const float4*>(a.bias + ch * 8 + 4));
+          const float bias8[8] = {bA.x, bA.y, bA.z, bA.w, bB.x, bB.y, bB.z, bB.w};
+          uint32_t packed[4], idx[2] = {0u, 0u};
+#pragma unroll
+          for (int c = 0; c < 8; c += 2) {
+            float x[2];
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+              // same tie-breaking as G1: lower row wins only if strictly greater, then right column likewise
+              const bool l0 = v10[c + h] > v00[c + h];
+              const bool l1 = v11[c + h] > v01[c + h];
+              const float m0 = l0 ? v10[c + h] : v00[c + h];
+              const float m1 = l1 ? v11[c + h] : v01[c + h];
+              const bool rw = m1 > m0;
+              const uint32_t rowbit = (rw ? l1 : l0) ? 1u : 0u;
+              const float y = (rw ? m1 : m0) + bias8[c + h];
+              idx[(c + h) >> 2] |= ((rowbit << 1) | (rw ? 1u : 0u) | (y > 0.f ? 4u : 0u)) << (((c + h) & 3) * 8);
+              x[h] = y > 0.f ? y : 0.f;
+            }
+            packed[c >> 1] = pack_bf16x2(x[0], x[1]);
+          }
+          if (j < a.Wp) {
+            const size_t o = (row_out + j) * CO + ch * 8;
+            *reinterpret_cast<uint4*>(a.out + o) = make_uint4(packed[0], packed[1], packed[2], packed[3]);
+            if (a.argmax) *reinterpret_cast<uint2*>(a.argmax + o) = make_uint2(idx[0], idx[1]);
+          }
         }
       }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&tempty[tb]);
-      if (++tb == Cfg::NT) { tb = 0; tb_phase ^= 1; }
+      if (++buf == Cfg::NBUF) { buf = 0; phase ^= 1; }
     }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 9) {
-    tc_fence_after();
-    tmem_dealloc<Cfg::TMEM_COLS>(tmem_base);
   }
 }
 
@@ -742,7 +703,7 @@ static void launch_pair_fwd(const __nv_bfloat16* X, const __nv_bfloat16* Wt, Pai
   cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM);
   int gx = num_sms() * Cfg::OCC;
   if (gx > a.num_tiles) gx = a.num_tiles;
-  launch_pdl(kern, dim3(gx), dim3(352), Cfg::SMEM, st, tmA, tmW, a);
+  launch_pdl(kern, dim3(gx), dim3(288), Cfg::SMEM, st, tmA, tmW, a);
   hefl::cuda::note_launch();
 }
 
@@ -776,7 +737,7 @@ void conv_fwd_pool_pair(const void* X, const void* Wf, const float* bias, void* 
 // G2: weight-gradient kernel.
 //
 // dW[r,s][ci][co] = sum_m X[m + r*W + s][ci] * dY[m][co]. Both operands are consumed in their
-// native NHWC layout as MN-major UMMA operands (pixels = K), so no transposed copies exist.
+// native NHWC layout (ldmatrix.trans, pixels = K), so no transposed copies exist.
 // Work is organised by image rows: a CTA walks down a 64-column strip; at row h it needs the X
 // row segments h, h+1, h+2 (72 pixels each) and the dY chunk of row h. Segments live in a ring
 // of stages, so each X segment is fetched ONCE and serves filter rows r = 2, 1, 0 on three
@@ -785,10 +746,6 @@ void conv_fwd_pool_pair(const void* X, const void* Wf, const float* bias, void* 
 // Split over (image, strip, row range); fp32 vector-RED of the partial sums into a [9*C+1, Co]
 // buffer whose last row is the bias gradient (an all-ones A tile).
 // ------------------------------------------------------------------------------------------
-#ifndef HEFL_WGRAD_OCC3
-#define HEFL_WGRAD_OCC3 0     // 1: allow three wgrad CTAs per SM (validated build flag, see WgradCfg::OCC)
-#endif
-
 struct WgradArgs {
   int H, W, Ho;     // input grid height/width, valid output rows
   int strips;       // ceil((W-2) / 64)
@@ -796,8 +753,8 @@ struct WgradArgs {
   int rows_per;     // rows per range
   int units;        // B * strips * rsplit
   int nchunks;      // FLAT: ceil(B*H*W / 64)
-  int Co;           // total output channels (row pitch of dW32)
-  float* dW32;      // [9*CK + 1][Co] fp32, accumulated with vector RED
+  int Co;           // total output channels (row pitch of a partial)
+  float* ws;        // [gridDim.x][9*CK + 1][Co] fp32: the partial sums of CTA column x (plain stores)
 };
 
 // FLAT = small feature maps (W <= 32): a 64-pixel chunk of one image row would be mostly padding, so
@@ -805,18 +762,13 @@ struct WgradArgs {
 // three X segments (rows offset by W); no ring reuse, L2 traffic is irrelevant at these sizes.
 template <int CK, int COT, bool FLAT = false>
 struct WgradCfg {
-  // CK = 16 (layer 1): 32-byte MN-major atoms make the tensor core read shared memory 32 bytes at
-  // a time (measured ~128 cycles per MMA). Instead the X tensor map uses OVERLAPPING rows: row m is
-  // the 128 bytes starting at pixel m (4 pixels x 16 channels, row stride 32 B), so one 128-byte
-  // atom already holds the tap columns s = 0..3 and no pixel shift is needed.
+  // CK = 16 (layer 1): the X tensor map uses OVERLAPPING rows: row m is the 128 bytes starting at pixel m
+  // (4 pixels x 16 channels, row stride 32 B), so one 128-byte row already holds the tap columns s = 0..3 and
+  // no pixel shift is needed.
   static constexpr bool PACK4 = CK == 16;
-  static constexpr int ATOM_A = PACK4 ? 128 : CK * 2;          // bytes of one k-row of the A atom
+  static constexpr int ATOM_A = PACK4 ? 128 : CK * 2;          // bytes of one pixel row of the X tile
   static constexpr int ATOM_B = COT * 2;
-  static constexpr int TPG = PACK4 ? 4 : 128 / CK;             // tap columns covered by one MMA
-  static constexpr int MMA_PER_R = CK == 64 ? 2 : 1;           // s = {0,1},{2,3} for CK=64; one MMA otherwise
-  static constexpr int NACC = 3 * MMA_PER_R;
   static constexpr int XROWS = PACK4 ? 64 : 72;                // 64 + pixel shifts (none when packed)
-  static constexpr int A_LBO = PACK4 ? 0 : CK * 2;             // next atom = next pixel (packed: rows 64.. unused)
   static constexpr int X_BYTES = XROWS * ATOM_A;
   static constexpr int X_SEG = ((X_BYTES + 1023) / 1024) * 1024;
   static constexpr int DY_BYTES = 64 * ATOM_B;
@@ -824,60 +776,52 @@ struct WgradCfg {
   static constexpr int TX = (FLAT ? 3 : 1) * X_BYTES + DY_BYTES;
   static constexpr int STAGE_FULL = DY_OFF + ((DY_BYTES + 1023) / 1024) * 1024;
   static_assert(!(FLAT && PACK4), "layer 1 always uses the rolling-window path");
-  static constexpr int ONES_BYTES = 16 * 1024;                 // [128 x 64] bf16 of 1.0
   // deep ring: stages are small (one X row segment + one dY chunk), so the number of bytes in
-  // flight, not the MMA rate, bounds throughput (measured: 6 stages -> 204 us on layer 1)
-  static constexpr int NSTAGE_RAW = (200 * 1024 - ONES_BYTES) / STAGE_FULL;
+  // flight, not the MMA rate, bounds throughput
+  static constexpr int NSTAGE_RAW = (200 * 1024) / STAGE_FULL;
   static constexpr int NSTAGE = NSTAGE_RAW > 6 ? 6 : NSTAGE_RAW;
-  static constexpr int SMEM = NSTAGE * STAGE_FULL + ONES_BYTES + 512 + 1024;
-  static constexpr int COLS = (NACC + 1) * COT;                // + bias accumulator
+  static constexpr int SMEM = NSTAGE * STAGE_FULL + 512 + 1024;
   static_assert(NSTAGE >= 4, "ring needs 3 live stages + 1 in flight");
-  static constexpr int TMEM_COLS = COLS <= 32 ? 32 : (COLS <= 64 ? 64 : (COLS <= 128 ? 128 : (COLS <= 256 ? 256 : 512)));
-  static_assert(COLS <= 512, "accumulators exceed TMEM");
-  // CTAs per SM. ncu (prof_wgrad1): 22 % tensor-pipe active, 7 % issue active, occupancy limit 3 by shared memory
-  // while 2 were launched — the kernel is latency-bound, so take the third CTA when smem and TMEM allow it.
-  static constexpr int OCC = (HEFL_WGRAD_OCC3 && 3 * SMEM <= 226 * 1024 && 3 * TMEM_COLS <= 512) ? 3
-                             : ((2 * SMEM <= 226 * 1024 && 2 * TMEM_COLS <= 512) ? 2 : 1);
+  // m16 tiles of one filter row: (tap column s, 16 input channels); warp w owns tiles w and w + 8
+  static constexpr int MT = 3 * CK / 16;
+  static constexpr int NT = COT / 8;
+  static constexpr int OCC = blocks_fit(SMEM, 2) ? 2 : 1;
   static_assert(CK == 16 || CK == 32 || CK == 64, "CK must be one swizzle atom");
   static_assert(COT == 32 || COT == 64, "COT must be one swizzle atom");
 };
 
+// dW[r,s][ci][co] = sum_p X[p + s][ci] dY[p][co] for the filter row r = blockIdx.z over the pixels of CTA column
+// blockIdx.x, stored into that column's partial (reduce_partials adds the columns in a fixed order, so the gradient
+// is the same bits on every run): a CTA holds 3*CK x COT fp32 accumulators in the registers of its 8 compute warps (mma.sync m16n8k16, both operands read from their native
+// [pixel][channel] tiles with ldmatrix.trans: pixels are the K axis), warp 8 is the TMA producer. The bias
+// gradient (column sums of dY) is one more MMA per k-step with an all-ones A fragment, in the r = 0 CTAs.
 template <int CK, int COT, bool FLAT>
-__global__ void __launch_bounds__(192, WgradCfg<CK, COT, FLAT>::OCC)
+__global__ void __launch_bounds__(288, WgradCfg<CK, COT, FLAT>::OCC)
 wgrad_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ CUtensorMap tmDY,
              const WgradArgs a) {
   using Cfg = WgradCfg<CK, COT, FLAT>;
+  constexpr int SA = Cfg::ATOM_A, SB = Cfg::ATOM_B;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint8_t* ones = smem + Cfg::NSTAGE * Cfg::STAGE_FULL;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(ones + Cfg::ONES_BYTES);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + Cfg::NSTAGE * Cfg::STAGE_FULL);
   uint64_t* full = bars;
   uint64_t* empty = bars + Cfg::NSTAGE;
-  uint64_t* done = bars + 2 * Cfg::NSTAGE;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(done + 1);
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
   const int co0 = blockIdx.y * COT;
+  const int fr = blockIdx.z;                                    // filter row r
 
-  for (int i = threadIdx.x; i < Cfg::ONES_BYTES / 4; i += blockDim.x)
-    reinterpret_cast<uint32_t*>(ones)[i] = 0x3F803F80u;        // bf16 1.0 x2 (uniform => layout-agnostic)
-  if (warp == 4 && lane == 0) {
+  if (warp == 8 && lane == 0) {
     prefetch_tmap(&tmX);
     prefetch_tmap(&tmDY);
-    for (int s = 0; s < Cfg::NSTAGE; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 1); }
-    mbar_init(done, 1);
+    for (int s = 0; s < Cfg::NSTAGE; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 8); }
     fence_barrier_init();
   }
-  fence_proxy_async();   // generic-proxy writes (ones tile) visible to the tensor-core async proxy
-  if (warp == 5) tmem_alloc<Cfg::TMEM_COLS>(tmem_slot);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
   pdl_prologue();
   const int per_img = a.strips * a.rsplit;
 
-  if (warp == 4) {
+  if (warp == 8) {
     if (FLAT) {
       if (elect_one()) {
         int slot = 0;
@@ -911,137 +855,117 @@ wgrad_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ CU
         }
       }
     }
-  } else if (warp == 5) {
-    constexpr uint32_t idesc = make_idesc_bf16(128, COT, 1, 1);
-    constexpr uint32_t a_hi = desc_hi(8 * Cfg::ATOM_A, Cfg::ATOM_A);
-    constexpr uint32_t b_hi = desc_hi(8 * Cfg::ATOM_B, Cfg::ATOM_B);
-    constexpr uint32_t o_hi = desc_hi(8 * 128, 128);
-    const uint32_t smem_lo = desc_lo(smem_u32(smem));                 // stage 0, as a descriptor low word
-    const uint32_t ones_lo = desc_lo(smem_u32(ones), 64 * 128);
-    constexpr uint32_t a_lbo = (uint32_t)(Cfg::A_LBO >> 4) << 16;
-    constexpr uint32_t b_lbo = (uint32_t)(Cfg::DY_BYTES >> 4) << 16;
-    constexpr uint32_t stage16 = Cfg::STAGE_FULL >> 4;
-    int slot = 0;                                                     // ring position of the current stage
-    uint32_t phase = 0;
-    uint32_t first = 1;
-    if (FLAT) {
-      for (int c = blockIdx.x; c < a.nchunks; c += gridDim.x) {
-        mbar_wait(&full[slot], phase);
-        tc_fence_after();
-        if (elect_one()) {
-          const uint32_t st_lo = smem_lo + slot * stage16;
-          const uint32_t dy_lo = st_lo + (Cfg::DY_OFF >> 4) + b_lbo;
+    return;
+  }
+
+  // ===== compute warps 0..7
+  float acc[2][Cfg::NT][4];
+  float bacc[4] = {0.f, 0.f, 0.f, 0.f};
 #pragma unroll
-          for (int k = 0; k < 4; ++k) {
-            const uint32_t blo = dy_lo + ((k * 16 * Cfg::ATOM_B) >> 4);
-            const uint32_t accum = k == 0 ? (first ^ 1u) : 1u;
+  for (int u = 0; u < 2; ++u)
 #pragma unroll
-            for (int r = 0; r < 3; ++r) {
+    for (int n = 0; n < Cfg::NT; ++n)
 #pragma unroll
-              for (int mm = 0; mm < Cfg::MMA_PER_R; ++mm)
-                umma_bf16_lh(tmem_base + (r * Cfg::MMA_PER_R + mm) * COT,
-                             st_lo + a_lbo + ((r * Cfg::X_SEG + (mm * Cfg::TPG + k * 16) * Cfg::ATOM_A) >> 4), a_hi,
-                             blo, b_hi, idesc, accum);
-            }
-            umma_bf16_lh(tmem_base + Cfg::NACC * COT, ones_lo + ((k * 16 * 128) >> 4), o_hi, blo, b_hi, idesc, accum);
-          }
-          umma_commit(&empty[slot]);
-        }
-        __syncwarp();
-        first = 0;
-        if (++slot == Cfg::NSTAGE) { slot = 0; phase ^= 1; }
+      for (int q = 0; q < 4; ++q) acc[u][n][q] = 0.f;
+  constexpr uint32_t kOnes = 0x3F803F80u;                       // bf16 1.0 x2
+  const uint32_t ones[4] = {kOnes, kOnes, kOnes, kOnes};
+  const int bias_nt = warp % Cfg::NT;
+  // per-lane parts of the ldmatrix.trans addresses: matrix i = lane / 8 covers (M or N block i & 1 or i >> 1)
+  const int lrow = lane & 7;
+  const int ia = lane >> 3;
+  uint32_t a_off[2];                                            // byte offset of my A rows for tiles w, w + 8
+  int a_shift[2];
+#pragma unroll
+  for (int u = 0; u < 2; ++u) {
+    const int tile = warp + 8 * u;
+    const int s = tile / (CK / 16), ci0 = (tile % (CK / 16)) * 16;
+    a_shift[u] = Cfg::PACK4 ? 0 : s;
+    a_off[u] = (uint32_t)((Cfg::PACK4 ? s * CK + ci0 : ci0) * 2 + (ia & 1) * 16);
+  }
+  const uint32_t smem0 = smem_u32(smem);
+
+  auto step = [&](uint32_t x_tile, uint32_t dy_tile) {
+#pragma unroll
+    for (int kk = 0; kk < 4; ++kk) {                            // 4 x 16 pixels per 64-pixel chunk
+      uint32_t bf[Cfg::NT / 2][4];
+#pragma unroll
+      for (int n = 0; n < Cfg::NT; n += 2)
+        ldsm_x4_t(swz<SB>(dy_tile + (uint32_t)((kk * 16 + (ia & 1) * 8 + lrow) * SB + (n + (ia >> 1)) * 16)), bf[n / 2]);
+#pragma unroll
+      for (int u = 0; u < 2; ++u) {
+        if (warp + 8 * u >= Cfg::MT) break;
+        uint32_t af[4];
+        ldsm_x4_t(swz<SA>(x_tile + (uint32_t)((kk * 16 + (ia >> 1) * 8 + lrow + a_shift[u]) * SA) + a_off[u]), af);
+#pragma unroll
+        for (int n = 0; n < Cfg::NT; ++n) mma_bf16(acc[u][n], af, bf[n / 2][(n & 1) * 2], bf[n / 2][(n & 1) * 2 + 1]);
+      }
+      if (fr == 0) {
+#pragma unroll
+        for (int n = 0; n < Cfg::NT; ++n)
+          if (n == bias_nt) mma_bf16(bacc, ones, bf[n / 2][(n & 1) * 2], bf[n / 2][(n & 1) * 2 + 1]);
       }
     }
-    for (int u = FLAT ? a.units : (int)blockIdx.x; u < a.units; u += gridDim.x) {
-      const int b = u / per_img;
-      const int rem = u - b * per_img;
+  };
+
+  int slot = 0;
+  uint32_t phase = 0;
+  if (FLAT) {
+    for (int c = blockIdx.x; c < a.nchunks; c += gridDim.x) {
+      mbar_wait(&full[slot], phase);
+      const uint32_t st = smem0 + slot * Cfg::STAGE_FULL;
+      step(st + fr * Cfg::X_SEG, st + Cfg::DY_OFF);
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&empty[slot]);
+      if (++slot == Cfg::NSTAGE) { slot = 0; phase ^= 1; }
+    }
+  } else {
+    for (int u = blockIdx.x; u < a.units; u += gridDim.x) {
+      const int rem = u % per_img;
       const int strip = rem / a.rsplit;
       const int h0 = (rem - strip * a.rsplit) * a.rows_per;
       const int h1 = min(a.Ho, h0 + a.rows_per);
       if (h0 >= h1) continue;
-      (void)b;
       for (int i = h0 - 2; i < h1; ++i) {
         mbar_wait(&full[slot], phase);
-        tc_fence_after();
         const int s1 = slot == 0 ? Cfg::NSTAGE - 1 : slot - 1;       // stage of X row h+1
         const int s0 = s1 == 0 ? Cfg::NSTAGE - 1 : s1 - 1;           // stage of X row h
-        if (i >= h0 && elect_one()) {
-          const uint32_t x_lo[3] = {smem_lo + s0 * stage16 + a_lbo, smem_lo + s1 * stage16 + a_lbo,
-                                    smem_lo + slot * stage16 + a_lbo};
-          const uint32_t dy_lo = smem_lo + slot * stage16 + (Cfg::DY_OFF >> 4) + b_lbo;
-#pragma unroll
-          for (int k = 0; k < 4; ++k) {                        // 4 x UMMA_K(16) pixels per 64-pixel chunk
-            const uint32_t blo = dy_lo + ((k * 16 * Cfg::ATOM_B) >> 4);
-            const uint32_t accum = k == 0 ? (first ^ 1u) : 1u;
-#pragma unroll
-            for (int r = 0; r < 3; ++r) {
-#pragma unroll
-              for (int mm = 0; mm < Cfg::MMA_PER_R; ++mm)
-                umma_bf16_lh(tmem_base + (r * Cfg::MMA_PER_R + mm) * COT,
-                             x_lo[r] + (((mm * Cfg::TPG + k * 16) * Cfg::ATOM_A) >> 4), a_hi, blo, b_hi, idesc, accum);
-            }
-            umma_bf16_lh(tmem_base + Cfg::NACC * COT, ones_lo + ((k * 16 * 128) >> 4), o_hi, blo, b_hi, idesc, accum);
-          }
-          umma_commit(&empty[s0]);                              // stage of X row h is done
+        if (i >= h0) {
+          const int sx = fr == 0 ? s0 : (fr == 1 ? s1 : slot);
+          step(smem0 + sx * Cfg::STAGE_FULL, smem0 + slot * Cfg::STAGE_FULL + Cfg::DY_OFF);
+          __syncwarp();
+          if (lane == 0) mbar_arrive(&empty[s0]);                    // stage of X row h is done
         }
-        __syncwarp();
-        if (i >= h0) first = 0;
         if (++slot == Cfg::NSTAGE) { slot = 0; phase ^= 1; }
       }
-      if (elect_one()) {                                        // release the last two stages of the unit
+      __syncwarp();
+      if (lane == 0) {                                               // release the last two stages of the unit
         const int l1 = slot == 0 ? Cfg::NSTAGE - 1 : slot - 1;
         const int l0 = l1 == 0 ? Cfg::NSTAGE - 1 : l1 - 1;
-        umma_commit(&empty[l0]);
-        umma_commit(&empty[l1]);
+        mbar_arrive(&empty[l0]);
+        mbar_arrive(&empty[l1]);
       }
-      __syncwarp();
     }
-    if (elect_one()) umma_commit(done);
-    __syncwarp();
-    mbar_wait(done, 0);                 // this warp is idle now: it waits for the tensor core ...
-    named_barrier_arrive(2, 160);       // ... and releases the epilogue warps, which block in hardware
-  } else {
-    const int qd = warp;
-    const uint32_t lane_base = (uint32_t)(qd * 32) << 16;
-    named_barrier_sync(2, 160);         // no polling while the main loop runs
-    if ((int)blockIdx.x < (FLAT ? a.nchunks : a.units)) {
-      tc_fence_after();
-      const int row = qd * 32 + lane;                          // row inside an accumulator: s_local*CK + ci
-#pragma unroll 1
-      for (int acc = 0; acc <= Cfg::NACC; ++acc) {
-        int R;                                                 // dW32 row: (r*3+s)*CK + ci, or 9*CK = bias
-        bool valid;
-        if (acc == Cfg::NACC) {
-          R = 9 * CK;
-          valid = row == 0;
-        } else {
-          const int r = acc / Cfg::MMA_PER_R, mm = acc % Cfg::MMA_PER_R;
-          const int s = mm * Cfg::TPG + row / CK;
-          R = (r * 3 + s) * CK + row % CK;
-          valid = s < 3 && (!Cfg::PACK4 || row < 64);
-        }
-#pragma unroll 1
-        for (int ch = 0; ch < COT / 32; ++ch) {
-          float v[32];
-          tmem_ld32(tmem_base + lane_base + acc * COT + ch * 32, v);
-          if (valid) {
-            float* dst = a.dW32 + (size_t)R * a.Co + co0 + ch * 32;
+  }
+  // every CTA writes its whole share of the partial (zeros when it had no work), so the partial is fully defined
+  float* part = a.ws + (size_t)blockIdx.x * (9 * CK + 1) * a.Co;
+  // fragment element q of (m16 tile, n8 tile): row ci0 + lane/4 (+8 for q >= 2), column 2*(lane%4) + (q & 1)
 #pragma unroll
-            for (int c = 0; c < 32; c += 4)
-              asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(dst + c), "f"(v[c]), "f"(v[c + 1]),
-                           "f"(v[c + 2]), "f"(v[c + 3])
-                           : "memory");
-          }
-        }
-      }
+  for (int u = 0; u < 2; ++u) {
+    const int tile = warp + 8 * u;
+    if (tile >= Cfg::MT) break;
+    const int s = tile / (CK / 16), ci0 = (tile % (CK / 16)) * 16;
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int R = (fr * 3 + s) * CK + ci0 + (lane >> 2) + 8 * h;   // dW32 row: (r*3+s)*CK + ci
+      float* dst = part + (size_t)R * a.Co + co0 + 2 * (lane & 3);
+#pragma unroll
+      for (int n = 0; n < Cfg::NT; ++n)
+        *reinterpret_cast<float2*>(dst + n * 8) = make_float2(acc[u][n][2 * h], acc[u][n][2 * h + 1]);
     }
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 5) {
-    tc_fence_after();
-    tmem_dealloc<Cfg::TMEM_COLS>(tmem_base);
-  }
+  if (fr == 0 && warp < Cfg::NT && lane < 4)                        // bias: row 0 of the all-ones product
+    *reinterpret_cast<float2*>(part + (size_t)(9 * CK) * a.Co + co0 + bias_nt * 8 + 2 * lane) =
+        make_float2(bacc[0], bacc[1]);
 }
 
 // 3-D bf16 tensor [rows][W][C] (C contiguous); box = {box_c, box_w, 1}.
@@ -1079,10 +1003,27 @@ static CUtensorMap make_map_3d_strided(const void* ptr, uint64_t C, uint64_t W, 
 }
 
 template <int CK, int COT, bool FLAT>
-static void launch_wgrad(const __nv_bfloat16* X, const __nv_bfloat16* DY, int B, int H, int W, int Co, float* dW32,
-                         cudaStream_t st) {
+struct WgradKind {
+  static constexpr int kCK = CK, kCOT = COT;
+  static constexpr bool kFLAT = FLAT;
+};
+
+// Calls f(WgradKind<...>{}) for the kernel configuration that serves (W, CK, Co).
+template <class F>
+static auto wgrad_dispatch(int W, int CK, int Co, F&& f) {
+  const bool flat = W <= 32 && CK != 16;
+  if (CK == 16 && Co == 32) return f(WgradKind<16, 32, false>{});
+  if (CK == 32 && Co == 32) return flat ? f(WgradKind<32, 32, true>{}) : f(WgradKind<32, 32, false>{});
+  if (CK == 32 && Co == 64) return flat ? f(WgradKind<32, 64, true>{}) : f(WgradKind<32, 64, false>{});
+  if (CK == 64 && (Co == 64 || Co == 128)) return flat ? f(WgradKind<64, 64, true>{}) : f(WgradKind<64, 64, false>{});
+  throw std::runtime_error("conv_wgrad: unsupported (CK, Co)");
+}
+
+// Work split of one weight-gradient launch; returns the number of CTA columns (= partials).
+template <int CK, int COT, bool FLAT>
+static int wgrad_plan(int B, int H, int W, int Co, WgradArgs& a) {
   using Cfg = WgradCfg<CK, COT, FLAT>;
-  WgradArgs a{};
+  a = WgradArgs{};
   a.H = H; a.W = W; a.Ho = H - 2;
   a.strips = (W - 2 + 63) / 64;
   const int cot = Co / COT;
@@ -1090,51 +1031,77 @@ static void launch_wgrad(const __nv_bfloat16* X, const __nv_bfloat16* DY, int B,
   a.rows_per = a.Ho < 16 ? a.Ho : 16;
   a.rsplit = (a.Ho + a.rows_per - 1) / a.rows_per;
   a.units = B * a.strips * a.rsplit;
-  const int P = B * H * W;
-  a.nchunks = (P + 63) / 64;
+  a.nchunks = (B * H * W + 63) / 64;
   a.Co = Co;
-  a.dW32 = dW32;
-  CUtensorMap tmX, tmD;
-  int total_steps;
-  if (FLAT) {
-    tmX = make_map(X, CK, (uint64_t)P, (uint64_t)CK * 2, CK, Cfg::XROWS);
-    tmD = make_map(DY, Co, (uint64_t)P, (uint64_t)Co * 2, COT, 64);
-    total_steps = a.nchunks;
-  } else {
-    tmX = Cfg::PACK4 ? make_map_3d_strided(X, 64, W, (uint64_t)B * H, 32, (uint64_t)W * 32, 64, Cfg::XROWS)
-                     : make_map_3d(X, CK, W, (uint64_t)B * H, CK, Cfg::XROWS);
-    tmD = make_map_3d(DY, Co, W, (uint64_t)B * H, COT, 64);
-    total_steps = a.units * (a.rows_per + 2);
-  }
-  auto kern = wgrad_kernel<CK, COT, FLAT>;
-  cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM);
-  // every CTA pays a fixed epilogue (fp32 RED of all accumulators): give each at least a few steps
+  const int total_steps = FLAT ? a.nchunks : a.units * (a.rows_per + 2);
+  // every CTA pays a fixed epilogue (a store of all accumulators): give each at least a few steps
   int gx = total_steps / (FLAT ? 6 : 24);
-  if (gx > num_sms() * Cfg::OCC / cot) gx = num_sms() * Cfg::OCC / cot;
+  if (gx > num_sms() * Cfg::OCC / (3 * cot)) gx = num_sms() * Cfg::OCC / (3 * cot);
   if (gx > (FLAT ? a.nchunks : a.units)) gx = FLAT ? a.nchunks : a.units;
   if (gx < 1) gx = 1;
-  dim3 grid(gx, cot);
-  launch_pdl(kern, grid, dim3(192), Cfg::SMEM, st, tmX, tmD, a);
+  return gx;
+}
+
+// dst[i] += the sum of the partials ws[p * n + i] over p, in a fixed order (sum_partials).
+__global__ void __launch_bounds__(256) reduce_partials_kernel(const float* __restrict__ ws, int parts, int64_t n,
+                                                              float* __restrict__ dst) {
+  __shared__ float red[256];
+  const float s = sum_partials(ws, parts, n, red);
+  const int64_t i = (int64_t)blockIdx.x * 32 + threadIdx.x;
+  if (threadIdx.x < 32 && i < n) dst[i] += s;
+}
+
+void reduce_partials(const float* ws, int parts, int64_t n, float* dst, cudaStream_t st) {
+  reduce_partials_kernel<<<(unsigned)((n + 31) / 32), 256, 0, st>>>(ws, parts, n, dst);
   hefl::cuda::note_launch();
 }
 
-void conv_wgrad(const void* X, const void* DY, float* dW32, int B, int H, int W, int CK, int Co, cudaStream_t st) {
-  const auto* x = reinterpret_cast<const __nv_bfloat16*>(X);
-  const auto* d = reinterpret_cast<const __nv_bfloat16*>(DY);
-  const bool flat = W <= 32 && CK != 16;
-  if (CK == 16 && Co == 32) launch_wgrad<16, 32, false>(x, d, B, H, W, Co, dW32, st);
-  else if (CK == 32 && Co == 32) flat ? launch_wgrad<32, 32, true>(x, d, B, H, W, Co, dW32, st) : launch_wgrad<32, 32, false>(x, d, B, H, W, Co, dW32, st);
-  else if (CK == 32 && Co == 64) flat ? launch_wgrad<32, 64, true>(x, d, B, H, W, Co, dW32, st) : launch_wgrad<32, 64, false>(x, d, B, H, W, Co, dW32, st);
-  else if (CK == 64 && (Co == 64 || Co == 128)) flat ? launch_wgrad<64, 64, true>(x, d, B, H, W, Co, dW32, st) : launch_wgrad<64, 64, false>(x, d, B, H, W, Co, dW32, st);
-  else throw std::runtime_error("conv_wgrad: unsupported (CK, Co)");
+int64_t conv_wgrad_ws_floats(int B, int H, int W, int CK, int Co) {
+  return wgrad_dispatch(W, CK, Co, [&](auto k) -> int64_t {
+    using K = decltype(k);
+    WgradArgs a;
+    return (int64_t)wgrad_plan<K::kCK, K::kCOT, K::kFLAT>(B, H, W, Co, a) * (9 * CK + 1) * Co;
+  });
+}
+
+void conv_wgrad(const void* X, const void* DY, float* dW32, float* ws, int B, int H, int W, int CK, int Co,
+                cudaStream_t st) {
+  wgrad_dispatch(W, CK, Co, [&](auto k) {
+    using K = decltype(k);
+    constexpr int CKc = K::kCK, COT = K::kCOT;
+    constexpr bool FLAT = K::kFLAT;
+    using Cfg = WgradCfg<CKc, COT, FLAT>;
+    const auto* x = reinterpret_cast<const __nv_bfloat16*>(X);
+    const auto* d = reinterpret_cast<const __nv_bfloat16*>(DY);
+    WgradArgs a;
+    const int gx = wgrad_plan<CKc, COT, FLAT>(B, H, W, Co, a);
+    a.ws = ws;
+    const int P = B * H * W;
+    CUtensorMap tmX, tmD;
+    if (FLAT) {
+      tmX = make_map(x, CKc, (uint64_t)P, (uint64_t)CKc * 2, CKc, Cfg::XROWS);
+      tmD = make_map(d, Co, (uint64_t)P, (uint64_t)Co * 2, COT, 64);
+    } else {
+      tmX = Cfg::PACK4 ? make_map_3d_strided(x, 64, W, (uint64_t)B * H, 32, (uint64_t)W * 32, 64, Cfg::XROWS)
+                       : make_map_3d(x, CKc, W, (uint64_t)B * H, CKc, Cfg::XROWS);
+      tmD = make_map_3d(d, Co, W, (uint64_t)B * H, COT, 64);
+    }
+    auto kern = wgrad_kernel<CKc, COT, FLAT>;
+    cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM);
+    dim3 grid(gx, Co / COT, 3);                              // z = filter row
+    launch_pdl(kern, grid, dim3(288), Cfg::SMEM, st, tmX, tmD, a);
+    hefl::cuda::note_launch();
+    // a plain launch: starts only when every partial is written
+    reduce_partials(ws, gx, (int64_t)(9 * CKc + 1) * Co, dW32, st);
+  });
 }
 
 }  // namespace nn
 }  // namespace hefl
 
 // ------------------------------------------------------------------------------------------
-// Probe: can a K-major swizzled A tile be consumed starting at an arbitrary ROW offset (with the
-// descriptor's base_offset field carrying the swizzle phase)? Used to validate halo-tile reuse.
+// Probe: can a K-major swizzled A tile be consumed starting at an arbitrary ROW offset? out[128, 32] =
+// A[shift_rows .. shift_rows + 127, :] . B^T, read from one TMA tile. Used to validate halo-tile reuse.
 // ------------------------------------------------------------------------------------------
 namespace hefl {
 namespace nn {
@@ -1143,60 +1110,58 @@ using namespace hefl::tc;
 template <int CK>
 __global__ void __launch_bounds__(128, 1)
 umma_shift_probe_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-                        float* out, int shift_rows, int mode) {
+                        float* out, int shift_rows) {
   constexpr int RB = CK * 2;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* sA = smem;                      // 144 rows
   uint8_t* sB = smem + 144 * 128;          // 32 rows
   uint64_t* bar = reinterpret_cast<uint64_t*>(sB + 32 * 128);
-  uint64_t* done = bar + 1;
-  uint32_t* slot = reinterpret_cast<uint32_t*>(done + 1);
+  float* scr = reinterpret_cast<float*>(bar + 2);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  if (threadIdx.x == 0) { mbar_init(bar, 1); mbar_init(done, 1); fence_barrier_init(); }
-  if (warp == 0) tmem_alloc<32>(slot);
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = *slot;
   if (threadIdx.x == 0) {
+    mbar_init(bar, 1);
+    fence_barrier_init();
     mbar_expect_tx(bar, 144 * RB + 32 * RB);
     tma_load_2d(sA, &tmA, 0, 0, bar);
     tma_load_2d(sB, &tmB, 0, 0, bar);
-    mbar_wait(bar, 0);
-    tc_fence_after();
-    const uint32_t a0 = smem_u32(sA) + shift_rows * RB;
-    for (int k = 0; k < CK / 16; ++k) {
-      uint64_t ad = make_kmajor_desc(a0 + k * 32, RB);
-      if (mode == 1) ad |= (uint64_t)((a0 >> 7) & 7) << 49;   // base_offset = row phase in the 1024-B pattern
-      const uint64_t bd = make_kmajor_desc(smem_u32(sB) + k * 32, RB);
-      umma_bf16(tmem, ad, bd, make_idesc_bf16(128, 32), k ? 1u : 0u);
-    }
-    umma_commit(done);
   }
-  mbar_wait(done, 0);
-  tc_fence_after();
-  float v[32];
-  tmem_ld32(tmem + ((uint32_t)(warp * 32) << 16), v);
-  for (int c = 0; c < 32; ++c) out[(warp * 32 + lane) * 32 + c] = v[c];
-  tc_fence_before();
   __syncthreads();
-  if (warp == 0) { tc_fence_after(); tmem_dealloc<32>(tmem); }
+  mbar_wait(bar, 0);
+  float acc[4][2][4] = {};
+  for (int k = 0; k < CK / 16; ++k) {
+    uint32_t b01[4], b23[4];
+    ld_b_kmajor<RB>(smem_u32(sB), 0, 8, k * 32, lane, b01);
+    ld_b_kmajor<RB>(smem_u32(sB), 16, 24, k * 32, lane, b23);
+    for (int mt = 0; mt < 2; ++mt) {
+      uint32_t af[4];
+      ld_a_kmajor<RB>(smem_u32(sA), shift_rows + warp * 32 + mt * 16, k * 32, lane, af);
+      mma_bf16(acc[0][mt], af, b01[0], b01[1]);
+      mma_bf16(acc[1][mt], af, b01[2], b01[3]);
+      mma_bf16(acc[2][mt], af, b23[0], b23[1]);
+      mma_bf16(acc[3][mt], af, b23[2], b23[3]);
+    }
+  }
+  for (int n = 0; n < 4; ++n) {
+    float v[8];
+    frag_rows(scr + warp * 256, acc[n][0], acc[n][1], lane, v);
+    for (int c = 0; c < 8; ++c) out[(warp * 32 + lane) * 32 + n * 8 + c] = v[c];
+  }
 }
 
-void umma_shift_probe(const void* A, const void* Bm, float* out, int CK, int shift_rows, int mode, cudaStream_t st) {
+void umma_shift_probe(const void* A, const void* Bm, float* out, int CK, int shift_rows, cudaStream_t st) {
   const CUtensorMap tmA = make_map(A, CK, 144, (uint64_t)CK * 2, CK, 144);
   const CUtensorMap tmB = make_map(Bm, CK, 32, (uint64_t)CK * 2, CK, 32);
-  const int smem = 144 * 128 + 32 * 128 + 64 + 1024;
+  const int smem = 144 * 128 + 32 * 128 + 16 + 4 * 1024 + 1024;
   if (CK == 64) {
     cudaFuncSetAttribute(umma_shift_probe_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
-    umma_shift_probe_kernel<64><<<1, 128, smem, st>>>(tmA, tmB, out, shift_rows, mode);
+    umma_shift_probe_kernel<64><<<1, 128, smem, st>>>(tmA, tmB, out, shift_rows);
   } else if (CK == 32) {
     cudaFuncSetAttribute(umma_shift_probe_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
-    umma_shift_probe_kernel<32><<<1, 128, smem, st>>>(tmA, tmB, out, shift_rows, mode);
+    umma_shift_probe_kernel<32><<<1, 128, smem, st>>>(tmA, tmB, out, shift_rows);
   } else {
     cudaFuncSetAttribute(umma_shift_probe_kernel<16>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
-    umma_shift_probe_kernel<16><<<1, 128, smem, st>>>(tmA, tmB, out, shift_rows, mode);
+    umma_shift_probe_kernel<16><<<1, 128, smem, st>>>(tmA, tmB, out, shift_rows);
   }
 }
 

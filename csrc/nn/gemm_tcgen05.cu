@@ -1,20 +1,18 @@
-// General tcgen05 / TMEM / TMA GEMM kernels for the ResNet convolutions (SURVEY.md K13-K15; BASELINE.json
-// configs[2], [4]). On NHWC activations
+// TMA-fed tensor-core GEMM kernels for the ResNet convolutions (SURVEY.md K13-K15; BASELINE.json configs[2], [4]).
+// On NHWC activations
 //
 //   * a 1x1 convolution is the GEMM  Y[pixels, Co] = X[pixels, Ci] . W[Co, Ci]^T,
-//   * a 3x3 / pad-1 / stride-1 convolution is NINE such GEMMs accumulated in TMEM: tap (r, s) multiplies the same
+//   * a 3x3 / pad-1 / stride-1 convolution is NINE such GEMMs accumulated in one tile: tap (r, s) multiplies the same
 //     activation matrix shifted by (r-1)*Wp + (s-1) rows, when the activations live on a zero-padded
 //     (H+2) x (W+2) grid -- the shift is just the row coordinate of the TMA copy (no im2col),
 //   * dgrad is the same kernel with the transposed / flipped filter,
 //   * wgrad is  dW[tap][Co, Ci] = sum_pixels dY[p, Co] . X[p + shift(tap), Ci]: both operands are consumed as
-//     stored (MN-major UMMA descriptors, the pixel axis is K), split over pixel ranges, fp32 vector RED.
+//     stored (ldmatrix.trans, the pixel axis is K), split over pixel ranges, fp32 vector RED.
 //
-// kmajor_gemm_kernel : C[M, N] = sum_taps A[M + shift_t, K] . B_t[N, K]^T, bf16 (kind::f16) or e4m3 (kind::f8f6f4,
-//                      per-tensor scales folded into the epilogue), fp32 accumulation in TMEM, bf16 out.
-//                      Warp-specialised and persistent: 1 TMA producer warp, 1 MMA-issuing warp, 4 epilogue warps;
-//                      5-stage smem ring (128 B swizzle), two TMEM accumulator buffers so the epilogue of tile i
-//                      overlaps the main loop of tile i+1.
-// wgrad_mn_kernel    : up to three taps (one filter row) per CTA share the dY stage.
+// kmajor_gemm_kernel : C[M, N] = sum_taps A[M + shift_t, K] . B_t[N, K]^T, bf16 or e4m3 (per-tensor scales folded
+//                      into the epilogue), fp32 accumulation in registers (asynchronous wgmma), bf16 out. Warp-specialised
+//                      and persistent: 1 TMA producer warp, 2 consumer warpgroups; 6/7-stage smem ring (128 B swizzle).
+// wgrad_mn_kernel    : one tap per unit, split over pixel ranges.
 #include <cuda.h>
 #include <cuda_bf16.h>
 
@@ -78,22 +76,6 @@ int sm_count() {
   return n;
 }
 
-// e4m3 x e4m3 -> fp32 (kind::f8f6f4): same descriptor layout as kind::f16 with a/b format 0 (E4M3)
-__host__ __device__ constexpr uint32_t make_idesc_e4m3(int M, int N) {
-  return (1u << 4) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
-}
-__device__ __forceinline__ void umma_f8_lh(uint32_t tmem_d, uint32_t alo, uint32_t ahi, uint32_t blo, uint32_t bhi,
-                                           uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t.reg .b64 da, db;\n\t"
-      "mov.b64 da, {%1, %2};\n\t"
-      "mov.b64 db, {%3, %4};\n\t"
-      "setp.ne.b32 p, %6, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f8f6f4 [%0], da, db, %5, p;\n\t}"
-      ::"r"(tmem_d), "r"(alo), "r"(ahi), "r"(blo), "r"(bhi), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-
 // ------------------------------------------------------------------------------------------------------------
 // K-major GEMM with row-shifted taps
 // ------------------------------------------------------------------------------------------------------------
@@ -112,18 +94,62 @@ struct GemmArgs {
   const float* scale_b;
 };
 
+// ---- warpgroup MMA (sm_90a wgmma) ---------------------------------------------------------------------------------
+// Shared-memory matrix descriptor of a K-major tile written by TMA with 128-byte swizzle: 8-row core-matrix groups
+// 1024 bytes apart (SBO), LBO unused (1), layout type 1 = 128B swizzle. Advancing K by 32 bytes inside the swizzle
+// atom is +2 on the start-address field.
+__device__ __forceinline__ uint64_t gmma_desc_sw128(uint32_t smem_addr) {
+  return (uint64_t)((smem_addr & 0x3FFFFu) >> 4) | (1ull << 16) | ((uint64_t)(1024 >> 4) << 32) | (1ull << 62);
+}
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// D[64 x N] (fp32, registers of the warpgroup) += A[64 x K] . B[N x K]^T, both K-major in shared memory
+__device__ __forceinline__ void wgmma_n128_bf16(float (&d)[64], uint64_t da, uint64_t db) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(da), "l"(db));
+}
+__device__ __forceinline__ void wgmma_n64_bf16(float (&d)[32], uint64_t da, uint64_t db) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "l"(da), "l"(db));
+}
+__device__ __forceinline__ void wgmma_n128_e4m3(float (&d)[64], uint64_t da, uint64_t db) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k32.f32.e4m3.e4m3 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(da), "l"(db));
+}
+__device__ __forceinline__ void wgmma_n64_e4m3(float (&d)[32], uint64_t da, uint64_t db) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k32.f32.e4m3.e4m3 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "l"(da), "l"(db));
+}
+
 template <int BN>
 struct GemmCfg {
   static constexpr int A_BYTES = 128 * 128;          // 128 rows x 128 bytes of K
   static constexpr int B_BYTES = BN * 128;
   static constexpr int STAGE = A_BYTES + B_BYTES;
-  static constexpr int NSTAGE = BN == 128 ? 5 : 6;
+  static constexpr int NSTAGE = BN == 128 ? 6 : 7;
   static constexpr int SMEM = NSTAGE * STAGE + 256 + 1024;
-  static constexpr int TMEM_COLS = 2 * BN <= 128 ? 128 : 256;
+  static_assert(SMEM <= kSmemMax, "shared memory");
 };
 
+// Warpgroups 0 and 1 (warps 0..7) each own 64 rows x BN columns of the 128-row output tile, fp32 accumulators in
+// registers fed by asynchronous wgmma (m64nBNk16 bf16 / m64nBNk32 e4m3) straight from the TMA-written stages; the
+// wgmma group of one stage stays in flight while the next is issued. Warp 8 is the TMA producer; persistent.
 template <int BN, bool FP8>
-__global__ void __launch_bounds__(192, 1)
+__global__ void __launch_bounds__(288, 1)
 kmajor_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const GemmArgs a) {
   using Cfg = GemmCfg<BN>;
   extern __shared__ uint8_t smem_raw[];
@@ -131,29 +157,21 @@ kmajor_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constan
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + Cfg::NSTAGE * Cfg::STAGE);
   uint64_t* full = bars;                          // [NSTAGE]
   uint64_t* empty = bars + Cfg::NSTAGE;           // [NSTAGE]
-  uint64_t* tfull = empty + Cfg::NSTAGE;          // [2]
-  uint64_t* tempty = tfull + 2;                   // [2]
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tempty + 2);
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
   constexpr int KE = FP8 ? 128 : 64;              // K elements per 128-byte k-block
 
-  if (warp == 4 && lane == 0) {
+  if (warp == 8 && lane == 0) {
     prefetch_tmap(&tmA);
     prefetch_tmap(&tmB);
-    for (int s = 0; s < Cfg::NSTAGE; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 1); }
-    for (int i = 0; i < 2; ++i) { mbar_init(&tfull[i], 1); mbar_init(&tempty[i], 4); }
+    for (int s = 0; s < Cfg::NSTAGE; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 8); }
     fence_barrier_init();
   }
-  if (warp == 5) tmem_alloc<Cfg::TMEM_COLS>(tmem_slot);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
   const int num_tiles = a.m_tiles * a.n_tiles;
   const int ksteps = a.taps * a.kblocks;
 
-  if (warp == 4) {
+  if (warp == 8) {
     // ===== TMA producer =====
     if (elect_one()) {
       int st = 0;
@@ -174,48 +192,52 @@ kmajor_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constan
         }
       }
     }
-  } else if (warp == 5) {
-    // ===== MMA issuer =====
-    constexpr uint32_t idesc = FP8 ? make_idesc_e4m3(128, BN) : make_idesc_bf16(128, BN);
-    constexpr uint32_t hi = desc_hi(8 * 128, 128);
-    int st = 0;
-    uint32_t phase = 0;
-    int tb = 0;
-    uint32_t tb_phase = 0;
-    for (int t = blockIdx.x; t < num_tiles; t += gridDim.x) {
-      mbar_wait(&tempty[tb], tb_phase ^ 1u);
-      tc_fence_after();
-      const uint32_t d_tmem = tmem_base + tb * BN;
-      for (int ks = 0; ks < ksteps; ++ks) {
-        mbar_wait(&full[st], phase);
-        tc_fence_after();
-        if (elect_one()) {
-          const uint32_t a_lo = desc_lo(smem_u32(smem + st * Cfg::STAGE));
-          const uint32_t b_lo = desc_lo(smem_u32(smem + st * Cfg::STAGE + Cfg::A_BYTES));
+    return;
+  }
+  // ===== consumer warpgroups
+  const int wg = warp >> 2, wq = warp & 3;
+  float alpha = 1.0f;
+  if (FP8 && a.scale_a) alpha = (*a.scale_a) * (*a.scale_b);
+  int st = 0;
+  uint32_t phase = 0;
+  for (int t = blockIdx.x; t < num_tiles; t += gridDim.x) {
+    const int mb = t / a.n_tiles, nb = t - mb * a.n_tiles;
+    float acc[BN / 2];
 #pragma unroll
-          for (int k = 0; k < 4; ++k) {            // 4 x 32 bytes of K per stage (UMMA_K = 16 bf16 / 32 e4m3)
-            const uint32_t acc = (ks | k) != 0 ? 1u : 0u;
-            if (FP8) umma_f8_lh(d_tmem, a_lo + k * 2, hi, b_lo + k * 2, hi, idesc, acc);
-            else umma_bf16_lh(d_tmem, a_lo + k * 2, hi, b_lo + k * 2, hi, idesc, acc);
-          }
-          umma_commit(&empty[st]);
-          if (ks == ksteps - 1) umma_commit(&tfull[tb]);
+    for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+    int prev = -1;
+    for (int ks = 0; ks < ksteps; ++ks) {
+      mbar_wait(&full[st], phase);
+      const uint32_t sa = smem_u32(smem + st * Cfg::STAGE) + wg * 64 * 128;
+      const uint32_t sb = smem_u32(smem + st * Cfg::STAGE + Cfg::A_BYTES);
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < 4; ++k) {                // 4 x 32 bytes of K per stage
+        const uint64_t da = gmma_desc_sw128(sa + k * 32), db = gmma_desc_sw128(sb + k * 32);
+        if constexpr (FP8) {
+          if constexpr (BN == 128) wgmma_n128_e4m3(acc, da, db); else wgmma_n64_e4m3(acc, da, db);
+        } else {
+          if constexpr (BN == 128) wgmma_n128_bf16(acc, da, db); else wgmma_n64_bf16(acc, da, db);
         }
-        __syncwarp();
-        if (++st == Cfg::NSTAGE) { st = 0; phase ^= 1u; }
       }
-      if (++tb == 2) { tb = 0; tb_phase ^= 1u; }
+      wgmma_commit();
+      wgmma_wait<1>();                             // the previous stage's MMAs are done: release its buffer
+      if (prev >= 0) {
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&empty[prev]);
+      }
+      prev = st;
+      if (++st == Cfg::NSTAGE) { st = 0; phase ^= 1u; }
     }
-  } else {
-    // ===== epilogue warps 0..3: warp w owns TMEM lanes 32w .. 32w+31 (= tile rows) =====
-    const uint32_t lane_base = (uint32_t)(warp * 32) << 16;
-    float alpha = 1.0f;
-    if (FP8 && a.scale_a) alpha = (*a.scale_a) * (*a.scale_b);
-    int tb = 0;
-    uint32_t tb_phase = 0;
-    for (int t = blockIdx.x; t < num_tiles; t += gridDim.x) {
-      const int mb = t / a.n_tiles, nb = t - mb * a.n_tiles;
-      const int64_t m = (int64_t)mb * 128 + warp * 32 + lane;
+    wgmma_wait<0>();
+    if (prev >= 0) {
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&empty[prev]);
+    }
+    // accumulator layout: element 4j + q is row 16*wq + lane/4 (+8 for q >= 2), column 8j + 2*(lane%4) + (q & 1)
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int64_t m = (int64_t)mb * 128 + wg * 64 + wq * 16 + (lane >> 2) + 8 * h;
       bool valid;
       int64_t orow;
       if (a.padded) {
@@ -229,33 +251,12 @@ kmajor_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constan
         valid = m < a.m_rows;
         orow = m;
       }
-      mbar_wait(&tfull[tb], tb_phase);
-      tc_fence_after();
-      __nv_bfloat16* dst = a.C + orow * a.n_total + nb * BN;
-#pragma unroll 1
-      for (int ch = 0; ch < BN / 32; ++ch) {
-        float v[32];
-        tmem_ld32(tmem_base + lane_base + tb * BN + ch * 32, v);
-        if (valid) {
+      if (!valid) continue;
+      __nv_bfloat16* dst = a.C + orow * a.n_total + nb * BN + 2 * (lane & 3);
 #pragma unroll
-          for (int c = 0; c < 32; c += 8) {
-            const uint4 pk = make_uint4(pack_bf16x2(v[c] * alpha, v[c + 1] * alpha), pack_bf16x2(v[c + 2] * alpha, v[c + 3] * alpha),
-                                        pack_bf16x2(v[c + 4] * alpha, v[c + 5] * alpha), pack_bf16x2(v[c + 6] * alpha, v[c + 7] * alpha));
-            *reinterpret_cast<uint4*>(dst + ch * 32 + c) = pk;
-          }
-        }
-      }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&tempty[tb]);
-      if (++tb == 2) { tb = 0; tb_phase ^= 1u; }
+      for (int j = 0; j < BN / 8; ++j)
+        *reinterpret_cast<uint32_t*>(dst + 8 * j) = pack_bf16x2(acc[4 * j + 2 * h] * alpha, acc[4 * j + 2 * h + 1] * alpha);
     }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 5) {
-    tc_fence_after();
-    tmem_dealloc<Cfg::TMEM_COLS>(tmem_base);
   }
 }
 
@@ -270,18 +271,17 @@ void launch_kmajor(const void* A, const void* Bm, const GemmArgs& a, int64_t a_r
   cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM);
   const int tiles = a.m_tiles * a.n_tiles;
   const int grid = tiles < sm_count() ? tiles : sm_count();
-  kern<<<grid, 192, Cfg::SMEM, st>>>(tmA, tmB, a);
+  kern<<<grid, 288, Cfg::SMEM, st>>>(tmA, tmB, a);
   hefl::cuda::note_launch();
 }
 
 // ------------------------------------------------------------------------------------------------------------
-// Block-scaled e4m3 GEMM (kind::mxf8f6f4.block_scale): one UE8M0 scale per row and per 32 elements of K
+// Block-scaled e4m3 GEMM: one UE8M0 scale per row and per 32 elements of K
 // ------------------------------------------------------------------------------------------------------------
 // C[M, N] = sum_k (A[m, k] 2^(sa[m, k/32] - 127)) (B[n, k] 2^(sb[n, k/32] - 127)). A, B: e4m3 bytes, K-major.
-// Scale factors travel in the layout the tensor core wants: for every (128-row block, group of four 32-element
-// k-blocks) one 512-byte tile [lane l = 0..31][row quarter i = 0..3][k-block kb = 0..3] holding the scale of row
-// 32*i + l -- a stage brings its two tiles in with a bulk copy, `tcgen05.cp.32x128b.warpx4` replicates each into
-// four TMEM columns, and the instruction descriptor of MMA kb selects byte kb of those columns (a_sf_id / b_sf_id).
+// Scale factors travel in tiles: for every (128-row block, group of four 32-element k-blocks) one 512-byte tile
+// [lane l = 0..31][row quarter i = 0..3][k-block kb = 0..3] holding the scale of row 32*i + l; a stage brings its
+// two tiles in with a bulk copy.
 struct MxArgs {
   int m_tiles, n_tiles, kgroups;   // 128-row tiles, BN-column tiles, K / 128
   int n_total;
@@ -289,7 +289,6 @@ struct MxArgs {
   __nv_bfloat16* C;
   const uint8_t* sfa;              // [m_tiles][kgroups][512]
   const uint8_t* sfb;              // [N / 128][kgroups][512]
-  uint32_t idesc;                  // instruction descriptor without the scale-factor ids
 };
 
 constexpr int kMxStage = 128 * 128 + 128 * 128 + 1024;    // A tile, B tile, two scale tiles
@@ -301,58 +300,30 @@ __device__ __forceinline__ void bulk_load_1d(void* dst, const void* src, uint32_
                ::"r"(smem_u32(dst)), "l"(src), "r"(bytes), "r"(smem_u32(bar))
                : "memory");
 }
-// 32 rows x 16 bytes, no swizzle: four 8-row core matrices 128 bytes apart
-__device__ __forceinline__ uint64_t sf_desc(uint32_t smem_addr) {
-  uint64_t d = 0;
-  d |= (uint64_t)((smem_addr >> 4) & 0x3FFF);
-  d |= (uint64_t)((128u >> 4) & 0x3FFF) << 32;     // SBO
-  d |= 1ull << 46;
-  return d;
-}
-__device__ __forceinline__ void utccp_32x128b_warpx4(uint32_t taddr, uint64_t sdesc) {
-  asm volatile("tcgen05.cp.cta_group::1.32x128b.warpx4 [%0], %1;" ::"r"(taddr), "l"(sdesc) : "memory");
-}
-__device__ __forceinline__ void umma_mxf8(uint32_t tmem_d, uint32_t alo, uint32_t ahi, uint32_t blo, uint32_t bhi,
-                                          uint32_t idesc, uint32_t tsfa, uint32_t tsfb, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t.reg .b64 da, db;\n\t"
-      "mov.b64 da, {%1, %2};\n\t"
-      "mov.b64 db, {%3, %4};\n\t"
-      "setp.ne.b32 p, %8, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::mxf8f6f4.block_scale [%0], da, db, %5, [%6], [%7], p;\n\t}"
-      ::"r"(tmem_d), "r"(alo), "r"(ahi), "r"(blo), "r"(bhi), "r"(idesc), "r"(tsfa), "r"(tsfb), "r"(accumulate)
-      : "memory");
-}
 
-__global__ void __launch_bounds__(192, 1)
+// Warps 0..7 compute (warp w: rows 32*(w%4) .. +31, columns (w/4)*64 .. +63), warp 8 is the TMA producer. Each
+// 32-element k-block is one m16n8k32 e4m3 MMA into a zeroed fragment, which is then added to the fp32 accumulator
+// scaled by 2^(sa - 127) * 2^(sb - 127) of its row and column (powers of two: the scaling is exact).
+__global__ void __launch_bounds__(288, 1)
 mx_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const MxArgs a) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + kMxStages * kMxStage);
   uint64_t* full = bars;
   uint64_t* empty = bars + kMxStages;
-  uint64_t* tfull = empty + kMxStages;
-  uint64_t* tempty = tfull + 2;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tempty + 2);
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
   constexpr int BN = 128;
-  constexpr uint32_t SFA_COL = 2 * BN, SFB_COL = 2 * BN + 4;
-  if (warp == 4 && lane == 0) {
+  if (warp == 8 && lane == 0) {
     prefetch_tmap(&tmA);
     prefetch_tmap(&tmB);
-    for (int s = 0; s < kMxStages; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 1); }
-    for (int i = 0; i < 2; ++i) { mbar_init(&tfull[i], 1); mbar_init(&tempty[i], 4); }
+    for (int s = 0; s < kMxStages; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 8); }
     fence_barrier_init();
   }
-  if (warp == 5) tmem_alloc<512>(tmem_slot);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
   const int num_tiles = a.m_tiles * a.n_tiles;
 
-  if (warp == 4) {
+  if (warp == 8) {
     if (elect_one()) {
       int st = 0;
       uint32_t phase = 0;
@@ -370,72 +341,75 @@ mx_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         }
       }
     }
-  } else if (warp == 5) {
-    constexpr uint32_t hi = desc_hi(8 * 128, 128);
-    int st = 0;
-    uint32_t phase = 0;
-    int tb = 0;
-    uint32_t tb_phase = 0;
-    for (int t = blockIdx.x; t < num_tiles; t += gridDim.x) {
-      mbar_wait(&tempty[tb], tb_phase ^ 1u);
-      tc_fence_after();
-      const uint32_t d_tmem = tmem_base + tb * BN;
-      for (int kg = 0; kg < a.kgroups; ++kg) {
-        mbar_wait(&full[st], phase);
-        tc_fence_after();
-        if (elect_one()) {
-          uint8_t* s = smem + st * kMxStage;
-          const uint32_t a_lo = desc_lo(smem_u32(s));
-          const uint32_t b_lo = desc_lo(smem_u32(s + 16384));
-          utccp_32x128b_warpx4(tmem_base + SFA_COL, sf_desc(smem_u32(s + 32768)));
-          utccp_32x128b_warpx4(tmem_base + SFB_COL, sf_desc(smem_u32(s + 32768 + 512)));
-#pragma unroll
-          for (int k = 0; k < 4; ++k) {
-            const uint32_t idesc = a.idesc | ((uint32_t)k << 4) | ((uint32_t)k << 29);      // b_sf_id, a_sf_id
-            umma_mxf8(d_tmem, a_lo + k * 2, hi, b_lo + k * 2, hi, idesc, tmem_base + SFA_COL, tmem_base + SFB_COL,
-                      (kg | k) != 0 ? 1u : 0u);
-          }
-          umma_commit(&empty[st]);
-          if (kg == a.kgroups - 1) umma_commit(&tfull[tb]);
-        }
-        __syncwarp();
-        if (++st == kMxStages) { st = 0; phase ^= 1u; }
-      }
-      if (++tb == 2) { tb = 0; tb_phase ^= 1u; }
-    }
-  } else {
-    const uint32_t lane_base = (uint32_t)(warp * 32) << 16;
-    int tb = 0;
-    uint32_t tb_phase = 0;
-    for (int t = blockIdx.x; t < num_tiles; t += gridDim.x) {
-      const int mb = t / a.n_tiles, nb = t - mb * a.n_tiles;
-      const int64_t m = (int64_t)mb * 128 + warp * 32 + lane;
-      const bool valid = m < a.m_rows;
-      mbar_wait(&tfull[tb], tb_phase);
-      tc_fence_after();
-      __nv_bfloat16* dst = a.C + m * a.n_total + nb * BN;
-#pragma unroll 1
-      for (int ch = 0; ch < BN / 32; ++ch) {
-        float v[32];
-        tmem_ld32(tmem_base + lane_base + tb * BN + ch * 32, v);
-        if (valid) {
-#pragma unroll
-          for (int c = 0; c < 32; c += 8)
-            *reinterpret_cast<uint4*>(dst + ch * 32 + c) = make_uint4(pack_bf16x2(v[c], v[c + 1]), pack_bf16x2(v[c + 2], v[c + 3]),
-                                                                       pack_bf16x2(v[c + 4], v[c + 5]), pack_bf16x2(v[c + 6], v[c + 7]));
-        }
-      }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&tempty[tb]);
-      if (++tb == 2) { tb = 0; tb_phase ^= 1u; }
-    }
+    return;
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 5) {
-    tc_fence_after();
-    tmem_dealloc<512>(tmem_base);
+  const int qd = warp & 3, half = warp >> 2;
+  const int g8 = lane >> 2, c2 = (lane & 3) * 2;
+  int st = 0;
+  uint32_t phase = 0;
+  for (int t = blockIdx.x; t < num_tiles; t += gridDim.x) {
+    const int mb = t / a.n_tiles, nb = t - mb * a.n_tiles;
+    float acc[8][2][4];
+#pragma unroll
+    for (int n = 0; n < 8; ++n)
+#pragma unroll
+      for (int mt = 0; mt < 2; ++mt)
+#pragma unroll
+        for (int q = 0; q < 4; ++q) acc[n][mt][q] = 0.f;
+    for (int kg = 0; kg < a.kgroups; ++kg) {
+      mbar_wait(&full[st], phase);
+      uint8_t* s = smem + st * kMxStage;
+      const uint32_t sa = smem_u32(s), sb = sa + 16384;
+      // scale tile layout: byte l*16 + i*4 + kb holds the scale of row (or column) 32*i + l, k-block kb
+      const uint8_t* sfa = s + 32768;
+      const uint8_t* sfb = s + 32768 + 512;
+#pragma unroll
+      for (int kb = 0; kb < 4; ++kb) {
+        uint32_t af[2][4];
+        float fa[2][2];
+#pragma unroll
+        for (int mt = 0; mt < 2; ++mt) {
+          ld_a_kmajor<128>(sa, qd * 32 + mt * 16, kb * 32, lane, af[mt]);
+#pragma unroll
+          for (int h = 0; h < 2; ++h) fa[mt][h] = ldexpf(1.0f, (int)sfa[(mt * 16 + g8 + 8 * h) * 16 + qd * 4 + kb] - 127);
+        }
+#pragma unroll
+        for (int n = 0; n < 8; n += 2) {
+          uint32_t bf[4];
+          const int n0 = half * 64 + n * 8;
+          ld_b_kmajor<128>(sb, n0, n0 + 8, kb * 32, lane, bf);
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            const int col = n0 + e * 8 + c2;
+            const float fb0 = ldexpf(1.0f, (int)sfb[(col & 31) * 16 + (col >> 5) * 4 + kb] - 127);
+            const float fb1 = ldexpf(1.0f, (int)sfb[((col + 1) & 31) * 16 + ((col + 1) >> 5) * 4 + kb] - 127);
+#pragma unroll
+            for (int mt = 0; mt < 2; ++mt) {
+              float p[4] = {0.f, 0.f, 0.f, 0.f};
+              mma_e4m3(p, af[mt], bf[2 * e], bf[2 * e + 1]);
+              acc[n + e][mt][0] += p[0] * fa[mt][0] * fb0;
+              acc[n + e][mt][1] += p[1] * fa[mt][0] * fb1;
+              acc[n + e][mt][2] += p[2] * fa[mt][1] * fb0;
+              acc[n + e][mt][3] += p[3] * fa[mt][1] * fb1;
+            }
+          }
+        }
+      }
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&empty[st]);
+      if (++st == kMxStages) { st = 0; phase ^= 1u; }
+    }
+#pragma unroll
+    for (int mt = 0; mt < 2; ++mt)
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int64_t m = (int64_t)mb * 128 + qd * 32 + mt * 16 + g8 + 8 * h;
+        if (m >= a.m_rows) continue;
+        __nv_bfloat16* dst = a.C + m * a.n_total + nb * BN + half * 64 + c2;
+#pragma unroll
+        for (int n = 0; n < 8; ++n)
+          *reinterpret_cast<uint32_t*>(dst + n * 8) = pack_bf16x2(acc[n][mt][2 * h], acc[n][mt][2 * h + 1]);
+      }
   }
 }
 
@@ -456,20 +430,23 @@ struct WgArgs {
 // second atom lies outside the tensor and TMA fills it with zeros. CT = input-channel tile (MMA N): 64 or 128.
 template <int CT>
 struct WgCfg {
-  static constexpr int ATOMS = CT / 64;                       // 64-channel (128-byte) MN atoms of the X operand
+  static constexpr int ATOMS = CT / 64;                       // 64-channel (128-byte) atoms of the X operand
   static constexpr int A_ATOM = 64 * 128;                     // dY: 64 k-rows x 128 B
-  static constexpr int B_ROWS = 72;                           // X: 64 + 2 shifted rows, rounded to 8
+  static constexpr int B_ROWS = 72;                           // X: 64 rows, rounded up with slack
   static constexpr int B_ATOM = B_ROWS * 128;
   static constexpr int A_BYTES = 2 * A_ATOM;
   static constexpr int B_BYTES = ATOMS * B_ATOM;
   static constexpr int STAGE = ((A_BYTES + B_BYTES + 1023) / 1024) * 1024;
   static constexpr int NSTAGE = CT == 128 ? 5 : 7;
   static constexpr int SMEM = NSTAGE * STAGE + 256 + 1024;
-  static constexpr int TMEM_COLS = 3 * CT <= 256 ? 256 : 512;
+  static constexpr int NT = CT / 16;                          // n8 tiles per compute warp (half of CT)
 };
 
+// Warps 0..7 compute (warp w: output channels 32*(w%4) .. +31, input channels (w/4)*CT/2 .. +CT/2; both operands
+// read from their [pixel][channel] tiles with ldmatrix.trans, pixels = K), warp 8 is the TMA producer. A unit is
+// one (Co tile, Ci tile, tap, pixel range): its accumulators are flushed with fp32 RED.
 template <int CT>
-__global__ void __launch_bounds__(192, 1)
+__global__ void __launch_bounds__(288, 1)
 wgrad_mn_kernel(const __grid_constant__ CUtensorMap tmDY, const __grid_constant__ CUtensorMap tmX, const WgArgs a) {
   using Cfg = WgCfg<CT>;
   extern __shared__ uint8_t smem_raw[];
@@ -477,30 +454,23 @@ wgrad_mn_kernel(const __grid_constant__ CUtensorMap tmDY, const __grid_constant_
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + Cfg::NSTAGE * Cfg::STAGE);
   uint64_t* full = bars;
   uint64_t* empty = bars + Cfg::NSTAGE;
-  uint64_t* tfull = empty + Cfg::NSTAGE;          // [1]
-  uint64_t* tempty = tfull + 1;                   // [1]
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tempty + 1);
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
-  if (warp == 4 && lane == 0) {
+  if (warp == 8 && lane == 0) {
     prefetch_tmap(&tmDY);
     prefetch_tmap(&tmX);
-    for (int s = 0; s < Cfg::NSTAGE; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 1); }
-    mbar_init(tfull, 1);
-    mbar_init(tempty, 4);
+    for (int s = 0; s < Cfg::NSTAGE; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 8); }
     fence_barrier_init();
   }
-  if (warp == 5) tmem_alloc<Cfg::TMEM_COLS>(tmem_slot);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  const int units = a.co_tiles * a.ci_tiles * a.groups * a.ksplit;
+  const int units = a.co_tiles * a.ci_tiles * a.groups * a.taps_per * a.ksplit;
   const int per_split = (a.kchunks + a.ksplit - 1) / a.ksplit;
 
-  auto decode = [&](int u, int& co0, int& ci0, int& g, int& c0, int& c1) {
+  auto decode = [&](int u, int& co0, int& ci0, int& g, int& j, int& c0, int& c1) {
     const int ks = u % a.ksplit;
     int r = u / a.ksplit;
+    j = r % a.taps_per;
+    r /= a.taps_per;
     g = r % a.groups;
     r /= a.groups;
     ci0 = (r % a.ci_tiles) * CT;
@@ -509,97 +479,83 @@ wgrad_mn_kernel(const __grid_constant__ CUtensorMap tmDY, const __grid_constant_
     c1 = min(a.kchunks, c0 + per_split);
   };
 
-  if (warp == 4) {
+  if (warp == 8) {
     if (elect_one()) {
       int st = 0;
       uint32_t phase = 0;
       for (int u = blockIdx.x; u < units; u += gridDim.x) {
-        int co0, ci0, g, c0, c1;
-        decode(u, co0, ci0, g, c0, c1);
+        int co0, ci0, g, j, c0, c1;
+        decode(u, co0, ci0, g, j, c0, c1);
         for (int c = c0; c < c1; ++c) {
           mbar_wait(&empty[st], phase ^ 1u);
           uint8_t* s = smem + st * Cfg::STAGE;
           mbar_expect_tx(&full[st], Cfg::A_BYTES + Cfg::B_BYTES);
           for (int at = 0; at < 2; ++at) tma_load_2d(s + at * Cfg::A_ATOM, &tmDY, co0 + at * 64, c * 64, &full[st]);
           for (int at = 0; at < Cfg::ATOMS; ++at)
-            tma_load_2d(s + Cfg::A_BYTES + at * Cfg::B_ATOM, &tmX, ci0 + at * 64, c * 64 + a.gshift[g], &full[st]);
+            tma_load_2d(s + Cfg::A_BYTES + at * Cfg::B_ATOM, &tmX, ci0 + at * 64, c * 64 + a.gshift[g] + j, &full[st]);
           if (++st == Cfg::NSTAGE) { st = 0; phase ^= 1u; }
         }
       }
     }
-  } else if (warp == 5) {
-    constexpr uint32_t idesc = make_idesc_bf16(128, CT, 1, 1);
-    constexpr uint32_t hi = desc_hi(8 * 128, 128);
-    constexpr uint32_t a_lbo = (uint32_t)(Cfg::A_ATOM >> 4) << 16;
-    constexpr uint32_t b_lbo = (uint32_t)(Cfg::B_ATOM >> 4) << 16;
-    int st = 0;
-    uint32_t phase = 0, tphase = 0;
-    for (int u = blockIdx.x; u < units; u += gridDim.x) {
-      int co0, ci0, g, c0, c1;
-      decode(u, co0, ci0, g, c0, c1);
-      mbar_wait(tempty, tphase ^ 1u);
-      tc_fence_after();
-      for (int c = c0; c < c1; ++c) {
-        mbar_wait(&full[st], phase);
-        tc_fence_after();
-        if (elect_one()) {
-          const uint32_t a_lo = desc_lo(smem_u32(smem + st * Cfg::STAGE)) + a_lbo;
-          const uint32_t b_lo = desc_lo(smem_u32(smem + st * Cfg::STAGE + Cfg::A_BYTES)) + b_lbo;
-#pragma unroll
-          for (int k = 0; k < 4; ++k) {                       // 4 x 16 pixel rows per chunk
-            const uint32_t acc = (c != c0 || k != 0) ? 1u : 0u;
-            for (int j = 0; j < a.taps_per; ++j)
-              umma_bf16_lh(tmem_base + j * CT, a_lo + ((k * 16 * 128) >> 4), hi, b_lo + (((k * 16 + j) * 128) >> 4), hi,
-                           idesc, acc);
-          }
-          umma_commit(&empty[st]);
-          if (c == c1 - 1) umma_commit(tfull);
-        }
-        __syncwarp();
-        if (++st == Cfg::NSTAGE) { st = 0; phase ^= 1u; }
-      }
-      if (c1 > c0) tphase ^= 1u;
-    }
-  } else {
-    // epilogue: TMEM lane = output channel (row of dW), 4 warps x 32 lanes = 128 rows
-    const uint32_t lane_base = (uint32_t)(warp * 32) << 16;
-    uint32_t tphase = 0;
-    for (int u = blockIdx.x; u < units; u += gridDim.x) {
-      int co0, ci0, g, c0, c1;
-      decode(u, co0, ci0, g, c0, c1);
-      if (c1 <= c0) continue;
-      mbar_wait(tfull, tphase);
-      tc_fence_after();
-      const int row = warp * 32 + lane;
-      const bool valid = co0 + row < a.Co;
-#pragma unroll 1
-      for (int j = 0; j < a.taps_per; ++j) {
-        const int tap = g * a.taps_per + j;
-#pragma unroll 1
-        for (int ch = 0; ch < CT / 32; ++ch) {
-          float v[32];
-          tmem_ld32(tmem_base + lane_base + j * CT + ch * 32, v);
-          if (valid) {
-            float* dst = a.dW + ((size_t)tap * a.Co + co0 + row) * a.Ci + ci0 + ch * 32;
-#pragma unroll
-            for (int c = 0; c < 32; c += 4)
-              asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(dst + c), "f"(v[c]), "f"(v[c + 1]),
-                           "f"(v[c + 2]), "f"(v[c + 3])
-                           : "memory");
-          }
-        }
-      }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(tempty);
-      tphase ^= 1u;
-    }
+    return;
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 5) {
-    tc_fence_after();
-    tmem_dealloc<Cfg::TMEM_COLS>(tmem_base);
+  const int qd = warp & 3, half = warp >> 2;
+  const int lrow = lane & 7, ia = lane >> 3;
+  int st = 0;
+  uint32_t phase = 0;
+  for (int u = blockIdx.x; u < units; u += gridDim.x) {
+    int co0, ci0, g, j, c0, c1;
+    decode(u, co0, ci0, g, j, c0, c1);
+    if (c1 <= c0) continue;
+    float acc[Cfg::NT][2][4];
+#pragma unroll
+    for (int n = 0; n < Cfg::NT; ++n)
+#pragma unroll
+      for (int mt = 0; mt < 2; ++mt)
+#pragma unroll
+        for (int q = 0; q < 4; ++q) acc[n][mt][q] = 0.f;
+    for (int c = c0; c < c1; ++c) {
+      mbar_wait(&full[st], phase);
+      const uint32_t sa = smem_u32(smem + st * Cfg::STAGE);
+      const uint32_t sb = sa + Cfg::A_BYTES;
+#pragma unroll
+      for (int k = 0; k < 4; ++k) {                       // 4 x 16 pixel rows per chunk
+        uint32_t af[2][4];
+#pragma unroll
+        for (int mt = 0; mt < 2; ++mt) {
+          const int m = qd * 32 + mt * 16 + (ia & 1) * 8;   // output channel of this lane's 8x8 matrix
+          ldsm_x4_t(swz<128>(sa + (m >> 6) * Cfg::A_ATOM + (k * 16 + (ia >> 1) * 8 + lrow) * 128 + (m & 63) * 2), af[mt]);
+        }
+#pragma unroll
+        for (int n = 0; n < Cfg::NT; n += 2) {
+          uint32_t bf[4];
+          const int nn = half * (CT / 2) + (n + (ia >> 1)) * 8;   // input channel of this lane's 8x8 matrix
+          ldsm_x4_t(swz<128>(sb + (nn >> 6) * Cfg::B_ATOM + (k * 16 + (ia & 1) * 8 + lrow) * 128 + (nn & 63) * 2), bf);
+#pragma unroll
+          for (int mt = 0; mt < 2; ++mt) {
+            mma_bf16(acc[n][mt], af[mt], bf[0], bf[1]);
+            mma_bf16(acc[n + 1][mt], af[mt], bf[2], bf[3]);
+          }
+        }
+      }
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&empty[st]);
+      if (++st == Cfg::NSTAGE) { st = 0; phase ^= 1u; }
+    }
+    const int tap = g * a.taps_per + j;
+#pragma unroll
+    for (int mt = 0; mt < 2; ++mt)
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int co = co0 + qd * 32 + mt * 16 + (lane >> 2) + 8 * h;
+        if (co >= a.Co) continue;
+        float* dst = a.dW + ((size_t)tap * a.Co + co) * a.Ci + ci0 + half * (CT / 2) + 2 * (lane & 3);
+#pragma unroll
+        for (int n = 0; n < Cfg::NT; ++n)
+          asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" ::"l"(dst + n * 8), "f"(acc[n][mt][2 * h]),
+                       "f"(acc[n][mt][2 * h + 1])
+                       : "memory");
+      }
   }
 }
 
@@ -610,9 +566,9 @@ void launch_wgrad_mn(const void* DY, const void* X, const WgArgs& a, int64_t row
   const CUtensorMap tmX = map2d(X, 2, (uint64_t)a.Ci, (uint64_t)rows, (uint64_t)a.Ci * 2, 64, Cfg::B_ROWS);
   auto kern = wgrad_mn_kernel<CT>;
   cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM);
-  const int units = a.co_tiles * a.ci_tiles * a.groups * a.ksplit;
+  const int units = a.co_tiles * a.ci_tiles * a.groups * a.taps_per * a.ksplit;
   const int grid = units < sm_count() ? units : sm_count();
-  kern<<<grid, 192, Cfg::SMEM, st>>>(tmDY, tmX, a);
+  kern<<<grid, 288, Cfg::SMEM, st>>>(tmDY, tmX, a);
   hefl::cuda::note_launch();
 }
 
@@ -679,7 +635,7 @@ void pad_nhwc(const void* x, void* xp, int B, int H, int W, int C, cudaStream_t 
   if (C % 8) throw std::runtime_error("pad_nhwc: C must be a multiple of 8");
   const int64_t total = (int64_t)B * (H + 2) * (W + 2) * (C / 8);
   int blocks = (int)((total + 255) / 256);
-  if (blocks > 148 * 16) blocks = 148 * 16;
+  if (blocks > sm_count() * 16) blocks = sm_count() * 16;
   pad_nhwc_kernel<<<blocks, 256, 0, st>>>(reinterpret_cast<const uint4*>(x), reinterpret_cast<uint4*>(xp), B, H, W, C / 8);
   hefl::cuda::note_launch();
 }
@@ -693,15 +649,14 @@ void conv_weight_prep(const float* w, void* wt, void* wd, int Co, int Ci, int kk
 void conv_wgrad_unpack(const float* dw, float* g, int Co, int Ci, int kk, cudaStream_t st) {
   const int64_t total = (int64_t)kk * Co * Ci;
   int blocks = (int)((total + 255) / 256);
-  if (blocks > 148 * 8) blocks = 148 * 8;
+  if (blocks > sm_count() * 8) blocks = sm_count() * 8;
   conv_wgrad_unpack_kernel<<<blocks, 256, 0, st>>>(dw, g, Co, Ci, kk);
   hefl::cuda::note_launch();
 }
 
-// Block-scaled e4m3 GEMM; sfa / sfb in the tiled layout described at MxArgs. idesc_variant selects the encoding of
-// the M field of the block-scaled instruction descriptor (0: M >> 7 at bit 27, the documented layout; 1: M >> 4 at bit 24).
+// Block-scaled e4m3 GEMM; sfa / sfb in the tiled layout described at MxArgs.
 void gemm_mxfp8(const void* A, const void* Bm, const void* sfa, const void* sfb, void* C, int64_t M, int N, int K,
-                int idesc_variant, cudaStream_t st) {
+                cudaStream_t st) {
   if (K % 128 != 0 || N % 128 != 0) throw std::runtime_error("gemm_mxfp8: K and N must be multiples of 128");
   MxArgs a{};
   a.m_tiles = (int)((M + 127) / 128);
@@ -712,16 +667,12 @@ void gemm_mxfp8(const void* A, const void* Bm, const void* sfa, const void* sfb,
   a.C = reinterpret_cast<__nv_bfloat16*>(C);
   a.sfa = reinterpret_cast<const uint8_t*>(sfa);
   a.sfb = reinterpret_cast<const uint8_t*>(sfb);
-  // e4m3 x e4m3 (formats 0), K-major both, N >> 3 at bit 17, UE8M0 scales (bit 23)
-  uint32_t idesc = ((uint32_t)(128 >> 3) << 17) | (1u << 23);
-  idesc |= idesc_variant == 0 ? ((uint32_t)(128 >> 7) << 27) : ((uint32_t)(128 >> 4) << 24);
-  a.idesc = idesc;
   const CUtensorMap tmA = map2d(A, 1, (uint64_t)K, (uint64_t)M, (uint64_t)K, 128, 128);
   const CUtensorMap tmB = map2d(Bm, 1, (uint64_t)K, (uint64_t)N, (uint64_t)K, 128, 128);
   cudaFuncSetAttribute(mx_gemm_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kMxSmem);
   const int tiles = a.m_tiles * a.n_tiles;
   const int grid = tiles < sm_count() ? tiles : sm_count();
-  mx_gemm_kernel<<<grid, 192, kMxSmem, st>>>(tmA, tmB, a);
+  mx_gemm_kernel<<<grid, 288, kMxSmem, st>>>(tmA, tmB, a);
   hefl::cuda::note_launch();
 }
 
@@ -769,7 +720,7 @@ void wgrad_taps(const void* DY, const void* X, float* dW, int64_t rows, int Co, 
   a.taps_per = taps == 9 ? 3 : 1;
   for (int g = 0; g < a.groups; ++g) a.gshift[g] = taps == 9 ? (g - 1) * Wp - 1 : 0;
   a.kchunks = (int)((rows + 63) / 64);
-  const int base_units = a.co_tiles * a.ci_tiles * a.groups;
+  const int base_units = a.co_tiles * a.ci_tiles * a.groups * a.taps_per;
   int ks = (sm_count() + base_units - 1) / base_units;          // about one wave of CTAs: longer K runs per unit,
                                                                 // fewer REDs onto the same dW words
   if (ks < 1) ks = 1;

@@ -1,5 +1,5 @@
 // Programmatic dependent launch (PDL) for the training-step kernels. Every kernel of the step calls
-// pdl_prologue() after its private set-up (barrier init, tensor-map prefetch, TMEM allocation) and
+// pdl_prologue() after its private set-up (barrier init, tensor-map prefetch) and
 // before it touches global memory; launches go through launch_pdl(), which sets
 // cudaLaunchAttributeProgrammaticStreamSerialization so the next kernel's CTAs become resident and run
 // their set-up while the previous kernel drains. griddepcontrol.wait returns only when the previous

@@ -13,7 +13,7 @@ void adam_step(float* p, float* g, float* m, float* v, void* shadow_bf16, int64_
                const int64_t* step, const float* lr_scale, float lr, float decay, float beta1,
                float beta2, float eps, cudaStream_t st);
 
-// ---- tcgen05 implicit-GEMM convolution (conv_tcgen05.cu) ----
+// ---- tensor-core implicit-GEMM convolution (conv_tcgen05.cu) ----
 void conv_fwd_pool(const void* X, const void* Wf, const float* bias, void* out, uint8_t* argmax, int B, int H,
                    int W, int CK, int CO, int spack, cudaStream_t st);
 bool conv_fwd_pool_pair_supported(int H, int W, int CK, int CO);
@@ -22,7 +22,11 @@ void conv_fwd_pool_pair(const void* X, const void* Wf, const float* bias, void* 
 void conv_set_debug(int mask);
 void conv_dgrad(const void* dY, const void* Wd, void* dX, int B, int H, int W, int CK, int CO, const uint8_t* up_amax,
                 int up_W, cudaStream_t st);
-void conv_wgrad(const void* X, const void* DY, float* dW32, int B, int H, int W, int CK, int Co, cudaStream_t st);
+// Split-K weight gradients write one partial per CTA into a workspace and add the partials to dW32 in a fixed order
+// (fp32 atomics would make the sum, and so training, depend on timing). ws: conv_wgrad_ws_floats(...) floats.
+int64_t conv_wgrad_ws_floats(int B, int H, int W, int CK, int Co);
+void conv_wgrad(const void* X, const void* DY, float* dW32, float* ws, int B, int H, int W, int CK, int Co,
+                cudaStream_t st);
 
 // Dense head (Flatten -> Dense/ReLU -> Dense/ReLU -> Dense -> softmax-CE) forward + backward.
 void head_forward_backward(const void* feat, const float* W1, const float* b1, const float* W2, const float* b2,
@@ -36,13 +40,17 @@ void head_cluster(const void* feat, const float* W1, const float* b1, const floa
                   float* gW3, float* gb3, void* dfeat, float* out, int64_t* step, int B, int C, int train,
                   cudaStream_t st);
 bool wgrad0_gather_supported(int W, int Wp, int CK, int Ci, int Co);
-void wgrad0_gather(const void* X, const void* g, const uint8_t* amax, float* dW, int B, int H, int W, int Hp, int Wp,
-                   cudaStream_t st);
+// layer-1 partials: [wgrad0_parts(B, Hp)][kWgrad0Part] floats of workspace
+constexpr int kWgrad0Part = 28 * 32;
+int wgrad0_parts(int B, int Hp);
+void wgrad0_reduce(const float* ws, int parts, float* dW, cudaStream_t st);
+void wgrad0_gather(const void* X, const void* g, const uint8_t* amax, float* dW, float* ws, int B, int H, int W, int Hp,
+                   int Wp, cudaStream_t st);
 // the same gradient as four masked GEMMs on the tensor cores (wgrad0_mma.cu); needs the s-packed layer-1 input
 bool wgrad0_mma_supported(int W, int Wp, int CK, int Ci, int Co);
-void wgrad0_mma(const void* X, const void* g, const uint8_t* amax, float* dW, int B, int H, int W, int Hp, int Wp,
-                cudaStream_t st);
-// ---- general tcgen05 GEMMs for the ResNet convolutions (gemm_tcgen05.cu) ----
+void wgrad0_mma(const void* X, const void* g, const uint8_t* amax, float* dW, float* ws, int B, int H, int W, int Hp,
+                int Wp, cudaStream_t st);
+// ---- general tensor-core GEMMs for the ResNet convolutions (gemm_tcgen05.cu) ----
 // C[rows_out, N] (bf16) = sum_{t < taps} A[m + shifts[t], K] . B[t*N + n, K]^T. padded != 0: A rows index a zero-padded
 // [Bn][H+2][W+2] grid and only interior pixels are written (to the dense [Bn*H*W, N] output). fp8: A and B hold e4m3
 // bytes and the product of the two device scalars scale_a * scale_b multiplies the result.
@@ -52,7 +60,7 @@ void gemm_taps(const void* A, const void* Bm, void* C, int64_t a_rows, int N, in
 // grid whose rows are Wp pixels long.
 void wgrad_taps(const void* DY, const void* X, float* dW, int64_t rows, int Co, int Ci, int taps, int Wp, cudaStream_t st);
 void gemm_mxfp8(const void* A, const void* Bm, const void* sfa, const void* sfb, void* C, int64_t M, int N, int K,
-                int idesc_variant, cudaStream_t st);
+                cudaStream_t st);
 void pad_nhwc(const void* x, void* xp, int B, int H, int W, int C, cudaStream_t st);          // bf16, zero border of 1
 void conv_weight_prep(const float* w, void* wt, void* wd, int Co, int Ci, int kk, cudaStream_t st);
 void conv_wgrad_unpack(const float* dw, float* g, int Co, int Ci, int kk, cudaStream_t st);
@@ -68,7 +76,7 @@ void fp8_quantize(const void* x, uint8_t* q, const float* scale, float* amax, in
 // bf16 [R,K] -> e4m3 [R,K] + UE8M0 scale tiles [ceil(R/128)][K/128][512] (rows beyond R must be pre-set by the caller)
 void mxfp8_quantize(const void* x, uint8_t* q, uint8_t* sf, int64_t R, int K, cudaStream_t st);
 void fp8_scale_update(float* amax, float* scale, float* inv, float target, cudaStream_t st);
-void umma_shift_probe(const void* A, const void* Bm, float* out, int CK, int shift_rows, int mode, cudaStream_t st);
+void umma_shift_probe(const void* A, const void* Bm, float* out, int CK, int shift_rows, cudaStream_t st);
 
 // ---- data-movement kernels around the convolutions (nn_kernels.cu) ----
 constexpr int kMaxConvLayers = 8;

@@ -137,7 +137,9 @@ void conv_wgrad(const Tensor& X, const Tensor& DY, Tensor dW32, int64_t B, int64
   const int64_t P = B * H * W;
   TORCH_CHECK(X.numel() == P * CK && DY.numel() == P * Co, "X must be [B*H*W,CK] and DY [B*H*W,Co]");
   TORCH_CHECK(dW32.is_cuda() && dW32.scalar_type() == at::kFloat && dW32.numel() >= (9 * CK + 1) * Co, "dW32 too small");
-  hefl::nn::conv_wgrad(X.data_ptr(), DY.data_ptr(), dW32.data_ptr<float>(), (int)B, (int)H, (int)W, (int)CK, (int)Co, cur());
+  Tensor ws = at::empty({hefl::nn::conv_wgrad_ws_floats((int)B, (int)H, (int)W, (int)CK, (int)Co)}, dW32.options());
+  hefl::nn::conv_wgrad(X.data_ptr(), DY.data_ptr(), dW32.data_ptr<float>(), ws.data_ptr<float>(), (int)B, (int)H, (int)W,
+                       (int)CK, (int)Co, cur());
 }
 
 void preprocess_u8(const Tensor& x, const c10::optional<Tensor>& theta, Tensor X, int64_t aug_seed,
@@ -244,13 +246,14 @@ void wgrad0_gather(const Tensor& X, const Tensor& g, const Tensor& amax, Tensor 
   TORCH_CHECK(hefl::nn::wgrad0_gather_supported((int)W, (int)Wp, 16, 3, 32), "wgrad0_gather: unsupported shape");
   TORCH_CHECK(X.numel() >= B * H * W * 16 && g.numel() == B * Hp * Wp * 32 && amax.numel() == g.numel(), "shape mismatch");
   TORCH_CHECK(amax.scalar_type() == at::kByte && dW32.scalar_type() == at::kFloat && dW32.numel() >= (9 * 16 + 1) * 32, "dtype / size");
+  Tensor ws = at::empty({(int64_t)hefl::nn::wgrad0_parts((int)B, (int)Hp) * hefl::nn::kWgrad0Part}, dW32.options());
   if (spack && hefl::nn::wgrad0_mma_supported((int)W, (int)Wp, 16, 3, 32)) {      // s-packed input: masked GEMMs on the tensor cores
-    hefl::nn::wgrad0_mma(X.data_ptr(), g.data_ptr(), amax.data_ptr<uint8_t>(), dW32.data_ptr<float>(), (int)B, (int)H, (int)W,
-                         (int)Hp, (int)Wp, cur());
+    hefl::nn::wgrad0_mma(X.data_ptr(), g.data_ptr(), amax.data_ptr<uint8_t>(), dW32.data_ptr<float>(), ws.data_ptr<float>(),
+                         (int)B, (int)H, (int)W, (int)Hp, (int)Wp, cur());
     return;
   }
-  hefl::nn::wgrad0_gather(X.data_ptr(), g.data_ptr(), amax.data_ptr<uint8_t>(), dW32.data_ptr<float>(), (int)B, (int)H,
-                          (int)W, (int)Hp, (int)Wp, cur());
+  hefl::nn::wgrad0_gather(X.data_ptr(), g.data_ptr(), amax.data_ptr<uint8_t>(), dW32.data_ptr<float>(), ws.data_ptr<float>(),
+                          (int)B, (int)H, (int)W, (int)Hp, (int)Wp, cur());
 }
 
 void avgpool_forward(const Tensor& x, Tensor out, int64_t B, int64_t HW, int64_t C) {
@@ -266,10 +269,10 @@ void avgpool_backward(const Tensor& dout, Tensor dx, int64_t B, int64_t HW, int6
 }
 
 // q = e4m3(sat(x * scale)) (q: uint8 storage, viewed as float8_e4m3fn by the caller); amax = max(amax, |x|).
-// out[rows_out, N] bf16 = sum_taps A[m + shift, K] . B[t*N + n, K]^T (tcgen05; csrc/nn/gemm_tcgen05.cu)
+// out[rows_out, N] bf16 = sum_taps A[m + shift, K] . B[t*N + n, K]^T (tensor cores; csrc/nn/gemm_tcgen05.cu)
 void gemm_taps(const Tensor& A, const Tensor& Bm, Tensor out, int64_t N, int64_t K, at::IntArrayRef shifts, int64_t padded,
                int64_t Bn, int64_t H, int64_t W, const c10::optional<Tensor>& scale_a, const c10::optional<Tensor>& scale_b) {
-  TORCH_CHECK(A.is_cuda() && Bm.is_cuda() && out.is_cuda(), "gemm_taps is a CUDA (sm_100a) op");
+  TORCH_CHECK(A.is_cuda() && Bm.is_cuda() && out.is_cuda(), "gemm_taps is a CUDA (sm_90a) op");
   TORCH_CHECK(A.is_contiguous() && Bm.is_contiguous() && out.is_contiguous(), "contiguous operands expected");
   const bool fp8 = A.element_size() == 1;
   TORCH_CHECK(A.element_size() == Bm.element_size() && (fp8 || A.scalar_type() == at::kBFloat16), "bf16 or e4m3 operands");
@@ -288,7 +291,7 @@ void gemm_taps(const Tensor& A, const Tensor& Bm, Tensor out, int64_t N, int64_t
 
 // dW [taps, Co, Ci] fp32 (zeroed here) = dY[rows, Co]^T . X[rows + shift(tap), Ci]
 void wgrad_taps(const Tensor& DY, const Tensor& X, Tensor dW, int64_t taps, int64_t Wp) {
-  TORCH_CHECK(DY.is_cuda() && X.is_cuda() && dW.is_cuda(), "wgrad_taps is a CUDA (sm_100a) op");
+  TORCH_CHECK(DY.is_cuda() && X.is_cuda() && dW.is_cuda(), "wgrad_taps is a CUDA (sm_90a) op");
   TORCH_CHECK(DY.scalar_type() == at::kBFloat16 && X.scalar_type() == at::kBFloat16 && dW.scalar_type() == at::kFloat, "dtypes");
   TORCH_CHECK(DY.dim() == 2 && X.dim() == 2 && DY.size(0) == X.size(0) && DY.is_contiguous() && X.is_contiguous() && dW.is_contiguous(),
               "DY [rows, Co], X [rows, Ci]");
@@ -299,14 +302,14 @@ void wgrad_taps(const Tensor& DY, const Tensor& X, Tensor dW, int64_t taps, int6
 }
 
 // out [M,N] bf16 = block-scaled e4m3 GEMM (kind::mxf8f6f4.block_scale); sfa / sfb: uint8 tiles [rows/128][K/128][512]
-void gemm_mxfp8(const Tensor& A, const Tensor& Bm, const Tensor& sfa, const Tensor& sfb, Tensor out, int64_t variant) {
+void gemm_mxfp8(const Tensor& A, const Tensor& Bm, const Tensor& sfa, const Tensor& sfb, Tensor out) {
   TORCH_CHECK(A.is_cuda() && A.element_size() == 1 && Bm.element_size() == 1 && A.dim() == 2 && Bm.dim() == 2 &&
               A.is_contiguous() && Bm.is_contiguous() && A.size(1) == Bm.size(1), "A [M,K], B [N,K] e4m3 bytes");
   const int64_t M = A.size(0), K = A.size(1), N = Bm.size(0);
   TORCH_CHECK(out.scalar_type() == at::kBFloat16 && out.numel() == M * N && out.is_contiguous(), "out [M,N] bf16");
   TORCH_CHECK(sfa.numel() == ((M + 127) / 128) * (K / 128) * 512 && sfb.numel() == (N / 128) * (K / 128) * 512 &&
               sfa.is_contiguous() && sfb.is_contiguous(), "scale-factor tiles have the wrong size");
-  hefl::nn::gemm_mxfp8(A.data_ptr(), Bm.data_ptr(), sfa.data_ptr(), sfb.data_ptr(), out.data_ptr(), M, (int)N, (int)K, (int)variant, cur());
+  hefl::nn::gemm_mxfp8(A.data_ptr(), Bm.data_ptr(), sfa.data_ptr(), sfb.data_ptr(), out.data_ptr(), M, (int)N, (int)K, cur());
 }
 
 // x bf16 [R,K] (K % 128 == 0) -> (e4m3 bytes [R,K], UE8M0 scale tiles uint8 [ceil(R/128) * K/128 * 512])
@@ -375,11 +378,11 @@ void fused_update(Tensor dW32, const Tensor& table, Tensor flat, Tensor grad, Te
                          (float)lr, (float)decay, (float)beta1, (float)beta2, (float)eps, dense_off, n_trainable, cur());
 }
 
-Tensor umma_shift_probe(const Tensor& A, const Tensor& Bm, int64_t CK, int64_t shift_rows, int64_t mode) {
+Tensor umma_shift_probe(const Tensor& A, const Tensor& Bm, int64_t CK, int64_t shift_rows) {
   chk_bf16(A, "A"); chk_bf16(Bm, "Bm");
   TORCH_CHECK(A.numel() == 144 * CK && Bm.numel() == 32 * CK, "A must be [144,CK], B [32,CK]");
   Tensor out = at::zeros({128, 32}, A.options().dtype(at::kFloat));
-  hefl::nn::umma_shift_probe(A.data_ptr(), Bm.data_ptr(), out.data_ptr<float>(), (int)CK, (int)shift_rows, (int)mode, cur());
+  hefl::nn::umma_shift_probe(A.data_ptr(), Bm.data_ptr(), out.data_ptr<float>(), (int)CK, (int)shift_rows, cur());
   return out;
 }
 
@@ -438,7 +441,7 @@ TORCH_LIBRARY_FRAGMENT(hefl, m) {
   m.def("wgrad_taps(Tensor DY, Tensor X, Tensor(a!) dW, int taps, int Wp) -> ()", &wgrad_taps);
   m.def("pad_nhwc(Tensor x) -> Tensor", &pad_nhwc);
   m.def("mxfp8_quantize(Tensor x) -> (Tensor, Tensor)", &mxfp8_quantize);
-  m.def("gemm_mxfp8(Tensor A, Tensor B, Tensor sfa, Tensor sfb, Tensor(a!) out, int variant) -> ()", &gemm_mxfp8);
+  m.def("gemm_mxfp8(Tensor A, Tensor B, Tensor sfa, Tensor sfb, Tensor(a!) out) -> ()", &gemm_mxfp8);
   m.def("fp8_scale_update(Tensor(a!) amax, Tensor(b!) scale, Tensor(c!) inv, float target) -> ()", &fp8_scale_update);
   m.def("conv_weight_prep(Tensor w) -> (Tensor, Tensor)", &conv_weight_prep);
   m.def("conv_wgrad_unpack(Tensor dw, int Co, int Ci, int k) -> Tensor", &conv_wgrad_unpack);
@@ -446,7 +449,7 @@ TORCH_LIBRARY_FRAGMENT(hefl, m) {
   m.def("bn_backward(Tensor dy, Tensor x, Tensor y, Tensor mean, Tensor invstd, Tensor gamma, Tensor(a!) sums, Tensor(b!) dx, Tensor(c!)? dres, bool relu) -> ()", &bn_backward);
   m.def("avgpool_forward(Tensor x, Tensor(a!) out, int B, int HW, int C) -> ()", &avgpool_forward);
   m.def("avgpool_backward(Tensor dout, Tensor(a!) dx, int B, int HW, int C) -> ()", &avgpool_backward);
-  m.def("umma_shift_probe(Tensor A, Tensor Bm, int CK, int shift_rows, int mode) -> Tensor", &umma_shift_probe);
+  m.def("umma_shift_probe(Tensor A, Tensor Bm, int CK, int shift_rows) -> Tensor", &umma_shift_probe);
   m.def("conv_weight_relayout(Tensor shadow, Tensor table, Tensor(a!) Wf, Tensor(b!) Wd, int l0=0, int l1=-1, bool spack0=False) -> ()", &conv_weight_relayout);
   m.def("conv_grad_finalize(Tensor(a!) dW32, Tensor table, Tensor(b!) grad, int l0=0, int l1=-1) -> ()", &conv_grad_finalize);
 }

@@ -1,4 +1,4 @@
-// Small fused NN kernels for sm_100a: Adam (+ bf16 weight shadow), input preprocessing,
+// Small fused NN kernels for sm_90a: Adam (+ bf16 weight shadow), input preprocessing,
 // un-pooling of gradients. SURVEY.md §2.4 K17.
 #include <cuda_bf16.h>
 
@@ -42,7 +42,7 @@ void adam_step(float* p, float* g, float* m, float* v, void* shadow_bf16, int64_
                float beta2, float eps, cudaStream_t st) {
   if (n == 0) return;
   int blocks = (int)((n + 255) / 256);
-  if (blocks > 148 * 8) blocks = 148 * 8;
+  if (blocks > hefl::cuda::device_sm_count() * 8) blocks = hefl::cuda::device_sm_count() * 8;
   launch_pdl(adam_kernel, dim3(blocks), dim3(256), 0, st, p, g, m, v, reinterpret_cast<__nv_bfloat16*>(shadow_bf16), n,
                                       step, lr_scale, lr, decay, beta1, beta2, eps);
   hefl::cuda::note_launch();

@@ -1,4 +1,4 @@
-// ResNet building blocks for sm_100a (SURVEY.md K18): training-mode BatchNorm over NHWC bf16 with
+// ResNet building blocks for sm_90a (SURVEY.md K18): training-mode BatchNorm over NHWC bf16 with
 // fused residual add and ReLU (forward and backward), and global average pooling. Activations are
 // [P = B*H*W pixels, C channels] bf16, statistics and parameters fp32.
 //
@@ -219,9 +219,9 @@ void bn_forward(const void* x, const void* res, const float* gamma, const float*
   cudaMemsetAsync(sums, 0, 2 * C * sizeof(float), st);
   const int threads = 256 - 256 % (C / 8 > 256 ? 256 : (C / 8));   // multiple of the channel-group count
   const int rows_per_iter = threads / (C / 8);
-  bn_stats_kernel<<<blocks_for(P, rows_per_iter * 8, 148 * 4), threads, 2 * C * 4, st>>>(
+  bn_stats_kernel<<<blocks_for(P, rows_per_iter * 8, hefl::cuda::device_sm_count() * 4), threads, 2 * C * 4, st>>>(
       reinterpret_cast<const __nv_bfloat16*>(x), sums, P, C);
-  bn_apply_kernel<<<blocks_for(P, rows_per_iter * 4, 148 * 8), threads, 2 * C * 4, st>>>(
+  bn_apply_kernel<<<blocks_for(P, rows_per_iter * 4, hefl::cuda::device_sm_count() * 8), threads, 2 * C * 4, st>>>(
       reinterpret_cast<const __nv_bfloat16*>(x), reinterpret_cast<const __nv_bfloat16*>(res), sums, gamma, beta, mean,
       invstd, run_mean, run_var, reinterpret_cast<__nv_bfloat16*>(y), P, C, momentum, eps, relu);
   hefl::cuda::note_launch(2);
@@ -232,10 +232,10 @@ void bn_backward(const void* dy, const void* x, const void* y, const float* mean
   cudaMemsetAsync(sums, 0, 2 * C * sizeof(float), st);
   const int threads = 256 - 256 % (C / 8 > 256 ? 256 : (C / 8));
   const int rows_per_iter = threads / (C / 8);
-  bn_bwd_reduce_kernel<<<blocks_for(P, rows_per_iter * 8, 148 * 4), threads, 2 * C * 4, st>>>(
+  bn_bwd_reduce_kernel<<<blocks_for(P, rows_per_iter * 8, hefl::cuda::device_sm_count() * 4), threads, 2 * C * 4, st>>>(
       reinterpret_cast<const __nv_bfloat16*>(dy), reinterpret_cast<const __nv_bfloat16*>(x),
       reinterpret_cast<const __nv_bfloat16*>(y), mean, invstd, sums, P, C, relu);
-  bn_bwd_apply_kernel<<<blocks_for(P, rows_per_iter * 4, 148 * 8), threads, 3 * C * 4, st>>>(
+  bn_bwd_apply_kernel<<<blocks_for(P, rows_per_iter * 4, hefl::cuda::device_sm_count() * 8), threads, 3 * C * 4, st>>>(
       reinterpret_cast<const __nv_bfloat16*>(dy), reinterpret_cast<const __nv_bfloat16*>(x),
       reinterpret_cast<const __nv_bfloat16*>(y), mean, invstd, gamma, sums, reinterpret_cast<__nv_bfloat16*>(dx),
       reinterpret_cast<__nv_bfloat16*>(dres), P, C, relu);
@@ -266,7 +266,7 @@ void avgpool_forward(const void* x, float* out, int B, int HW, int C, cudaStream
 }
 void avgpool_backward(const float* dout, void* dx, int B, int HW, int C, cudaStream_t st) {
   const int64_t total = (int64_t)B * HW * C;
-  avgpool_bwd_kernel<<<blocks_for(total, 256, 148 * 8), 256, 0, st>>>(dout, reinterpret_cast<__nv_bfloat16*>(dx), HW, C, total);
+  avgpool_bwd_kernel<<<blocks_for(total, 256, hefl::cuda::device_sm_count() * 8), 256, 0, st>>>(dout, reinterpret_cast<__nv_bfloat16*>(dx), HW, C, total);
   hefl::cuda::note_launch();
 }
 
@@ -360,7 +360,7 @@ __global__ void mxfp8_quantize_kernel(const __nv_bfloat16* __restrict__ x, uint8
 
 void mxfp8_quantize(const void* x, uint8_t* q, uint8_t* sf, int64_t R, int K, cudaStream_t st) {
   const int64_t total = R * (K >> 5);
-  mxfp8_quantize_kernel<<<blocks_for(total, 256, 148 * 16), 256, 0, st>>>(reinterpret_cast<const __nv_bfloat16*>(x), q, sf, R, K);
+  mxfp8_quantize_kernel<<<blocks_for(total, 256, hefl::cuda::device_sm_count() * 16), 256, 0, st>>>(reinterpret_cast<const __nv_bfloat16*>(x), q, sf, R, K);
   hefl::cuda::note_launch();
 }
 
@@ -383,7 +383,7 @@ void fp8_scale_update(float* amax, float* scale, float* inv, float target, cudaS
 
 void fp8_quantize(const void* x, uint8_t* q, const float* scale, float* amax, int64_t n, cudaStream_t st) {
   const int64_t n8 = n / 8;
-  fp8_quantize_kernel<<<blocks_for(n8, 256 * 4, 148 * 8), 256, 0, st>>>(reinterpret_cast<const __nv_bfloat16*>(x), q, scale,
+  fp8_quantize_kernel<<<blocks_for(n8, 256 * 4, hefl::cuda::device_sm_count() * 8), 256, 0, st>>>(reinterpret_cast<const __nv_bfloat16*>(x), q, scale,
                                                                        amax, n8);
   hefl::cuda::note_launch();
 }

@@ -1,6 +1,5 @@
-// Thin inline-PTX wrappers for the Blackwell (sm_100a) tensor-core programming model:
-// mbarrier, TMA (cp.async.bulk.tensor), TMEM allocation, tcgen05.mma / commit / ld, and the
-// shared-memory / instruction descriptors for K-major bf16 operands.
+// Thin inline-PTX wrappers for the Hopper (sm_90a) kernels: mbarrier, TMA (cp.async.bulk.tensor), and warp-level
+// tensor-core MMAs (ldmatrix + mma.sync) on the swizzled tiles TMA writes.
 #pragma once
 #include <cstdint>
 #include <cuda.h>
@@ -8,6 +7,11 @@
 
 namespace hefl {
 namespace tc {
+
+// Largest dynamic shared memory a block may opt into on H100 (sm_90): 227 KB. An SM has 228 KB and reserves 1 KB per
+// resident block, so `nblocks` blocks of `smem` dynamic bytes fit on one SM when blocks_fit(smem, nblocks).
+constexpr int kSmemMax = 227 * 1024;
+constexpr bool blocks_fit(int smem, int nblocks) { return nblocks * (smem + 1024) <= 228 * 1024; }
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) {
   return static_cast<uint32_t>(__cvta_generic_to_shared(p));
@@ -79,135 +83,92 @@ __device__ __forceinline__ void tma_load_3d(void* dst, const CUtensorMap* map, i
       : "memory");
 }
 
-// ---- TMEM ---------------------------------------------------------------------------------
-template <int NCOLS>
-__device__ __forceinline__ void tmem_alloc(uint32_t* dst_in_smem) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(dst_in_smem)),
-               "n"(NCOLS)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
+// ---- warp-level tensor-core MMA on TMA-written shared-memory tiles (sm_90) ---------------------
+// TMA writes a tile with a swizzle span of SW bytes (32, 64 or 128, equal to the tile's row length): the 16-byte
+// chunk index inside a span is XORed with address bits 7.. . The pattern is a function of the absolute shared-memory
+// address (tile bases are aligned to the pattern's repeat), so a tile may be read starting at ANY row: the halo
+// kernels read shifted row windows of one loaded tile instead of loading every tap separately.
+template <int SW>
+__device__ __forceinline__ uint32_t swz(uint32_t addr) {
+  constexpr uint32_t M = SW == 128 ? 7u : (SW == 64 ? 3u : 1u);
+  return addr ^ (((addr >> 7) & M) << 4);
 }
-template <int NCOLS>
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "n"(NCOLS) : "memory");
+__device__ __forceinline__ void ldsm_x4(uint32_t addr, uint32_t (&r)[4]) {
+  asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0, %1, %2, %3}, [%4];"
+               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]) : "r"(addr) : "memory");
 }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-// D[tmem] (+)= A[smem] * B[smem]^T, bf16 inputs, fp32 accumulate, issued by ONE thread.
-__device__ __forceinline__ void umma_bf16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                          uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
+__device__ __forceinline__ void ldsm_x4_t(uint32_t addr, uint32_t (&r)[4]) {
+  asm volatile("ldmatrix.sync.aligned.m8n8.x4.trans.shared.b16 {%0, %1, %2, %3}, [%4];"
+               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]) : "r"(addr) : "memory");
 }
-// Same, with the two 64-bit descriptors passed as 32-bit halves: the issuing thread only ever does
-// 32-bit adds on the low word (start address >> 4 lives in bits 0..13, LBO in 16..29).
-__device__ __forceinline__ void umma_bf16_lh(uint32_t tmem_d, uint32_t alo, uint32_t ahi, uint32_t blo, uint32_t bhi,
-                                             uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t.reg .b64 da, db;\n\t"
-      "mov.b64 da, {%1, %2};\n\t"
-      "mov.b64 db, {%3, %4};\n\t"
-      "setp.ne.b32 p, %6, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], da, db, %5, p;\n\t}"
-      ::"r"(tmem_d), "r"(alo), "r"(ahi), "r"(blo), "r"(bhi), "r"(idesc), "r"(accumulate)
-      : "memory");
+// d (m16 x n8, fp32) += a (m16 x k16, bf16, row) * b (k16 x n8, bf16, col)
+__device__ __forceinline__ void mma_bf16(float (&d)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
+  asm volatile("mma.sync.aligned.m16n8k16.row.col.f32.bf16.bf16.f32 {%0, %1, %2, %3}, {%4, %5, %6, %7}, {%8, %9}, "
+               "{%0, %1, %2, %3};"
+               : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
+               : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
 }
-// One lane of a converged warp (lets the compiler keep MMA operands in uniform registers; a plain
-// `lane == 0` test costs a divergence "waterfall" around every tcgen05.mma).
-__device__ __forceinline__ bool elect_one() {
-  uint32_t pred;
-  asm volatile("{\n\t.reg .pred p;\n\telect.sync _|p, 0xffffffff;\n\tselp.u32 %0, 1, 0, p;\n\t}" : "=r"(pred));
-  return pred != 0;
+// d (m16 x n8, fp32) += a (m16 x k32, e4m3, row) * b (k32 x n8, e4m3, col)
+__device__ __forceinline__ void mma_e4m3(float (&d)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
+  asm volatile("mma.sync.aligned.m16n8k32.row.col.f32.e4m3.e4m3.f32 {%0, %1, %2, %3}, {%4, %5, %6, %7}, {%8, %9}, "
+               "{%0, %1, %2, %3};"
+               : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
+               : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
 }
-__host__ __device__ constexpr uint32_t desc_hi(int sbo_bytes, int swizzle_bytes) {
-  return (uint32_t)((sbo_bytes >> 4) & 0x3FFF) | (1u << 14) |
-         ((swizzle_bytes == 128 ? 2u : (swizzle_bytes == 64 ? 4u : 6u)) << 29);
+// A fragment (m16 x 32 bytes of K) of a K-major tile: row r of the fragment is tile row row0 + r, K bytes kb0..kb0+31.
+template <int SW>
+__device__ __forceinline__ void ld_a_kmajor(uint32_t tile, int row0, int kb0, int lane, uint32_t (&a)[4]) {
+  ldsm_x4(swz<SW>(tile + (uint32_t)((row0 + (lane & 15)) * SW + kb0 + ((lane >> 4) << 4))), a);
 }
-__device__ __forceinline__ uint32_t desc_lo(uint32_t smem_addr, int lbo_bytes = 0) {
-  return ((smem_addr >> 4) & 0x3FFFu) | ((uint32_t)(lbo_bytes >> 4) << 16);
+// B fragments of two n8 tiles (rows n0 and n1 of a K-major [N][K] tile), 32 bytes of K: b[0..1] tile n0, b[2..3] n1.
+template <int SW>
+__device__ __forceinline__ void ld_b_kmajor(uint32_t tile, int n0, int n1, int kb0, int lane, uint32_t (&b)[4]) {
+  const int n = ((lane >> 4) ? n1 : n0) + (lane & 7);
+  ldsm_x4(swz<SW>(tile + (uint32_t)(n * SW + kb0 + (((lane >> 3) & 1) << 4))), b);
 }
-
-// Arrive on an mbarrier when all previously issued MMAs of this thread have completed.
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-               : "memory");
+// Accumulator staging: a warp's two m16 x n8 fragments (rows 0-15, 16-31 of its 32 rows) -> row `lane`, 8 columns.
+// `scr` is the warp's private 1 KB of shared memory.
+__device__ __forceinline__ void frag_rows(float* scr, const float (&c0)[4], const float (&c1)[4], int lane, float* v) {
+  const int r = lane >> 2, c = (lane & 3) * 2;
+  __syncwarp();
+  *reinterpret_cast<float2*>(scr + r * 8 + c) = make_float2(c0[0], c0[1]);
+  *reinterpret_cast<float2*>(scr + (r + 8) * 8 + c) = make_float2(c0[2], c0[3]);
+  *reinterpret_cast<float2*>(scr + (r + 16) * 8 + c) = make_float2(c1[0], c1[1]);
+  *reinterpret_cast<float2*>(scr + (r + 24) * 8 + c) = make_float2(c1[2], c1[3]);
+  __syncwarp();
+  const float4 x = *reinterpret_cast<const float4*>(scr + lane * 8);
+  const float4 y = *reinterpret_cast<const float4*>(scr + lane * 8 + 4);
+  v[0] = x.x; v[1] = x.y; v[2] = x.z; v[3] = x.w; v[4] = y.x; v[5] = y.y; v[6] = y.z; v[7] = y.w;
 }
-// 32 lanes x 32 consecutive fp32 columns -> 32 registers per thread (thread t = lane base + t).
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, float* v) {
-  uint32_t* r = reinterpret_cast<uint32_t*>(v);
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-        "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]),
-        "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]),
-        "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
-
-// 32 lanes x 16 consecutive fp32 columns.
-__device__ __forceinline__ void tmem_ld16_nowait(uint32_t taddr, float* v) {
-  uint32_t* r = reinterpret_cast<uint32_t*>(v);
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-        "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
-}
-// 32 lanes x 8 consecutive fp32 columns.
-__device__ __forceinline__ void tmem_ld8_nowait(uint32_t taddr, float* v) {
-  uint32_t* r = reinterpret_cast<uint32_t*>(v);
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0, %1, %2, %3, %4, %5, %6, %7}, [%8];"
-               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7])
-               : "r"(taddr)
-               : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ uint32_t pack_bf16x2(float lo, float hi) {
   uint32_t r;
   asm("cvt.rn.bf16x2.f32 %0, %1, %2;" : "=r"(r) : "f"(hi), "f"(lo));
   return r;
 }
+// One lane of a converged warp.
+__device__ __forceinline__ bool elect_one() {
+  uint32_t pred;
+  asm volatile("{\n\t.reg .pred p;\n\telect.sync _|p, 0xffffffff;\n\tselp.u32 %0, 1, 0, p;\n\t}" : "=r"(pred));
+  return pred != 0;
+}
 
-// ---- descriptors ----------------------------------------------------------------------------
-// K-major operand tile whose K extent is exactly one swizzle atom wide (row_bytes in {32,64,128}):
-// 8-row groups are `8*row_bytes` apart (SBO), LBO unused, sm_100 descriptor version 1.
-__device__ __forceinline__ uint64_t make_kmajor_desc(uint32_t smem_addr, int row_bytes) {
-  const uint64_t layout = row_bytes == 128 ? 2ull : (row_bytes == 64 ? 4ull : 6ull);
-  uint64_t d = 0;
-  d |= (uint64_t)((smem_addr >> 4) & 0x3FFF);
-  d |= (uint64_t)(((8u * (uint32_t)row_bytes) >> 4) & 0x3FFF) << 32;
-  d |= 1ull << 46;
-  d |= layout << 61;
-  return d;
-}
-// MN-major operand tile: smem holds [MN atoms][K rows][atom_bytes] where one "row" is a single k
-// with atom_bytes/2 contiguous M (or N) elements, swizzled in 8-row groups. SBO = stride between
-// 8-k-row groups, LBO = stride between MN atoms (DeepGEMM convention for swizzled MN-major).
-__device__ __forceinline__ uint64_t make_mnmajor_desc(uint32_t smem_addr, int atom_bytes, int lbo_bytes) {
-  const uint64_t layout = atom_bytes == 128 ? 2ull : (atom_bytes == 64 ? 4ull : 6ull);
-  uint64_t d = 0;
-  d |= (uint64_t)((smem_addr >> 4) & 0x3FFF);
-  d |= (uint64_t)(((uint32_t)lbo_bytes >> 4) & 0x3FFF) << 16;
-  d |= (uint64_t)(((8u * (uint32_t)atom_bytes) >> 4) & 0x3FFF) << 32;
-  d |= 1ull << 46;
-  d |= layout << 61;
-  return d;
-}
-// bf16 x bf16 -> fp32; a_mn / b_mn select MN-major (1) or K-major (0) operands.
-__host__ __device__ constexpr uint32_t make_idesc_bf16(int M, int N, int a_mn = 0, int b_mn = 0) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)a_mn << 15) | ((uint32_t)b_mn << 16) |
-         ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
+// Deterministic split-K reduction: returns sum over p = 0 .. parts-1 of ws[p * n + i] for element i = blockIdx.x * 32 +
+// lane, with a fixed summation tree (warp j of the 256-thread block sums p = j, j + 8, ... in order, then the eight
+// warp sums are added in warp order), so the result is the same bits on every run. Call with blockDim.x == 256;
+// `red` is 256 floats of shared memory; the result is valid in warp 0.
+__device__ __forceinline__ float sum_partials(const float* __restrict__ ws, int parts, int64_t n, float* red) {
+  const int lane = threadIdx.x & 31, j = threadIdx.x >> 5;
+  const int64_t i = (int64_t)blockIdx.x * 32 + lane;
+  float s = 0.f;
+  if (i < n)
+    for (int p = j; p < parts; p += 8) s += ws[(int64_t)p * n + i];
+  red[threadIdx.x] = s;
+  __syncthreads();
+  float t = 0.f;
+  if (j == 0)
+#pragma unroll
+    for (int w = 0; w < 8; ++w) t += red[w * 32 + lane];
+  return t;
 }
 
 __device__ __forceinline__ void named_barrier_sync(int id, int nthreads) {

@@ -77,7 +77,7 @@ __device__ __forceinline__ void mma16816(float (&d)[4], const uint32_t (&a)[4], 
 
 __global__ void __launch_bounds__(kT, 2)
 wgrad0_mma_kernel(const __grid_constant__ CUtensorMap tmX, const __nv_bfloat16* __restrict__ g,
-                  const uint8_t* __restrict__ amax, float* __restrict__ dW, int B, int H, int W, int Hp, int Wp) {
+                  const uint8_t* __restrict__ amax, float* __restrict__ ws, int B, int H, int W, int Hp, int Wp) {
   extern __shared__ __align__(1024) uint8_t sm[];
   uint8_t* ring = sm;
   uint8_t* gst = ring + kRing * kSlot;
@@ -241,19 +241,12 @@ wgrad0_mma_kernel(const __grid_constant__ CUtensorMap tmX, const __nv_bfloat16* 
   __syncthreads();
   for (int idx = tid; idx < 28 * 32; idx += kT) {
     const int row = idx >> 5, co = idx & 31;
-    int src, out_row;
-    if (row < 27) {
-      const int r = row / 9, m = row - r * 9, q = m / 3, ci = m - q * 3;
-      src = (r * 16 + m) * kPartStride + co;
-      out_row = (r * 3 + q) * 16 + ci;                       // dW32 rows: tap * CK + ci
-    } else {
-      src = 48 * kPartStride + co;
-      out_row = 9 * 16;                                      // bias row
-    }
+    // partial row = tap * 3 + ci (as in wgrad0_reduce_kernel), 27 = bias
+    const int src = row < 27 ? ((row / 9) * 16 + row % 9) * kPartStride + co : 48 * kPartStride + co;
     float v = 0.f;
 #pragma unroll
     for (int w = 0; w < 8; ++w) v += part[w * kPart + src];
-    atomicAdd(&dW[out_row * 32 + co], v);
+    ws[(size_t)blockIdx.x * kWgrad0Part + idx] = v;
   }
 }
 
@@ -290,8 +283,31 @@ bool wgrad0_mma_supported(int W, int Wp, int CK, int Ci, int Co) {
   return on && CK == 16 && Ci <= 3 && Co == 32 && W <= 256 && (W & 1) == 0 && Wp <= kPx && Wp >= 1;
 }
 
-void wgrad0_mma(const void* X, const void* g, const uint8_t* amax, float* dW, int B, int H, int W, int Hp, int Wp,
-                cudaStream_t st) {
+// dW[out_row(i) * 32 + co] += sum over CTAs p (in order) of ws[p][i]: the same bits on every run, unlike fp32 atomics
+__global__ void __launch_bounds__(256) wgrad0_reduce_kernel(const float* __restrict__ ws, int parts, float* __restrict__ dW) {
+  __shared__ float red[256];
+  const float s = sum_partials(ws, parts, kWgrad0Part, red);
+  const int i = blockIdx.x * 32 + threadIdx.x;
+  if (threadIdx.x >= 32 || i >= kWgrad0Part) return;
+  const int row = i >> 5, co = i & 31;
+  const int out_row = row < 27 ? (row / 3) * 16 + (row % 3) : 9 * 16;     // dW32 rows: tap*CK + ci, bias at 9*CK
+  dW[out_row * 32 + co] += s;
+}
+
+int wgrad0_parts(int B, int Hp) {
+  int dev = 0, sms = 0;
+  cudaGetDevice(&dev);
+  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+  return sms * 2 < B * Hp ? sms * 2 : B * Hp;
+}
+
+void wgrad0_reduce(const float* ws, int parts, float* dW, cudaStream_t st) {
+  wgrad0_reduce_kernel<<<(kWgrad0Part + 31) / 32, 256, 0, st>>>(ws, parts, dW);
+  hefl::cuda::note_launch();
+}
+
+void wgrad0_mma(const void* X, const void* g, const uint8_t* amax, float* dW, float* ws, int B, int H, int W, int Hp,
+                int Wp, cudaStream_t st) {
   static int sms = 0;
   if (!sms) {
     int dev = 0;
@@ -301,11 +317,11 @@ void wgrad0_mma(const void* X, const void* g, const uint8_t* amax, float* dW, in
     cudaFuncSetAttribute(wgrad0_mma_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, 100);
   }
   const CUtensorMap tmX = make_row_map(X, (uint64_t)B * H * (W / 2), (uint32_t)(W / 2));
-  int grid = sms * 2;
-  if (grid > B * Hp) grid = B * Hp;
-  launch_pdl(wgrad0_mma_kernel, dim3(grid), dim3(kT), kSmem, st, tmX, reinterpret_cast<const __nv_bfloat16*>(g), amax, dW,
+  const int grid = wgrad0_parts(B, Hp);
+  launch_pdl(wgrad0_mma_kernel, dim3(grid), dim3(kT), kSmem, st, tmX, reinterpret_cast<const __nv_bfloat16*>(g), amax, ws,
              B, H, W, Hp, Wp);
   hefl::cuda::note_launch();
+  wgrad0_reduce(ws, grid, dW, st);
 }
 
 }  // namespace nn

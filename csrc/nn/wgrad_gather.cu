@@ -6,9 +6,8 @@
 //     dW[r,s,ci,co] = sum over windows  g[window,co] * X[argmax_pos(window,co) + (r,s), ci]
 // is a gather with 27 MACs per (window, channel) instead of a dense GEMM over 4x as many pixels padded to
 // 16 channels. The tensor-core path spent 47 us (unpool) + 88 us (wgrad) on this layer; the position
-// depends on the channel, so the work is not GEMM-shaped — it runs on the FP32 pipes with the sm_100
-// mixed-precision FMA (fma.rn.f32.bf16 -> FHFMA.BF16: bf16 operands read from register halves, fp32
-// accumulate, so the staged bf16 pixels need no unpack instructions):
+// depends on the channel, so the work is not GEMM-shaped — it runs on the FP32 pipes (bf16 operands widened
+// to fp32 by a shift, fp32 FMA):
 //   * lane = output channel (Co = 32), a warp walks the windows of one pooled row;
 //   * the 4 input rows under a pooled row are staged once per strip in shared memory as 4 x bf16 per pixel
 //     (row pitch padded by 16 B so the 4 candidate positions of a window hit distinct banks). Shared-memory
@@ -16,8 +15,8 @@
 //     wavefronts and the kernel ran slower than the tensor-core path (measured); LDS.64 halves that;
 //   * g / argmax of all the warp's windows of the strip are fetched up front (16 loads in flight per lane);
 //   * the next strip's rows are prefetched into registers while the current strip is processed;
-//   * 27 + 1 (bias) accumulators per lane, reduced across warps in shared memory, then one fp32 RED per
-//     CTA and element into the split-K buffer the tensor-core wgrad kernels use.
+//   * 27 + 1 (bias) accumulators per lane, reduced across warps in shared memory in warp order, then one
+//     partial per CTA, added into the split-K buffer in CTA order (wgrad0_reduce).
 // Reference semantics: Keras Conv2D/MaxPooling2D backward of the first block (FLPyfhelin.py:120-121).
 #include <cuda_bf16.h>
 
@@ -28,10 +27,10 @@
 namespace hefl {
 namespace nn {
 
-// d += a * b with bf16 operands taken straight from 16-bit register halves and an fp32 accumulator
-// (PTX 8.6 mixed-precision fma -> FHFMA.BF16 with .H0/.H1 selectors: no unpack instructions at all)
+// d += a * b with bf16 operands and an fp32 accumulator; a bf16 is the upper half of an fp32, so widening is
+// exact and the single-rounding fp32 FMA gives the same bits as a mixed-precision bf16 FMA
 __device__ __forceinline__ void fhfma(float& d, uint16_t a, uint16_t b) {
-  asm("fma.rn.f32.bf16 %0, %1, %2, %0;" : "+f"(d) : "h"(a), "h"(b));
+  d = fmaf(__uint_as_float((uint32_t)a << 16), __uint_as_float((uint32_t)b << 16), d);
 }
 __device__ __forceinline__ void split16(uint32_t v, uint16_t& lo, uint16_t& hi) {
   asm("mov.b32 {%0, %1}, %2;" : "=h"(lo), "=h"(hi) : "r"(v));
@@ -44,7 +43,7 @@ constexpr int kGatherNJ = 8;          // windows per warp and strip: Wp <= 16 * 
 
 __global__ void __launch_bounds__(kGatherThreads, 2)
 wgrad0_gather_kernel(const __nv_bfloat16* __restrict__ X, const __nv_bfloat16* __restrict__ g,
-                     const uint8_t* __restrict__ amax, float* __restrict__ dW, int B, int H, int W, int Hp, int Wp) {
+                     const uint8_t* __restrict__ amax, float* __restrict__ ws, int B, int H, int W, int Hp, int Wp) {
   extern __shared__ __align__(16) uint8_t sm[];
   const int rowb = W * 8 + 16;
   const int bufb = 4 * rowb;
@@ -131,37 +130,37 @@ wgrad0_gather_kernel(const __nv_bfloat16* __restrict__ X, const __nv_bfloat16* _
     buf ^= 1;
   }
 
-  // cross-warp reduction, then one RED per element and CTA
+  // cross-warp reduction in warp order (a fixed summation order: the same bits on every run), then this CTA's
+  // partial; wgrad0_reduce adds the partials of all CTAs in CTA order
+#pragma unroll 1
+  for (int w = 0; w < kGatherWarps; ++w) {
+    if (warp == w) {
 #pragma unroll
-  for (int t = 0; t < 9; ++t) {
-    atomicAdd(&red[(t * 3 + 0) * 32 + lane], acc[t][0]);
-    atomicAdd(&red[(t * 3 + 1) * 32 + lane], acc[t][1]);
-    atomicAdd(&red[(t * 3 + 2) * 32 + lane], acc[t][2]);
+      for (int t = 0; t < 9; ++t) {
+        red[(t * 3 + 0) * 32 + lane] += acc[t][0];
+        red[(t * 3 + 1) * 32 + lane] += acc[t][1];
+        red[(t * 3 + 2) * 32 + lane] += acc[t][2];
+      }
+      red[27 * 32 + lane] += accb;
+    }
+    __syncthreads();
   }
-  atomicAdd(&red[27 * 32 + lane], accb);
-  __syncthreads();
-  for (int i = threadIdx.x; i < 28 * 32; i += kGatherThreads) {
-    const int row = i >> 5, co = i & 31;
-    const int out_row = row < 27 ? (row / 3) * 16 + (row % 3) : 9 * 16;     // dW32 rows: tap*CK + ci, bias at 9*CK
-    atomicAdd(&dW[out_row * 32 + co], red[i]);
-  }
+  for (int i = threadIdx.x; i < kWgrad0Part; i += kGatherThreads) ws[(size_t)blockIdx.x * kWgrad0Part + i] = red[i];
 }
 
 bool wgrad0_gather_supported(int W, int Wp, int CK, int Ci, int Co) {
   return CK == 16 && Ci <= 3 && Co == 32 && 4 * W <= kGatherPre * kGatherThreads && Wp <= kGatherWarps * kGatherNJ;
 }
 
-void wgrad0_gather(const void* X, const void* g, const uint8_t* amax, float* dW, int B, int H, int W, int Hp, int Wp,
-                   cudaStream_t st) {
+void wgrad0_gather(const void* X, const void* g, const uint8_t* amax, float* dW, float* ws, int B, int H, int W, int Hp,
+                   int Wp, cudaStream_t st) {
   const int smem = 2 * 4 * (W * 8 + 16) + 28 * 32 * 4;
-  static int sms = 0;
-  if (!sms) { int dev = 0; cudaGetDevice(&dev); cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev); }
-  int grid = sms * 2;
-  if (grid > B * Hp) grid = B * Hp;
+  const int grid = wgrad0_parts(B, Hp);
   cudaFuncSetAttribute(wgrad0_gather_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
   launch_pdl(wgrad0_gather_kernel, dim3(grid), dim3(kGatherThreads), smem, st, reinterpret_cast<const __nv_bfloat16*>(X),
-             reinterpret_cast<const __nv_bfloat16*>(g), amax, dW, B, H, W, Hp, Wp);
+             reinterpret_cast<const __nv_bfloat16*>(g), amax, ws, B, H, W, Hp, Wp);
   hefl::cuda::note_launch();
+  wgrad0_reduce(ws, grid, dW, st);
 }
 
 }  // namespace nn

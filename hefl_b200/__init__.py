@@ -1,10 +1,10 @@
-"""hefl_b200 — B200-native encrypted federated learning engine.
+"""hefl_b200 — H100-native encrypted federated learning engine.
 
-Packed-CKKS FedAvg with hand-written sm_100a kernels (NTT/INTT, CKKS codec, fused
-encrypt/decrypt, fused ciphertext all-reduce over NVLink peer memory, tcgen05 implicit-GEMM
+Packed-CKKS FedAvg with hand-written sm_90a kernels (NTT/INTT, CKKS codec, fused
+encrypt/decrypt, fused ciphertext all-reduce over NVLink peer memory, tensor-core implicit-GEMM
 convolution), plus a compatibility surface that keeps the reference's ``FLPyfhelin`` function
 names, Pyfhel 2.3.1-style key generation and pickle file layout
-(/root/reference/FLPyfhelin.py).
+(the reference's FLPyfhelin.py).
 
 Sub-packages: ``he`` (scheme), ``ops`` (kernel wrappers), ``models`` (CNNs), ``parallel``
 (symmetric memory + collectives), ``fl`` (round loop), ``compat`` (Pyfhel / FLPyfhelin

@@ -1,7 +1,7 @@
 """In-tree build of the native library ``hefl_b200/_native.so``.
 
-* ``.cu`` files are compiled by nvcc for sm_100a only (``-gencode arch=compute_100a,
-  code=sm_100a -lineinfo``) and do **not** include PyTorch headers (seconds per file);
+* ``.cu`` files are compiled by nvcc for sm_90a only (``-gencode arch=compute_90a,
+  code=sm_90a -lineinfo``) and do **not** include PyTorch headers (seconds per file);
 * ``*_bindings.cpp`` files are compiled by g++ against the PyTorch headers and register
   ``torch.ops.hefl.*``;
 * objects are cached by a content hash of (source, headers, flags), so the GPU box, which
@@ -29,12 +29,12 @@ NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 CXX = os.environ.get("HEFL_CXX", "/usr/bin/g++")
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-O3", "-lineinfo", "-std=c++17",
     "--expt-relaxed-constexpr",
     "-Xcompiler", "-fPIC",
     "-Xptxas", "-v",
-] + os.environ.get("HEFL_NVCC_EXTRA", "").split()      # e.g. HEFL_NVCC_EXTRA="-DHEFL_WGRAD_OCC3=1" (experiments)
+] + os.environ.get("HEFL_NVCC_EXTRA", "").split()      # e.g. HEFL_NVCC_EXTRA="-DHEFL_CONV_DEBUG" (experiments)
 
 CUDA_SOURCES = [
     "he/cuda/he_kernels.cu",

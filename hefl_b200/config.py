@@ -60,7 +60,8 @@ class FLConfig:
                                               # model -- the reference's roles: aggregation with get_pk (FLPyfhelin.py:370),
                                               # get_sk only in decrypt (:284). -1: rank 0 generates and hands sk to every
                                               # rank (every client can decrypt; weaker, kept for experiments)
-    deterministic_crypto: bool = False        # tests / debugging ONLY: derive the key pair and every encryption seed from
+    deterministic_crypto: bool = False        # tests, debugging and bench.py (reproducible inputs) ONLY, never a deployment:
+                                              # derive the key pair and every encryption seed from
                                               # ``seed`` (public!) instead of OS entropy, so runs are bit-reproducible
     pairwise_masks: bool = False              # add PRG masks (X25519-agreed pair seeds, +/- per pair) to each client's
                                               # ciphertext before the all-reduce; they cancel in the sum

@@ -94,7 +94,7 @@ class FederatedRunner:
     def _setup_keys(self) -> None:
         cfg = self.cfg
         if cfg.deterministic_crypto:
-            # bit-reproducible runs for tests: everything from the PUBLIC cfg.seed -- never in production
+            # bit-reproducible runs (tests, bench.py): everything from the PUBLIC cfg.seed -- never in a deployment
             sk, self.pk = self.ctx.keygen(seed=cfg.seed)
             self.sk = sk if self.has_sk else None
             return
@@ -234,7 +234,7 @@ class FederatedRunner:
         buf = self.transport.buffer(self.ct_numel)
         # The three stages only overlap if they fit on the chip together: encrypt / decrypt are persistent
         # one-CTA-per-SM kernels and the all-reduce is a copy engine that saturates NVLink from a few SMs, so the
-        # SMs are partitioned for the duration of the pipeline (measured on ResNet-18, 8 GPUs: see profiles/).
+        # SMs are partitioned for the duration of the pipeline (HEFL_PIPE_SPLIT overrides the default split).
         split = None
         if self.world > 1 and dev.type == "cuda" and self.transport.name == "fused":
             sms = torch.cuda.get_device_properties(dev).multi_processor_count

@@ -7,7 +7,7 @@ categorical cross-entropy + accuracy (:141), batch 32 (:33), EarlyStopping on tr
 factor 0.3, floor 1e-6, :187), ModelCheckpoint on best training accuracy (:189-191),
 augmentation shear/zoom/flip and 1/255 rescale (:80-86).
 
-B200 design: parameters, gradients and Adam moments are flat fp32 buffers (``ParamPack``),
+Design: parameters, gradients and Adam moments are flat fp32 buffers (``ParamPack``),
 the optimiser is one fused kernel, the step (forward -> backward -> Adam) is captured in a CUDA
 graph and replayed, the learning-rate scale and step counter live on the device, and losses are
 read back asynchronously (one sync per epoch, not per step). With the tcgen05 engine an epoch is

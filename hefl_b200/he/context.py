@@ -8,7 +8,7 @@ slots, 2 polynomials, L RNS limbs, NTT form), so that FedAvg is one coefficient-
 modular add-reduce (fused with the collective in ``hefl_b200.parallel``) and the 1/K factor
 is folded into the decode scale (SURVEY.md §2.2 X1.h, §7.5).
 
-All heavy lifting is in ``torch.ops.hefl`` (csrc/he): the same calls run the sm_100a
+All heavy lifting is in ``torch.ops.hefl`` (csrc/he): the same calls run the sm_90a
 kernels for CUDA tensors and the host C++ implementation for CPU tensors.
 """
 from __future__ import annotations

@@ -1,6 +1,6 @@
 """ResNet-18 / ResNet-50 (BASELINE.json configs[2], configs[4]) written against plain
 torch.nn so there is no torchvision dependency. BatchNorm(+residual)+ReLU and the global average
-pool run on the fused sm_100a kernels of ``ops/resnet_ops.py`` when activations are NHWC bf16. BatchNorm running statistics are part of the
+pool run on the fused sm_90a kernels of ``ops/resnet_ops.py`` when activations are NHWC bf16. BatchNorm running statistics are part of the
 federated state (Keras ``get_weights`` includes moving mean/variance, FLPyfhelin.py:151)."""
 from __future__ import annotations
 

@@ -1,1 +1,1 @@
-"""Python wrappers around the hand-written sm_100a kernels (torch.ops.hefl.*)."""
+"""Python wrappers around the hand-written sm_90a kernels (torch.ops.hefl.*)."""

@@ -1,18 +1,19 @@
-"""Training engine for the sequential 3x3-conv CNNs on the hand-written sm_100a kernels.
+"""Training engine for the sequential 3x3-conv CNNs on the hand-written sm_90a kernels.
 
 Replaces Keras' ``model.fit`` compute path (FLPyfhelin.py:118-136, :193) for the medical CNN:
 
   input     preprocess_u8 (uint8 -> bf16 NHWC [P,16], 1/255, Philox affine augmentation; layer-1 input
             carries pixels w, w+1, w+2 in its channels) into one of two X0 slots — the trainer stages
             batch i+1 on a side stream while step i runs
-  forward   6 x conv_fwd_pool  (TMA-fed tcgen05 tap GEMMs, bias + ReLU + 2x2 max-pool + 3-bit
-                                arg-max/active code fused in the TMEM epilogue; only pooled tensors
+  forward   6 x conv_fwd_pool  (TMA-fed tensor-core tap GEMMs, bias + ReLU + 2x2 max-pool + 3-bit
+                                arg-max/active code fused in the epilogue; only pooled tensors
                                 reach HBM; layer 1 on the pair-row variant: the whole pooling window
-                                in one TMEM lane)
+                                in one thread)
             head_forward_backward (Dense 128-64-C + softmax CE, forward AND backward, one launch on a
                                    cluster of 8 CTAs)
   backward  unpool_relu / conv_dgrad chain on the main stream (layers 6..2),
-            conv_wgrad (tcgen05, MN-major operands, split-K RED) on a side stream,
+            conv_wgrad (tensor cores, operands read in place, split-K partials added in a fixed order) on a
+            side stream,
             layer 1: wgrad0_gather straight from the pooled gradient (no un-pool, no dY tensor): four
                      masked GEMMs on the tensor cores (wgrad0_mma.cu), FP32-pipe gather as the fallback
   update    conv_grad_finalize + Adam + conv_weight_relayout: layers 2..6 and the head on the side
@@ -43,7 +44,7 @@ def _round_up(x: int, m: int) -> int:
 class MedCNNEngine:
     def __init__(self, model, pack: ParamPack, cfg: FLConfig, device: torch.device):
         if device.type != "cuda":
-            raise RuntimeError("the tcgen05 engine needs a CUDA device (sm_100a)")
+            raise RuntimeError("the tcgen05 engine needs a CUDA device (sm_90a)")
         self.ops = _ext.ops()
         self.ops.set_head_cluster(0 if os.environ.get("HEFL_HEAD_CLUSTER", "1") == "0" else 1)
         self.ops.set_pdl(0 if os.environ.get("HEFL_PDL", "1") == "0" else 1)   # programmatic dependent launch
@@ -78,10 +79,9 @@ class MedCNNEngine:
                        and self.Co[0] == 32)
         # un-pool inside the dgrad epilogue: correct (bit-exact test) but measured 10 us/step SLOWER than the
         # separate un-pool kernels (the epilogue is issue-bound; 4x the stores), so off by default
-        # pair-row forward kernel (both columns of a pooling window in one TMEM lane, conv_tcgen05.cu G1b): on by
-        # default for layer 1, where it reads the same s-packed input and issues the same three MMAs per accumulator
-        # as the tap-GEMM forward (bit-identical outputs, tests). On the small layers it is slower (one 128-window
-        # tile per pooled row: 20.3 vs 16.8 us, 16.2 vs 11.6 us), so HEFL_FWD_PAIR=all is only for experiments.
+        # pair-row forward kernel (both columns of a pooling window in one thread, conv_tcgen05.cu G1b): on by
+        # default for layer 1, where it reads the same s-packed input as the tap-GEMM forward (same outputs, tests).
+        # On the small layers it runs one 128-window tile per pooled row, so HEFL_FWD_PAIR=all is only for experiments.
         mode = os.environ.get("HEFL_FWD_PAIR", "1")
         self.fwd_pair = {"0": 0, "1": 1, "all": self.n}.get(mode, 0)      # number of leading layers that may use it
         self.fuse_unpool = os.environ.get("HEFL_FUSE_UNPOOL", "0") != "0"

@@ -1,4 +1,4 @@
-"""ResNet building blocks on hand-written sm_100a kernels (SURVEY.md K18): training-mode
+"""ResNet building blocks on hand-written sm_90a kernels (SURVEY.md K18): training-mode
 BatchNorm over NHWC bf16 fused with the residual add and ReLU (forward and backward, 5 kernels
 per BN layer and direction instead of cuDNN BN + add + ReLU + their autograd nodes) and global
 average pooling. The convolutions of the ResNets stay on cuDNN (library GEMMs); everything

@@ -1,10 +1,10 @@
-"""ResNet convolutions on the hand-written tcgen05 GEMM kernels (csrc/nn/gemm_tcgen05.cu): 1x1 (any stride, by
+"""ResNet convolutions on the hand-written tensor-core GEMM kernels (csrc/nn/gemm_tcgen05.cu): 1x1 (any stride, by
 sub-sampling first) and 3x3 / pad 1 / stride 1, forward, dgrad and wgrad, bf16 with fp32 accumulation; the 1x1
-forward can run in e4m3 (``kind::f8f6f4``) with per-tensor delayed scaling.
+forward can run in e4m3 (wgmma e4m3) with per-tensor delayed scaling.
 
 Layout: activations are channels_last bf16, i.e. ``[pixels, C]`` matrices. A 3x3 convolution works on a
 zero-padded copy ``[B, H+2, W+2, C]``: tap (r, s) is the same matrix shifted by ``(r-1)*(W+2) + (s-1)`` rows, so
-the nine tap GEMMs accumulate in one TMEM tile with nothing but a different TMA row coordinate (no im2col).
+the nine tap GEMMs accumulate in one register tile with nothing but a different TMA row coordinate (no im2col).
 
 What stays on cuDNN: the 7x7 stem (3 input channels) and the three 3x3 stride-2 convolutions of a ResNet.
 
@@ -64,7 +64,7 @@ class _Conv1x1TC(torch.autograd.Function):
             # block-scaled e4m3 (kind::mxf8f6f4.block_scale): one UE8M0 scale per row and 32 channels, no amax history
             xq, xs = ops.mxfp8_quantize(x2 if x2.is_contiguous() else x2.contiguous())
             wq, ws = ops.mxfp8_quantize(wb)
-            ops.gemm_mxfp8(xq, wq, xs, ws, y2, 0)
+            ops.gemm_mxfp8(xq, wq, xs, ws, y2)
         elif fp8_state is not None and fp8_state != "mx" and Cin % 128 == 0:   # per-tensor delayed scaling (kind::f8f6f4)
             sx, sw = fp8_state
             xq = _fp8._quantize(x2, sx).view(torch.uint8)
@@ -89,7 +89,7 @@ class _Conv1x1TC(torch.autograd.Function):
         if ctx.mx:                                                                              # dX = dY . W, block-scaled
             gq, gs = ops.mxfp8_quantize(g2)
             tq, ts = ops.mxfp8_quantize(wT)
-            ops.gemm_mxfp8(gq, tq, gs, ts, dx2, 0)
+            ops.gemm_mxfp8(gq, tq, gs, ts, dx2)
         else:
             ops.gemm_taps(g2, wT, dx2, Cin, Cout, [], 0, 0, 0, 0, None, None)                   # dX = dY . W
         dw = torch.empty(1, Cout, Cin, dtype=torch.float32, device=gy.device)

@@ -4,7 +4,7 @@ FedAvg's server loop (FLPyfhelin.py:372-381: import each client's pickle, ``enc 
 scalar ciphertext) is a coefficient-wise modular sum over clients. Three interchangeable
 transports implement it behind one interface:
 
-* ``FusedTransport``   — the product: one sm_100a kernel that pulls peer tiles over NVLink,
+* ``FusedTransport``   — the product: one sm_90a kernel that pulls peer tiles over NVLink,
   adds, reduces mod q_l and pushes/broadcasts the result (csrc/comm/allreduce_modq.cu).
 * ``CollectiveTransport`` — the baseline the product must beat: ``all_reduce(int64, SUM)``
   through NCCL (or gloo on CPU) followed by a separate mod-q kernel (SURVEY.md K2).

@@ -1,4 +1,4 @@
-"""Sample SM clocks and throttle reasons during a timed region (B200_PROFILING.md)."""
+"""Sample SM clocks and throttle reasons during a timed region."""
 from __future__ import annotations
 
 import statistics

@@ -416,7 +416,7 @@ def test_engine_gradients_match_autograd(gather, fuse):
         cos = F.cosine_similarity(a, b, dim=0).item() if b.norm() > 0 else 1.0
         rels[key] = (round(rel, 4), round(cos, 5))
     print("engine vs autograd, (max rel err, cosine) per tensor:", rels)
-    # measured on B200 (bf16 activations and gradients through six conv + pool blocks against fp32 autograd on the
+    # measured on the GPU (bf16 activations and gradients through six conv + pool blocks against fp32 autograd on the
     # same bf16-rounded tensors): cosine 0.9955 (first convolution) ... 0.9995 (last) ... 1.0000 (dense layers);
     # max-norm relative error 0.137 / 0.081 / 0.065 / 0.052 / 0.046 / 0.036 for the six convolutions, < 0.08 for
     # the first dense layer, < 0.001 beyond. The verdict's 0.05 holds from the fourth block on; the early layers

@@ -1,5 +1,5 @@
-"""GPU tests: every sm_100a HE kernel against its host C++ twin (bit-exact for integer
-kernels) and the CKKS pipeline end to end. Run on the B200 box: pytest -m gpu."""
+"""GPU tests: every sm_90a HE kernel against its host C++ twin (bit-exact for integer
+kernels) and the CKKS pipeline end to end. Run on an H100: pytest -m gpu."""
 import pytest
 import torch
 

@@ -47,7 +47,7 @@ def test_three_epochs_of_the_bf16_engine_track_fp32_pytorch():
     # accuracy is a thresholded quantity (observed 0.512 vs 0.512 on one box, 0.574 vs 0.512 on another, with the
     # losses 0.6457 / 0.6497 both times); it only has to be in the same regime
     assert abs(h_e[0].accuracy - h_r[0].accuracy) <= 0.15
-    # measured on B200: losses (0.6454, 0.1647, 0.0000) vs fp32 (0.6498, 0.1791, 0.0000), accuracy 1.0 / 1.0 from
+    # measured on the GPU: losses (0.6454, 0.1647, 0.0000) vs fp32 (0.6498, 0.1791, 0.0000), accuracy 1.0 / 1.0 from
     # epoch 2 on both; the trained weights stay close (bf16 activations, fp32 master weights and moments): cosine 0.9963
     cos = torch.nn.functional.cosine_similarity(pack_e.flat, pack_r.flat, dim=0).item()
     assert cos > 0.99

@@ -1,5 +1,5 @@
 """Multi-process tests. CPU (gloo, world 2) checks the host-side transport logic here;
-the GPU variants run the fused NVLink kernel across real devices on the B200 box."""
+the GPU variants run the fused NVLink kernel across real devices on an H100."""
 import json
 import os
 import subprocess

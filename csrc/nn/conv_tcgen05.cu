@@ -9,7 +9,8 @@
 //   conv_fwd_pool : per CTA tile = 2 image rows x 128 columns (two accumulators) so that the
 //                   epilogue does bias + ReLU + 2x2 max-pool + argmax straight from the accumulators (vertical
 //                   max in-thread across the two accumulators, horizontal max by one shuffle) and
-//                   writes only the pooled tensor (4x less HBM traffic than the conv output).
+//                   writes only the pooled tensor (4x less HBM traffic than the conv output). Maps of even
+//                   height and width <= 64 pack 128 / W row pairs into one tile instead (G1).
 //   conv_dgrad    : dX[m,:] = sum_taps dY[m - off, :] * W[r,s]   (same kernel, negative offsets,
 //                   plain bf16 store).
 //   conv_wgrad    : dW[r,s] = sum_m X[m+off,:]^T dY[m,:]. Both operands are consumed in their
@@ -79,6 +80,32 @@ static CUtensorMap make_map(const void* ptr, uint64_t inner, uint64_t outer, uin
   return m;
 }
 
+// NHWC bf16 activation [B*H rows][W][C] viewed as image-row pairs: 4-D {C, W, row parity, B*H/2 pairs};
+// box = {box_c, W, 1, box_pairs}, i.e. box_pairs * W consecutive smem rows of one parity (pairs past the end
+// zero-fill).
+static CUtensorMap make_pair_row_map(const void* ptr, uint64_t C, uint64_t W, uint64_t pairs, uint32_t box_c,
+                                     uint32_t box_pairs) {
+  CUtensorMap m;
+  cuuint64_t dims[4] = {C, W, 2, pairs};
+  cuuint64_t strides[3] = {C * 2, W * C * 2, 2 * W * C * 2};
+  cuuint32_t box[4] = {box_c, (cuuint32_t)W, 1, box_pairs};
+  cuuint32_t estr[4] = {1, 1, 1, 1};
+  const uint32_t inner_bytes = box_c * 2;
+  CUtensorMapSwizzle sw = inner_bytes == 128 ? CU_TENSOR_MAP_SWIZZLE_128B
+                          : inner_bytes == 64 ? CU_TENSOR_MAP_SWIZZLE_64B
+                                              : CU_TENSOR_MAP_SWIZZLE_32B;
+  CUresult r = encode_fn()(&m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, const_cast<void*>(ptr), dims, strides, box,
+                           estr, CU_TENSOR_MAP_INTERLEAVE_NONE, sw, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
+                           CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (r != CUDA_SUCCESS) {
+    char buf[256];
+    snprintf(buf, sizeof(buf), "cuTensorMapEncodeTiled(4d) failed (%d): C=%llu W=%llu pairs=%llu box_pairs=%u", (int)r,
+             (unsigned long long)C, (unsigned long long)W, (unsigned long long)pairs, box_pairs);
+    throw std::runtime_error(buf);
+  }
+  return m;
+}
+
 static int num_sms() {
   static int n = 0;
   if (!n) {
@@ -97,6 +124,12 @@ static int num_sms() {
 // is loaded ONCE per tile and all 9 taps address shifted windows of it:
 //   forward : tile = 2 image rows x 128 columns; 4 halo segments (rows h..h+3) of 130 pixels;
 //             accumulator j (row h+j), tap (r,s) reads segment j+r at row offset s.
+//   forward, row-packed (even H and W <= 64): a 2 x 128 tile of a narrow map would be mostly pixels of the
+//             following rows whose results are discarded, so a tile is instead R = 128 / W image-row PAIRS
+//             (pairs q0 .. q0+R-1, pair q = rows 2q, 2q+1 of the [B*H] row axis). Segment j holds R*W rows:
+//             GEMM row m = k*W + w is column w of row 2(q0+k) + j (4-D tensor map, one TMA box per segment).
+//             The accumulators, taps and row offsets are the ones above, so every output gets the same MMAs
+//             in the same order (bit-identical results) on a fraction of the tiles.
 //   dgrad   : tile = 128 consecutive pixels; 3 segments starting at m0 - r*W - 2; tap (r,s)
 //             reads segment r at row offset 2 - s.
 // L2->SM traffic drops from 9 tap tiles to ~2 (fwd) / ~3 (dgrad) tiles per output tile.
@@ -104,7 +137,8 @@ static int num_sms() {
 struct TapGemmArgs {
   int B, H, W;          // input grid of the A matrix
   int Hp, Wp;           // pooled output grid (POOL)
-  int tiles_w;          // column tiles per row pair (POOL)
+  int tiles_w;          // column tiles per row pair (POOL, column tiling)
+  int pairs_per_tile;   // POOL: R image-row pairs per tile when row-packed, 0 = 2 rows x 128 columns
   int num_tiles;
   int P;                // B*H*W
   int co_total;         // output channels of the layer (CO per CTA column block = blockIdx.y)
@@ -123,7 +157,13 @@ struct TapGemmArgs {
   // n, d < 2^16 with magic = ceil(2^32 / d) (the epilogue warps spent ~40 of their ~100 per-tile set-up
   // instructions in two software divisions)
   uint32_t magic_per_img, magic_tiles_w;
+  uint32_t magic_w, magic_half_h;     // row-packed: GEMM row -> (pair, column), pair -> (image, pooled row)
 };
+
+// magic for fast_div(n, d) when every n is below n_max; 0 = divide at run time
+static uint32_t div_magic(int n_max, int d) {
+  return (n_max < 65536 && d > 1 && d < 65536) ? (uint32_t)((0x100000000ull + d - 1) / d) : 0u;
+}
 
 __device__ __forceinline__ int fast_div(int n, int d, uint32_t magic) {
   if (d == 1) return n;
@@ -210,28 +250,36 @@ tap_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
       int buf = 0;
       uint32_t phase = 0;
       for (int t = blockIdx.x; t < a.num_tiles; t += gridDim.x) {
-        int base, seg_stride;
-        if (POOL) {
-          const int per_img = a.Hp * a.tiles_w;
-          const int b = fast_div(t, per_img, a.magic_per_img);
-          const int rem = t - b * per_img;
-          const int hp = fast_div(rem, a.tiles_w, a.magic_tiles_w);
-          const int tw = rem - hp * a.tiles_w;
-          base = (b * a.H + 2 * hp) * a.W + tw * 128;
-          seg_stride = a.W;                      // segment j = image row h + j
-        } else {
-          base = t * 128 - 2;
-          seg_stride = -a.W;                     // segment r starts at m0 - r*W - 2
-        }
         mbar_wait(&empty[buf], phase ^ 1);
+        uint8_t* dst = sA + buf * Cfg::HALO;
 #ifdef HEFL_CONV_DEBUG
         if (a.dbg & 1) {
           mbar_arrive(&full[buf]);
         } else
 #endif
-        {
+        if (POOL && a.pairs_per_tile) {
+          // segment sg = row parity sg & 1 of pairs q0 + (sg >> 1) ..: rows 2(q0+k) + sg; bytes actually boxed
+          const int q0 = t * a.pairs_per_tile;
+          mbar_expect_tx(&full[buf], Cfg::NKB * Cfg::NSEG * a.pairs_per_tile * a.W * RB);
+          for (int kb = 0; kb < Cfg::NKB; ++kb)
+            for (int sg = 0; sg < Cfg::NSEG; ++sg)
+              tma_load_4d(dst + (kb * Cfg::NSEG + sg) * Cfg::SEG_BYTES, &tmA, kb * Cfg::KB, 0, sg & 1, q0 + (sg >> 1),
+                          &full[buf]);
+        } else {
+          int base, seg_stride;
+          if (POOL) {
+            const int per_img = a.Hp * a.tiles_w;
+            const int b = fast_div(t, per_img, a.magic_per_img);
+            const int rem = t - b * per_img;
+            const int hp = fast_div(rem, a.tiles_w, a.magic_tiles_w);
+            const int tw = rem - hp * a.tiles_w;
+            base = (b * a.H + 2 * hp) * a.W + tw * 128;
+            seg_stride = a.W;                      // segment j = image row h + j
+          } else {
+            base = t * 128 - 2;
+            seg_stride = -a.W;                     // segment r starts at m0 - r*W - 2
+          }
           mbar_expect_tx(&full[buf], Cfg::HALO);
-          uint8_t* dst = sA + buf * Cfg::HALO;
           for (int kb = 0; kb < Cfg::NKB; ++kb)
             for (int sg = 0; sg < Cfg::NSEG; ++sg)
               tma_load_2d(dst + (kb * Cfg::NSEG + sg) * Cfg::SEG_BYTES, &tmA, kb * Cfg::KB, base + sg * seg_stride,
@@ -252,6 +300,32 @@ tap_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
     for (int t = blockIdx.x; t < a.num_tiles; t += gridDim.x) {
       mbar_wait(&full[buf], phase);
       const uint32_t a_base = smem_u32(sA + buf * Cfg::HALO);
+      // POOL: pooled pixel of this lane's conv column (window = this lane and lane ^ 1) and whether it is stored
+      int pix = 0;
+      bool writer = false;
+      if (POOL) {
+        if (a.pairs_per_tile) {
+          // W even: m and w have the same parity, so lane ^ 1 is the other column of the same window
+          const int m = qd * 32 + lane;
+          const int k = fast_div(m, a.W, a.magic_w);
+          const int w = m - k * a.W;
+          const int half_h = a.H >> 1;
+          const int q = t * a.pairs_per_tile + k;
+          const int b = fast_div(q, half_h, a.magic_half_h);
+          const int hp = q - b * half_h;                      // the last pair of an image is never a pooled row
+          writer = k < a.pairs_per_tile && b < a.B && hp < a.Hp && (w >> 1) < a.Wp;
+          pix = (b * a.Hp + hp) * a.Wp + (w >> 1);
+        } else {
+          const int per_img = a.Hp * a.tiles_w;
+          const int b = fast_div(t, per_img, a.magic_per_img);
+          const int rem = t - b * per_img;
+          const int hp = fast_div(rem, a.tiles_w, a.magic_tiles_w);
+          const int tw = rem - hp * a.tiles_w;
+          const int wp = (tw * 128 + qd * 32 + lane) >> 1;   // conv-output column of this thread, halved
+          writer = wp < a.Wp;
+          pix = (b * a.Hp + hp) * a.Wp + wp;
+        }
+      }
 #pragma unroll 1
       for (int g = 0; g < CO / 16 / Cfg::NG; ++g) {
         float acc[Cfg::NACC][Cfg::NG][2][4];
@@ -308,20 +382,13 @@ tap_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
           if (a.dbg & 4) continue;
 #endif
           if (POOL) {
-            const int per_img = a.Hp * a.tiles_w;
-            const int b = fast_div(t, per_img, a.magic_per_img);
-            const int rem = t - b * per_img;
-            const int hp = fast_div(rem, a.tiles_w, a.magic_tiles_w);
-            const int tw = rem - hp * a.tiles_w;
-            const int col = tw * 128 + qd * 32 + lane;           // conv-output column of this thread
-            const int wp = col >> 1;
-            const bool writer = wp < a.Wp;
             const bool odd = (lane & 1) != 0;
+            const int c0 = blockIdx.y * CO + ch * 8 + (odd ? 4 : 0);   // channel of the layer's co_total
             float v0[8], v1[8];
             frag_rows(scr, acc[0][i][0], acc[0][i][1], lane, v0);
             frag_rows(scr, acc[Cfg::NACC - 1][i][0], acc[Cfg::NACC - 1][i][1], lane, v1);
             // the two lanes of a window split the 8 channels: even lane -> 0..3, odd lane -> 4..7
-            const float4 bq = __ldg(reinterpret_cast<const float4*>(a.bias + ch * 8 + (odd ? 4 : 0)));
+            const float4 bq = __ldg(reinterpret_cast<const float4*>(a.bias + c0));
             const float bias4[4] = {bq.x, bq.y, bq.z, bq.w};
             // max over the two image rows on the raw accumulators (bias + ReLU commute with max)
             uint32_t vbits = 0;                                 // 1 = lower image row wins
@@ -350,7 +417,7 @@ tap_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
               x[q] = y > 0.f ? y : 0.f;
             }
             if (writer) {
-              const size_t o = ((size_t)(b * a.Hp + hp) * a.Wp + wp) * CO + ch * 8 + (odd ? 4 : 0);
+              const size_t o = (size_t)pix * a.co_total + c0;
               *reinterpret_cast<uint2*>(a.out + o) = make_uint2(pack_bf16x2(x[0], x[1]), pack_bf16x2(x[2], x[3]));
               if (a.argmax) *reinterpret_cast<uint32_t*>(a.argmax + o) = idx;
             }
@@ -398,7 +465,10 @@ tap_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
 template <int CK, int CO, bool POOL, int TS = 3>
 static void launch_tap_gemm(const __nv_bfloat16* A, const __nv_bfloat16* Wt, TapGemmArgs a, cudaStream_t st) {
   using Cfg = TapGemmCfg<CK, CO, POOL, TS>;
-  const CUtensorMap tmA = make_map(A, CK, (uint64_t)a.P, (uint64_t)CK * 2, Cfg::KB, Cfg::SEG_ROWS);
+  const CUtensorMap tmA =
+      (POOL && a.pairs_per_tile)
+          ? make_pair_row_map(A, CK, (uint64_t)a.W, (uint64_t)a.B * a.H / 2, Cfg::KB, (uint32_t)a.pairs_per_tile)
+          : make_map(A, CK, (uint64_t)a.P, (uint64_t)CK * 2, Cfg::KB, Cfg::SEG_ROWS);
   const CUtensorMap tmW = make_map(Wt, CK, (uint64_t)Cfg::NTAP * a.co_total, (uint64_t)CK * 2, Cfg::KB, CO);
   auto kern = tap_gemm_kernel<CK, CO, POOL, TS>;
   cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM);
@@ -428,30 +498,42 @@ void conv_fwd_pool(const void* X, const void* Wf, const float* bias, void* out, 
 #ifdef HEFL_CONV_DEBUG
   a.dbg = g_dbg;
 #endif
+  if (!((CK == 16 && CO == 32) || (CK == 32 && (CO == 32 || CO == 64)) || (CK == 64 && (CO == 64 || CO == 128))))
+    throw std::runtime_error("conv_fwd_pool: unsupported (CK, CO)");
   a.B = B; a.H = H; a.W = W;
   a.Hp = (H - 2) / 2; a.Wp = (W - 2) / 2;
-  a.tiles_w = (2 * a.Wp + 127) / 128;
-  a.num_tiles = B * a.Hp * a.tiles_w;
-  {
-    const int per_img = a.Hp * a.tiles_w;
-    const bool ok = a.num_tiles < 65536 && per_img > 1 && per_img < 65536;
-    a.magic_per_img = ok ? (uint32_t)((0x100000000ull + per_img - 1) / per_img) : 0u;
-    a.magic_tiles_w = (ok && a.tiles_w > 1) ? (uint32_t)((0x100000000ull + a.tiles_w - 1) / a.tiles_w) : 0u;
+  if (W % 2 == 0 && H % 2 == 0 && W <= 64) {
+    // row-packed tiles (G1 above): R = 128 / W pairs of image rows per tile instead of 2 rows x 128 columns;
+    // even H keeps every pair inside one image, even W keeps both columns of a pooling window in one lane pair
+    a.pairs_per_tile = 128 / W;
+    const int pairs = B * H / 2;
+    a.num_tiles = (pairs + a.pairs_per_tile - 1) / a.pairs_per_tile;
+    a.magic_w = div_magic(128, W);
+    a.magic_half_h = div_magic(a.num_tiles * a.pairs_per_tile, H / 2);
+  } else {
+    a.tiles_w = (2 * a.Wp + 127) / 128;
+    a.num_tiles = B * a.Hp * a.tiles_w;
+    a.magic_per_img = div_magic(a.num_tiles, a.Hp * a.tiles_w);
+    a.magic_tiles_w = div_magic(a.num_tiles, a.tiles_w);
   }
   a.P = B * H * W;
   a.co_total = CO;
   a.bias = bias;
   a.out = reinterpret_cast<__nv_bfloat16*>(out);
   a.argmax = argmax;
+  // Output-channel blocks (blockIdx.y) while the tiles alone would leave SMs idle (the late, small layers): a CTA
+  // then holds and multiplies 1/ny of the weights, and the input tile is read once per block (from L2).
+  int co_blk = CO;
+  while (co_blk % 64 == 0 && a.num_tiles * (CO / co_blk) < num_sms()) co_blk /= 2;
   const auto* x = reinterpret_cast<const __nv_bfloat16*>(X);
   const auto* w = reinterpret_cast<const __nv_bfloat16*>(Wf);
-  if (CK == 16 && CO == 32 && spack) launch_tap_gemm<16, 32, true, 1>(x, w, a, st);
-  else if (CK == 16 && CO == 32) launch_tap_gemm<16, 32, true>(x, w, a, st);
-  else if (CK == 32 && CO == 32) launch_tap_gemm<32, 32, true>(x, w, a, st);
-  else if (CK == 32 && CO == 64) launch_tap_gemm<32, 64, true>(x, w, a, st);
-  else if (CK == 64 && CO == 64) launch_tap_gemm<64, 64, true>(x, w, a, st);
-  else if (CK == 64 && CO == 128) launch_tap_gemm<64, 128, true>(x, w, a, st);
-  else throw std::runtime_error("conv_fwd_pool: unsupported (CK, CO)");
+  if (CK == 16 && spack) launch_tap_gemm<16, 32, true, 1>(x, w, a, st);
+  else if (CK == 16) launch_tap_gemm<16, 32, true>(x, w, a, st);
+  else if (CK == 32 && co_blk == 32) launch_tap_gemm<32, 32, true>(x, w, a, st);
+  else if (CK == 32) launch_tap_gemm<32, 64, true>(x, w, a, st);
+  else if (co_blk == 32) launch_tap_gemm<64, 32, true>(x, w, a, st);
+  else if (co_blk == 64) launch_tap_gemm<64, 64, true>(x, w, a, st);
+  else launch_tap_gemm<64, 128, true>(x, w, a, st);
 }
 
 void conv_dgrad(const void* dY, const void* Wd, void* dX, int B, int H, int W, int CK, int CO, const uint8_t* up_amax,

@@ -83,6 +83,15 @@ __device__ __forceinline__ void tma_load_3d(void* dst, const CUtensorMap* map, i
       : "memory");
 }
 
+__device__ __forceinline__ void tma_load_4d(void* dst, const CUtensorMap* map, int c0, int c1, int c2, int c3,
+                                            uint64_t* bar) {
+  asm volatile(
+      "cp.async.bulk.tensor.4d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3, %4, %5}], [%6];"
+      ::"r"(smem_u32(dst)), "l"(reinterpret_cast<uint64_t>(map)), "r"(c0), "r"(c1), "r"(c2), "r"(c3),
+        "r"(smem_u32(bar))
+      : "memory");
+}
+
 // ---- warp-level tensor-core MMA on TMA-written shared-memory tiles (sm_90) ---------------------
 // TMA writes a tile with a swizzle span of SW bytes (32, 64 or 128, equal to the tile's row length): the 16-byte
 // chunk index inside a span is XORed with address bits 7.. . The pattern is a function of the absolute shared-memory

@@ -22,6 +22,7 @@ namespace hefl {
 namespace cuda {
 
 using namespace hefl::dev2;
+using namespace hefl::sm90;
 
 namespace {
 
@@ -299,37 +300,14 @@ __global__ void tensor3_kernel(const uint64_t* __restrict__ A, const uint64_t* _
   }
 }
 
-int sms() {
-  static int n = 0;
-  if (!n) {
-    int dev = 0;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
-  }
-  return n;
-}
-
-template <int LOGN>
-unsigned corr_for(int qbits) {
-  constexpr int NP = num_passes(LOGN);
-  const unsigned cands[3] = {0u, 1u << 1, (1u << (NP - 1)) - 1u};
-  for (int i = 0; i < 3; ++i) {
-    const long long worst = inv_bound_max<LOGN>(4, cands[i]);
-    int wb = 0;
-    while ((1ll << wb) < worst) ++wb;
-    if (wb + qbits <= 63) return cands[i];
-  }
-  return ~0u;
-}
-
 template <int LOGN>
 bool launch_rescale(const RescaleArgs& a, int qbits, cudaStream_t st) {
   constexpr int NP = num_passes(LOGN);
   constexpr int POLYS = (1 << unit_log(LOGN)) >> LOGN;
   const int smem = 2 * unit_bytes(LOGN);
   const int64_t units = (a.rows + POLYS - 1) / POLYS;
-  const int grid = (int)std::min<int64_t>(units, sms());
-  const unsigned corr = corr_for<LOGN>(qbits);
+  const int grid = (int)std::min<int64_t>(units, device_sm_count());
+  const unsigned corr = pick_corr<LOGN>(qbits);
   auto go = [&](auto k) {
     cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
     k<<<grid, kThreads, smem, st>>>(a);
@@ -346,7 +324,7 @@ void launch_keyswitch(const KsArgs& a, cudaStream_t st) {
   constexpr int POLYS = (1 << unit_log(LOGN)) >> LOGN;
   const int smem = 3 * unit_bytes(LOGN);
   const int64_t units = ((a.C + POLYS - 1) / POLYS) * a.lvl;
-  const int grid = (int)std::min<int64_t>(units, sms());
+  const int grid = (int)std::min<int64_t>(units, device_sm_count());
   auto k = keyswitch2_kernel<LOGN>;
   cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
   k<<<grid, kThreads, smem, st>>>(a);

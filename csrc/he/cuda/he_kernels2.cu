@@ -16,9 +16,6 @@
 #include <cuda.h>
 
 #include <algorithm>
-#include <cstdio>
-#include <stdexcept>
-#include <string>
 
 #include "../kernels.h"
 #include "../philox.h"
@@ -28,6 +25,7 @@ namespace hefl {
 namespace cuda {
 
 using namespace hefl::dev2;
+using namespace hefl::sm90;
 
 namespace {
 
@@ -63,7 +61,7 @@ __device__ __forceinline__ LimbWork limb_work(int nlimbs) {
 // Both CTAs of the cluster: arm the local barrier for the whole table, then issue one half of it
 // as a multicast copy into both CTAs. Must be preceded by a cluster-wide barrier after mbar_init.
 template <int LOGN>
-__device__ __forceinline__ void load_twiddles(uint32_t tw_smem, uint64_t* bar, const CUtensorMap* tmap,
+__device__ __forceinline__ void load_twiddles(uint8_t* tw_smem, uint64_t* bar, const CUtensorMap* tmap,
                                               int table_row0) {
   constexpr int ROWS = tw_rows(LOGN);
   constexpr int HALF = ROWS / 2;                 // <= 256 rows per copy
@@ -134,7 +132,7 @@ ntt2_kernel(const __grid_constant__ CUtensorMap dmap, const __grid_constant__ CU
   if (tid >= kThreads) {
     // ===== producer warp: twiddles, then the load / store ring =====
     if (tid == kThreads) {
-      load_twiddles<LOGN>(sbase + S::kTw, &bars[0], &tmap, table * (N * 16 / 128));
+      load_twiddles<LOGN>(smem + S::kTw, &bars[0], &tmap, table * (N * 16 / 128));
       auto issue_load = [&](int64_t u, int b) {
         const int64_t j0 = u * POLYS;
         const int np = (int)((J - j0) < POLYS ? (J - j0) : POLYS);
@@ -142,7 +140,7 @@ ntt2_kernel(const __grid_constant__ CUtensorMap dmap, const __grid_constant__ CU
         for (int p = 0; p < np; ++p) {
           const int64_t row = W.limb + a.L * (j0 + p);
           for (int x = 0; x < B::PER_POLY; ++x)
-            tma_load_2d(sbase + S::kBuf + b * unit_bytes(LOGN) + p * N * 8 + x * B::BOX * 128, &dmap, 0,
+            tma_load_2d(smem + S::kBuf + b * unit_bytes(LOGN) + p * N * 8 + x * B::BOX * 128, &dmap, 0,
                         (int)(row * B::ROWS128 + x * B::BOX), &bars[1 + b]);
         }
       };
@@ -157,7 +155,7 @@ ntt2_kernel(const __grid_constant__ CUtensorMap dmap, const __grid_constant__ CU
           const int64_t row = W.limb + a.L * (j0 + p);
           for (int x = 0; x < B::PER_POLY; ++x)
             tma_store_2d(&dmap, 0, (int)(row * B::ROWS128 + x * B::BOX),
-                         sbase + S::kBuf + b * unit_bytes(LOGN) + p * N * 8 + x * B::BOX * 128);
+                         smem + S::kBuf + b * unit_bytes(LOGN) + p * N * 8 + x * B::BOX * 128);
         }
         tma_commit();
         const int64_t un = u + (int64_t)NBUF * W.nworkers;
@@ -220,9 +218,7 @@ ntt2_kernel(const __grid_constant__ CUtensorMap dmap, const __grid_constant__ CU
       }
       fence_proxy_async();                 // generic-proxy writes -> visible to the TMA store
       __syncwarp();
-      if ((tid & 31) == 0) {
-        asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(&bars[3 + b])) : "memory");
-      }
+      if ((tid & 31) == 0) mbar_arrive(&bars[3 + b]);
     }
   }
   cluster_sync_all();   // nobody leaves while the partner may still be receiving its multicast half
@@ -321,7 +317,7 @@ encrypt2_kernel(const __grid_constant__ CUtensorMap tmap, EncArgs a) {
     fence_barrier_init();
   }
   cluster_sync_all();
-  if (tid == 0) load_twiddles<LOGN>(sbase + S::kTw, &bars[0], &tmap, (W.limb * 2) * (N * 16 / 128));
+  if (tid == 0) load_twiddles<LOGN>(smem + S::kTw, &bars[0], &tmap, (W.limb * 2) * (N * 16 / 128));
   const Limb T = make_limb(sbase + S::kTw, a.tw2 + (size_t)(W.limb * 2) * N * 2, a.consts, W.limb);
   const Modulus m{T.q, a.consts[W.limb * 8 + 1], a.consts[W.limb * 8 + 2]};
   const uint64_t sc = a.msg_scale ? a.msg_scale[W.limb] : 1;
@@ -448,7 +444,7 @@ decrypt2_kernel(const __grid_constant__ CUtensorMap tmap, DecArgs a) {
     fence_barrier_init();
   }
   cluster_sync_all();
-  if (tid == 0) load_twiddles<LOGN>(sbase + S::kTw, &bars[0], &tmap, (W.limb * 2 + 1) * (N * 16 / 128));
+  if (tid == 0) load_twiddles<LOGN>(smem + S::kTw, &bars[0], &tmap, (W.limb * 2 + 1) * (N * 16 / 128));
   const Limb T = make_limb(sbase + S::kTw, a.tw2 + (size_t)(W.limb * 2 + 1) * N * 2, a.consts, W.limb);
   const uint32_t buf = sbase + S::kBuf;
   const uint64_t* sx = a.skx + (size_t)W.limb * N * 2;
@@ -544,39 +540,10 @@ __global__ void shoup_pairs_kernel(const uint64_t* __restrict__ x, uint64_t* __r
 // ------------------------------------------------------------------------------------------
 // host side
 // ------------------------------------------------------------------------------------------
-typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
-                                  const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
-                                  CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-
-EncodeTiledFn encode_fn() {
-  static EncodeTiledFn fn = nullptr;
-  if (!fn) {
-    void* p = nullptr;
-    cudaDriverEntryPointQueryResult q;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &q) != cudaSuccess || !p)
-      throw std::runtime_error("cuTensorMapEncodeTiled not available");
-    fn = reinterpret_cast<EncodeTiledFn>(p);
-  }
-  return fn;
-}
-
 // u64 buffer of `bytes` bytes seen as [bytes/128][16]; copies move `box_rows` rows of 128 bytes.
 CUtensorMap rows128_map(const void* ptr, uint64_t bytes, uint32_t box_rows) {
-  CUtensorMap m;
-  cuuint64_t dims[2] = {16, bytes / 128};
-  cuuint64_t strides[1] = {128};
-  cuuint32_t box[2] = {16, box_rows};
-  cuuint32_t estr[2] = {1, 1};
-  const CUresult r = encode_fn()(&m, CU_TENSOR_MAP_DATA_TYPE_UINT64, 2, const_cast<void*>(ptr), dims, strides, box,
-                                 estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
-                                 CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) {
-    char buf[200];
-    snprintf(buf, sizeof(buf), "cuTensorMapEncodeTiled(u64 rows) failed (%d): bytes=%llu box_rows=%u ptr=%p", (int)r,
-             (unsigned long long)bytes, box_rows, ptr);
-    throw std::runtime_error(buf);
-  }
-  return m;
+  return tensor_map(ptr, CU_TENSOR_MAP_DATA_TYPE_UINT64, {16, bytes / 128}, {128}, {16, box_rows},
+                    CU_TENSOR_MAP_SWIZZLE_128B);
 }
 
 // Per-role CTA budgets (0 = every SM). The persistent kernels take one SM per CTA; when the pipelined FedAvg
@@ -584,17 +551,8 @@ CUtensorMap rows128_map(const void* ptr, uint64_t bytes, uint32_t box_rows) {
 // the others, so the runner partitions the chip (set_cta_limits) instead of letting three full-chip kernels queue.
 int g_limit[3] = {0, 0, 0};   // 0 ntt, 1 encrypt, 2 decrypt
 
-int sm_count() {
-  static int n = 0;
-  if (!n) {
-    int dev = 0;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
-  }
-  return n;
-}
 int grid_ctas(int role = 0) {
-  int n = sm_count() & ~1;
+  int n = device_sm_count() & ~1;
   if (g_limit[role] > 0 && g_limit[role] < n) n = g_limit[role] & ~1;
   return n < 2 ? 2 : n;
 }
@@ -602,21 +560,6 @@ int grid_ctas(int role = 0) {
 template <class K>
 void set_smem(K kernel, int bytes) {
   cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
-}
-
-// Cheapest inverse-correction schedule (bit p = reduce to [0,2q) before pass p) whose largest
-// intermediate, inv_bound_max * q, stays below 2^64.
-template <int LOGN>
-int pick_corr(int qbits) {
-  constexpr int NP = num_passes(LOGN);
-  const unsigned cands[3] = {0u, 1u << 1, (1u << (NP - 1)) - 1u};
-  for (int i = 0; i < 3; ++i) {
-    const long long worst = inv_bound_max<LOGN>(4, cands[i]);
-    int wb = 0;
-    while ((1ll << wb) < worst) ++wb;
-    if (wb + qbits <= 63) return i;
-  }
-  return -1;
 }
 
 template <int LOGN, bool INV, unsigned CORR>
@@ -640,9 +583,9 @@ bool dispatch_ntt2(uint64_t* data, int64_t rows, int L, const uint64_t* tw2, con
     return true;
   }
   switch (pick_corr<LOGN>(qbits)) {
-    case 0: launch_ntt2<LOGN, true, 0u>(data, rows, L, tw2, consts, st); return true;
-    case 1: launch_ntt2<LOGN, true, 1u << 1>(data, rows, L, tw2, consts, st); return true;
-    case 2: launch_ntt2<LOGN, true, (1u << (NP - 1)) - 1u>(data, rows, L, tw2, consts, st); return true;
+    case 0u: launch_ntt2<LOGN, true, 0u>(data, rows, L, tw2, consts, st); return true;
+    case 1u << 1: launch_ntt2<LOGN, true, 1u << 1>(data, rows, L, tw2, consts, st); return true;
+    case (1u << (NP - 1)) - 1u: launch_ntt2<LOGN, true, (1u << (NP - 1)) - 1u>(data, rows, L, tw2, consts, st); return true;
     default: return false;
   }
 }
@@ -660,7 +603,7 @@ void launch_encrypt2(EncArgs a, cudaStream_t st) {
     static uint64_t* scratch[16] = {nullptr};
     int dev = 0;
     cudaGetDevice(&dev);
-    if (!scratch[dev & 15]) cudaMalloc(&scratch[dev & 15], (size_t)sm_count() * N * 8);
+    if (!scratch[dev & 15]) cudaMalloc(&scratch[dev & 15], (size_t)device_sm_count() * N * 8);
     a.scratch = scratch[dev & 15];
   }
   k<<<grid, kThreads, Smem<LOGN, NBUF>::kTotal, st>>>(tmap, a);
@@ -679,9 +622,9 @@ template <int LOGN>
 bool dispatch_decrypt2(const DecArgs& a, int Ltab, int qbits, cudaStream_t st) {
   constexpr int NP = num_passes(LOGN);
   switch (pick_corr<LOGN>(qbits)) {
-    case 0: launch_decrypt2<LOGN, 0u>(a, Ltab, st); return true;
-    case 1: launch_decrypt2<LOGN, 1u << 1>(a, Ltab, st); return true;
-    case 2: launch_decrypt2<LOGN, (1u << (NP - 1)) - 1u>(a, Ltab, st); return true;
+    case 0u: launch_decrypt2<LOGN, 0u>(a, Ltab, st); return true;
+    case 1u << 1: launch_decrypt2<LOGN, 1u << 1>(a, Ltab, st); return true;
+    case (1u << (NP - 1)) - 1u: launch_decrypt2<LOGN, (1u << (NP - 1)) - 1u>(a, Ltab, st); return true;
     default: return false;
   }
 }

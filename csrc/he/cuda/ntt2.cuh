@@ -24,6 +24,7 @@
 #include <cstdint>
 #include <cuda_runtime.h>
 
+#include "../../common/hopper.cuh"
 #include "../modarith.h"
 
 namespace hefl {
@@ -54,9 +55,6 @@ __host__ __device__ constexpr int unit_bytes(int logn) { return (1 << unit_log(l
 // byte offset inside a 1024-byte-aligned buffer -> swizzled byte offset (TMA SWIZZLE_128B)
 __device__ __forceinline__ uint32_t swz(uint32_t o) { return o ^ ((o >> 3) & 0x70u); }
 
-__device__ __forceinline__ uint32_t smem_u32(const void* p) {
-  return static_cast<uint32_t>(__cvta_generic_to_shared(p));
-}
 __device__ __forceinline__ uint64_t lds64(uint32_t a) {
   uint64_t v;
   asm volatile("ld.shared.u64 %0, [%1];" : "=l"(v) : "r"(a));
@@ -278,70 +276,21 @@ __host__ __device__ constexpr int inv_bound_max(int B0, unsigned corr) {
   return worst;
 }
 
-// ---- mbarrier / TMA / cluster wrappers (kept local: the HE objects do not include csrc/nn) ----
-__device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count) : "memory");
-}
-__device__ __forceinline__ void fence_barrier_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
-__device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-__device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
-}
-// Bounded wait (traps after ~2 s instead of hanging the GPU).
-__device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
-  const uint32_t addr = smem_u32(bar);
-  uint32_t done = 0, spins = 0;
-  long long start = 0;
-  while (true) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2, 1000000;\n\t"
-        "selp.u32 %0, 1, 0, p;\n\t}"
-        : "=r"(done)
-        : "r"(addr), "r"(parity)
-        : "memory");
-    if (done) break;
-    if ((++spins & 0x3FFu) == 0) {
-      const long long now = clock64();
-      if (start == 0) start = now;
-      else if (now - start > 4000000000ll) __trap();
-    }
+// Cheapest inverse-correction schedule (bit p = reduce to [0, 2q) before pass p) whose largest intermediate,
+// inv_bound_max * q from inputs below 4q, stays below 2^64 for primes of `qbits` bits; ~0u when none does. The
+// inverse kernels are instantiated for these three schedules.
+template <int LOGN>
+unsigned pick_corr(int qbits) {
+  constexpr int NP = num_passes(LOGN);
+  const unsigned cands[3] = {0u, 1u << 1, (1u << (NP - 1)) - 1u};
+  for (const unsigned corr : cands) {
+    const long long worst = inv_bound_max<LOGN>(4, corr);
+    int wb = 0;
+    while ((1ll << wb) < worst) ++wb;
+    if (wb + qbits <= 63) return corr;
   }
+  return ~0u;
 }
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
-  asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-// 2-D tensor copy global -> shared memory of every CTA in `mask` (same offsets in each CTA).
-__device__ __forceinline__ void tma_load_2d_mc(uint32_t dst, const void* map, int c0, int c1, uint64_t* bar,
-                                               uint16_t mask) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster"
-      " [%0], [%1, {%2, %3}], [%4], %5;"
-      ::"r"(dst), "l"(reinterpret_cast<uint64_t>(map)), "r"(c0), "r"(c1), "r"(smem_u32(bar)), "h"(mask)
-      : "memory");
-}
-__device__ __forceinline__ void tma_load_2d(uint32_t dst, const void* map, int c0, int c1, uint64_t* bar) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3}], [%4];"
-      ::"r"(dst), "l"(reinterpret_cast<uint64_t>(map)), "r"(c0), "r"(c1), "r"(smem_u32(bar))
-      : "memory");
-}
-__device__ __forceinline__ void tma_store_2d(const void* map, int c0, int c1, uint32_t src) {
-  asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%1, %2}], [%3];"
-               ::"l"(reinterpret_cast<uint64_t>(map)), "r"(c0), "r"(c1), "r"(src)
-               : "memory");
-}
-__device__ __forceinline__ void tma_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
-template <int N>
-__device__ __forceinline__ void tma_wait_read() { asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory"); }
-template <int N>
-__device__ __forceinline__ void tma_wait_all() { asm volatile("cp.async.bulk.wait_group %0;" ::"n"(N) : "memory"); }
 
 }  // namespace dev2
 }  // namespace hefl

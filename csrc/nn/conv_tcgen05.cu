@@ -23,7 +23,6 @@
 // multiplied. Weights for all 9 taps stay resident in shared memory for the CTA's lifetime.
 #include <cuda_bf16.h>
 
-#include <cstdio>
 #include <stdexcept>
 
 #include "../he/kernels.h"
@@ -34,86 +33,17 @@
 namespace hefl {
 namespace nn {
 
+using namespace hefl::sm90;
 using namespace hefl::tc;
 
 // ------------------------------------------------------------------------------------------
 // host: tensor maps
 // ------------------------------------------------------------------------------------------
-typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
-                                  const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
-                                  CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-
-static EncodeTiledFn encode_fn() {
-  static EncodeTiledFn fn = nullptr;
-  if (!fn) {
-    void* p = nullptr;
-    cudaDriverEntryPointQueryResult q;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &q) != cudaSuccess || !p)
-      throw std::runtime_error("cuTensorMapEncodeTiled not available");
-    fn = reinterpret_cast<EncodeTiledFn>(p);
-  }
-  return fn;
-}
-
 // 2-D bf16 tensor [outer rows][inner cols], row pitch in bytes; box = box_inner x box_outer.
 static CUtensorMap make_map(const void* ptr, uint64_t inner, uint64_t outer, uint64_t pitch_bytes,
                             uint32_t box_inner, uint32_t box_outer) {
-  CUtensorMap m;
-  cuuint64_t dims[2] = {inner, outer};
-  cuuint64_t strides[1] = {pitch_bytes};
-  cuuint32_t box[2] = {box_inner, box_outer};
-  cuuint32_t estr[2] = {1, 1};
-  const uint32_t inner_bytes = box_inner * 2;
-  CUtensorMapSwizzle sw = inner_bytes == 128 ? CU_TENSOR_MAP_SWIZZLE_128B
-                          : inner_bytes == 64 ? CU_TENSOR_MAP_SWIZZLE_64B
-                                              : CU_TENSOR_MAP_SWIZZLE_32B;
-  CUresult r = encode_fn()(&m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(ptr), dims, strides, box,
-                           estr, CU_TENSOR_MAP_INTERLEAVE_NONE, sw, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-                           CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) {
-    char buf[256];
-    snprintf(buf, sizeof(buf), "cuTensorMapEncodeTiled failed (%d): inner=%llu outer=%llu pitch=%llu box=%ux%u",
-             (int)r, (unsigned long long)inner, (unsigned long long)outer, (unsigned long long)pitch_bytes,
-             box_inner, box_outer);
-    throw std::runtime_error(buf);
-  }
-  return m;
-}
-
-// NHWC bf16 activation [B*H rows][W][C] viewed as image-row pairs: 4-D {C, W, row parity, B*H/2 pairs};
-// box = {box_c, W, 1, box_pairs}, i.e. box_pairs * W consecutive smem rows of one parity (pairs past the end
-// zero-fill).
-static CUtensorMap make_pair_row_map(const void* ptr, uint64_t C, uint64_t W, uint64_t pairs, uint32_t box_c,
-                                     uint32_t box_pairs) {
-  CUtensorMap m;
-  cuuint64_t dims[4] = {C, W, 2, pairs};
-  cuuint64_t strides[3] = {C * 2, W * C * 2, 2 * W * C * 2};
-  cuuint32_t box[4] = {box_c, (cuuint32_t)W, 1, box_pairs};
-  cuuint32_t estr[4] = {1, 1, 1, 1};
-  const uint32_t inner_bytes = box_c * 2;
-  CUtensorMapSwizzle sw = inner_bytes == 128 ? CU_TENSOR_MAP_SWIZZLE_128B
-                          : inner_bytes == 64 ? CU_TENSOR_MAP_SWIZZLE_64B
-                                              : CU_TENSOR_MAP_SWIZZLE_32B;
-  CUresult r = encode_fn()(&m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, const_cast<void*>(ptr), dims, strides, box,
-                           estr, CU_TENSOR_MAP_INTERLEAVE_NONE, sw, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-                           CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) {
-    char buf[256];
-    snprintf(buf, sizeof(buf), "cuTensorMapEncodeTiled(4d) failed (%d): C=%llu W=%llu pairs=%llu box_pairs=%u", (int)r,
-             (unsigned long long)C, (unsigned long long)W, (unsigned long long)pairs, box_pairs);
-    throw std::runtime_error(buf);
-  }
-  return m;
-}
-
-static int num_sms() {
-  static int n = 0;
-  if (!n) {
-    int dev = 0;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
-  }
-  return n;
+  return tensor_map(ptr, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, {inner, outer}, {pitch_bytes}, {box_inner, box_outer},
+                    swizzle_for(box_inner * 2));
 }
 
 // ------------------------------------------------------------------------------------------
@@ -465,15 +395,21 @@ tap_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
 template <int CK, int CO, bool POOL, int TS = 3>
 static void launch_tap_gemm(const __nv_bfloat16* A, const __nv_bfloat16* Wt, TapGemmArgs a, cudaStream_t st) {
   using Cfg = TapGemmCfg<CK, CO, POOL, TS>;
-  const CUtensorMap tmA =
-      (POOL && a.pairs_per_tile)
-          ? make_pair_row_map(A, CK, (uint64_t)a.W, (uint64_t)a.B * a.H / 2, Cfg::KB, (uint32_t)a.pairs_per_tile)
-          : make_map(A, CK, (uint64_t)a.P, (uint64_t)CK * 2, Cfg::KB, Cfg::SEG_ROWS);
+  CUtensorMap tmA;
+  if (POOL && a.pairs_per_tile) {
+    // [B*H rows][W][CK] viewed as image-row pairs, 4-D {CK, W, row parity, B*H/2 pairs}: one box is pairs_per_tile * W
+    // consecutive smem rows of one parity (pairs past the end zero-fill)
+    const uint64_t W = (uint64_t)a.W, pairs = (uint64_t)a.B * a.H / 2;
+    tmA = tensor_map(A, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, {CK, W, 2, pairs}, {CK * 2, W * CK * 2, 2 * W * CK * 2},
+                     {Cfg::KB, (uint32_t)a.W, 1, (uint32_t)a.pairs_per_tile}, swizzle_for(Cfg::KB * 2));
+  } else {
+    tmA = make_map(A, CK, (uint64_t)a.P, (uint64_t)CK * 2, Cfg::KB, Cfg::SEG_ROWS);
+  }
   const CUtensorMap tmW = make_map(Wt, CK, (uint64_t)Cfg::NTAP * a.co_total, (uint64_t)CK * 2, Cfg::KB, CO);
   auto kern = tap_gemm_kernel<CK, CO, POOL, TS>;
   cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM);
   const int ny = a.co_total / CO;
-  const int slots = num_sms() * Cfg::OCC / ny;
+  const int slots = hefl::cuda::device_sm_count() * Cfg::OCC / ny;
   int gx = a.num_tiles < slots ? a.num_tiles : slots;
   if (gx < 1) gx = 1;
   dim3 grid(gx, ny);
@@ -524,7 +460,7 @@ void conv_fwd_pool(const void* X, const void* Wf, const float* bias, void* out, 
   // Output-channel blocks (blockIdx.y) while the tiles alone would leave SMs idle (the late, small layers): a CTA
   // then holds and multiplies 1/ny of the weights, and the input tile is read once per block (from L2).
   int co_blk = CO;
-  while (co_blk % 64 == 0 && a.num_tiles * (CO / co_blk) < num_sms()) co_blk /= 2;
+  while (co_blk % 64 == 0 && a.num_tiles * (CO / co_blk) < hefl::cuda::device_sm_count()) co_blk /= 2;
   const auto* x = reinterpret_cast<const __nv_bfloat16*>(X);
   const auto* w = reinterpret_cast<const __nv_bfloat16*>(Wf);
   if (CK == 16 && spack) launch_tap_gemm<16, 32, true, 1>(x, w, a, st);
@@ -783,7 +719,7 @@ static void launch_pair_fwd(const __nv_bfloat16* X, const __nv_bfloat16* Wt, Pai
   const CUtensorMap tmW = make_map(Wt, CK, (uint64_t)(SP ? 3 : 9) * CO, (uint64_t)CK * 2, CK, CO);
   auto kern = pair_fwd_kernel<CK, CO, SP>;
   cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM);
-  int gx = num_sms() * Cfg::OCC;
+  int gx = hefl::cuda::device_sm_count() * Cfg::OCC;
   if (gx > a.num_tiles) gx = a.num_tiles;
   launch_pdl(kern, dim3(gx), dim3(288), Cfg::SMEM, st, tmA, tmW, a);
   hefl::cuda::note_launch();
@@ -1050,38 +986,12 @@ wgrad_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ CU
         make_float2(bacc[0], bacc[1]);
 }
 
-// 3-D bf16 tensor [rows][W][C] (C contiguous); box = {box_c, box_w, 1}.
-static CUtensorMap make_map_3d(const void* ptr, uint64_t C, uint64_t W, uint64_t rows, uint32_t box_c,
-                               uint32_t box_w) {
-  CUtensorMap m;
-  cuuint64_t dims[3] = {C, W, rows};
-  cuuint64_t strides[2] = {C * 2, W * C * 2};
-  cuuint32_t box[3] = {box_c, box_w, 1};
-  cuuint32_t estr[3] = {1, 1, 1};
-  const uint32_t inner_bytes = box_c * 2;
-  CUtensorMapSwizzle sw = inner_bytes == 128 ? CU_TENSOR_MAP_SWIZZLE_128B
-                          : inner_bytes == 64 ? CU_TENSOR_MAP_SWIZZLE_64B
-                                              : CU_TENSOR_MAP_SWIZZLE_32B;
-  CUresult r = encode_fn()(&m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, const_cast<void*>(ptr), dims, strides, box,
-                           estr, CU_TENSOR_MAP_INTERLEAVE_NONE, sw, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-                           CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) throw std::runtime_error("cuTensorMapEncodeTiled(3d) failed");
-  return m;
-}
-
-// Same, with explicit byte strides (overlapping rows: stride_w < C*2 is legal for TMA).
-static CUtensorMap make_map_3d_strided(const void* ptr, uint64_t C, uint64_t W, uint64_t rows, uint64_t stride_w,
-                                       uint64_t stride_row, uint32_t box_c, uint32_t box_w) {
-  CUtensorMap m;
-  cuuint64_t dims[3] = {C, W, rows};
-  cuuint64_t strides[2] = {stride_w, stride_row};
-  cuuint32_t box[3] = {box_c, box_w, 1};
-  cuuint32_t estr[3] = {1, 1, 1};
-  CUresult r = encode_fn()(&m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, const_cast<void*>(ptr), dims, strides, box,
-                           estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
-                           CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) throw std::runtime_error("cuTensorMapEncodeTiled(3d, strided) failed");
-  return m;
+// 3-D bf16 tensor [rows][W][C] (C contiguous) with pixels `pixel_bytes` apart (below C * 2 they overlap, which TMA
+// allows); box = {box_c, box_w, 1}.
+static CUtensorMap make_map_3d(const void* ptr, uint64_t C, uint64_t W, uint64_t rows, uint64_t pixel_bytes,
+                               uint32_t box_c, uint32_t box_w) {
+  return tensor_map(ptr, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, {C, W, rows}, {pixel_bytes, W * pixel_bytes},
+                    {box_c, box_w, 1}, swizzle_for(box_c * 2));
 }
 
 template <int CK, int COT, bool FLAT>
@@ -1118,7 +1028,8 @@ static int wgrad_plan(int B, int H, int W, int Co, WgradArgs& a) {
   const int total_steps = FLAT ? a.nchunks : a.units * (a.rows_per + 2);
   // every CTA pays a fixed epilogue (a store of all accumulators): give each at least a few steps
   int gx = total_steps / (FLAT ? 6 : 24);
-  if (gx > num_sms() * Cfg::OCC / (3 * cot)) gx = num_sms() * Cfg::OCC / (3 * cot);
+  const int slots = hefl::cuda::device_sm_count() * Cfg::OCC / (3 * cot);
+  if (gx > slots) gx = slots;
   if (gx > (FLAT ? a.nchunks : a.units)) gx = FLAT ? a.nchunks : a.units;
   if (gx < 1) gx = 1;
   return gx;
@@ -1164,9 +1075,9 @@ void conv_wgrad(const void* X, const void* DY, float* dW32, float* ws, int B, in
       tmX = make_map(x, CKc, (uint64_t)P, (uint64_t)CKc * 2, CKc, Cfg::XROWS);
       tmD = make_map(d, Co, (uint64_t)P, (uint64_t)Co * 2, COT, 64);
     } else {
-      tmX = Cfg::PACK4 ? make_map_3d_strided(x, 64, W, (uint64_t)B * H, 32, (uint64_t)W * 32, 64, Cfg::XROWS)
-                       : make_map_3d(x, CKc, W, (uint64_t)B * H, CKc, Cfg::XROWS);
-      tmD = make_map_3d(d, Co, W, (uint64_t)B * H, COT, 64);
+      tmX = Cfg::PACK4 ? make_map_3d(x, 64, W, (uint64_t)B * H, 32, 64, Cfg::XROWS)
+                       : make_map_3d(x, CKc, W, (uint64_t)B * H, CKc * 2, CKc, Cfg::XROWS);
+      tmD = make_map_3d(d, Co, W, (uint64_t)B * H, (uint64_t)Co * 2, COT, 64);
     }
     auto kern = wgrad_kernel<CKc, COT, FLAT>;
     cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM);
@@ -1187,6 +1098,7 @@ void conv_wgrad(const void* X, const void* DY, float* dW32, float* ws, int B, in
 // ------------------------------------------------------------------------------------------
 namespace hefl {
 namespace nn {
+using namespace hefl::sm90;
 using namespace hefl::tc;
 
 template <int CK>

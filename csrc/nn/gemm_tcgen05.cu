@@ -16,7 +16,7 @@
 #include <cuda.h>
 #include <cuda_bf16.h>
 
-#include <cstdio>
+#include <algorithm>
 #include <stdexcept>
 
 #include "../he/kernels.h"
@@ -26,54 +26,16 @@
 namespace hefl {
 namespace nn {
 
+using namespace hefl::sm90;
 using namespace hefl::tc;
 
 namespace {
 
-typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
-                                  const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
-                                  CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-EncodeTiledFn encode_fn() {
-  static EncodeTiledFn fn = nullptr;
-  if (!fn) {
-    void* p = nullptr;
-    cudaDriverEntryPointQueryResult q;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &q) != cudaSuccess || !p)
-      throw std::runtime_error("cuTensorMapEncodeTiled not available");
-    fn = reinterpret_cast<EncodeTiledFn>(p);
-  }
-  return fn;
-}
-
 // 2-D tensor [rows][cols] of `esize`-byte elements, row pitch in bytes; box = box_cols x box_rows, 128 B swizzle.
 CUtensorMap map2d(const void* ptr, int esize, uint64_t cols, uint64_t rows, uint64_t pitch_bytes, uint32_t box_cols,
                   uint32_t box_rows) {
-  CUtensorMap m;
-  cuuint64_t dims[2] = {cols, rows};
-  cuuint64_t strides[1] = {pitch_bytes};
-  cuuint32_t box[2] = {box_cols, box_rows};
-  cuuint32_t estr[2] = {1, 1};
-  const CUresult r = encode_fn()(&m, esize == 2 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_UINT8, 2,
-                                 const_cast<void*>(ptr), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                                 CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-                                 CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) {
-    char buf[200];
-    snprintf(buf, sizeof(buf), "cuTensorMapEncodeTiled(gemm) failed (%d): cols=%llu rows=%llu pitch=%llu box=%ux%u", (int)r,
-             (unsigned long long)cols, (unsigned long long)rows, (unsigned long long)pitch_bytes, box_cols, box_rows);
-    throw std::runtime_error(buf);
-  }
-  return m;
-}
-
-int sm_count() {
-  static int n = 0;
-  if (!n) {
-    int dev = 0;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
-  }
-  return n;
+  return tensor_map(ptr, esize == 2 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_UINT8, {cols, rows},
+                    {pitch_bytes}, {box_cols, box_rows}, CU_TENSOR_MAP_SWIZZLE_128B);
 }
 
 // ------------------------------------------------------------------------------------------------------------
@@ -270,7 +232,7 @@ void launch_kmajor(const void* A, const void* Bm, const GemmArgs& a, int64_t a_r
   auto kern = kmajor_gemm_kernel<BN, FP8>;
   cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM);
   const int tiles = a.m_tiles * a.n_tiles;
-  const int grid = tiles < sm_count() ? tiles : sm_count();
+  const int grid = std::min(tiles, hefl::cuda::device_sm_count());
   kern<<<grid, 288, Cfg::SMEM, st>>>(tmA, tmB, a);
   hefl::cuda::note_launch();
 }
@@ -294,12 +256,6 @@ struct MxArgs {
 constexpr int kMxStage = 128 * 128 + 128 * 128 + 1024;    // A tile, B tile, two scale tiles
 constexpr int kMxStages = 5;
 constexpr int kMxSmem = kMxStages * kMxStage + 256 + 1024;
-
-__device__ __forceinline__ void bulk_load_1d(void* dst, const void* src, uint32_t bytes, uint64_t* bar) {
-  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-               ::"r"(smem_u32(dst)), "l"(src), "r"(bytes), "r"(smem_u32(bar))
-               : "memory");
-}
 
 // Warps 0..7 compute (warp w: rows 32*(w%4) .. +31, columns (w/4)*64 .. +63), warp 8 is the TMA producer. Each
 // 32-element k-block is one m16n8k32 e4m3 MMA into a zeroed fragment, which is then added to the fp32 accumulator
@@ -567,7 +523,7 @@ void launch_wgrad_mn(const void* DY, const void* X, const WgArgs& a, int64_t row
   auto kern = wgrad_mn_kernel<CT>;
   cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM);
   const int units = a.co_tiles * a.ci_tiles * a.groups * a.taps_per * a.ksplit;
-  const int grid = units < sm_count() ? units : sm_count();
+  const int grid = std::min(units, hefl::cuda::device_sm_count());
   kern<<<grid, 288, Cfg::SMEM, st>>>(tmDY, tmX, a);
   hefl::cuda::note_launch();
 }
@@ -635,7 +591,7 @@ void pad_nhwc(const void* x, void* xp, int B, int H, int W, int C, cudaStream_t 
   if (C % 8) throw std::runtime_error("pad_nhwc: C must be a multiple of 8");
   const int64_t total = (int64_t)B * (H + 2) * (W + 2) * (C / 8);
   int blocks = (int)((total + 255) / 256);
-  if (blocks > sm_count() * 16) blocks = sm_count() * 16;
+  blocks = std::min(blocks, hefl::cuda::device_sm_count() * 16);
   pad_nhwc_kernel<<<blocks, 256, 0, st>>>(reinterpret_cast<const uint4*>(x), reinterpret_cast<uint4*>(xp), B, H, W, C / 8);
   hefl::cuda::note_launch();
 }
@@ -649,7 +605,7 @@ void conv_weight_prep(const float* w, void* wt, void* wd, int Co, int Ci, int kk
 void conv_wgrad_unpack(const float* dw, float* g, int Co, int Ci, int kk, cudaStream_t st) {
   const int64_t total = (int64_t)kk * Co * Ci;
   int blocks = (int)((total + 255) / 256);
-  if (blocks > sm_count() * 8) blocks = sm_count() * 8;
+  blocks = std::min(blocks, hefl::cuda::device_sm_count() * 8);
   conv_wgrad_unpack_kernel<<<blocks, 256, 0, st>>>(dw, g, Co, Ci, kk);
   hefl::cuda::note_launch();
 }
@@ -671,7 +627,7 @@ void gemm_mxfp8(const void* A, const void* Bm, const void* sfa, const void* sfb,
   const CUtensorMap tmB = map2d(Bm, 1, (uint64_t)K, (uint64_t)N, (uint64_t)K, 128, 128);
   cudaFuncSetAttribute(mx_gemm_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kMxSmem);
   const int tiles = a.m_tiles * a.n_tiles;
-  const int grid = tiles < sm_count() ? tiles : sm_count();
+  const int grid = std::min(tiles, hefl::cuda::device_sm_count());
   mx_gemm_kernel<<<grid, 288, kMxSmem, st>>>(tmA, tmB, a);
   hefl::cuda::note_launch();
 }
@@ -721,8 +677,8 @@ void wgrad_taps(const void* DY, const void* X, float* dW, int64_t rows, int Co, 
   for (int g = 0; g < a.groups; ++g) a.gshift[g] = taps == 9 ? (g - 1) * Wp - 1 : 0;
   a.kchunks = (int)((rows + 63) / 64);
   const int base_units = a.co_tiles * a.ci_tiles * a.groups * a.taps_per;
-  int ks = (sm_count() + base_units - 1) / base_units;          // about one wave of CTAs: longer K runs per unit,
-                                                                // fewer REDs onto the same dW words
+  // about one wave of CTAs: longer K runs per unit, fewer REDs onto the same dW words
+  int ks = (hefl::cuda::device_sm_count() + base_units - 1) / base_units;
   if (ks < 1) ks = 1;
   if (ks > a.kchunks) ks = a.kchunks;
   a.ksplit = ks;

@@ -1,9 +1,11 @@
-// Thin inline-PTX wrappers for the Hopper (sm_90a) kernels: mbarrier, TMA (cp.async.bulk.tensor), and warp-level
-// tensor-core MMAs (ldmatrix + mma.sync) on the swizzled tiles TMA writes.
+// Helpers of the NN tensor-core kernels (sm_90a): shared-memory budgets, warp-level MMAs (ldmatrix + mma.sync) on the
+// swizzled tiles TMA writes, accumulator staging, the deterministic split-K sum and named barriers. The mbarrier, TMA
+// and tensor-map plumbing they share with the HE kernels is in common/hopper.cuh.
 #pragma once
 #include <cstdint>
-#include <cuda.h>
 #include <cuda_runtime.h>
+
+#include "../common/hopper.cuh"
 
 namespace hefl {
 namespace tc {
@@ -12,85 +14,6 @@ namespace tc {
 // resident block, so `nblocks` blocks of `smem` dynamic bytes fit on one SM when blocks_fit(smem, nblocks).
 constexpr int kSmemMax = 227 * 1024;
 constexpr bool blocks_fit(int smem, int nblocks) { return nblocks * (smem + 1024) <= 228 * 1024; }
-
-__device__ __forceinline__ uint32_t smem_u32(const void* p) {
-  return static_cast<uint32_t>(__cvta_generic_to_shared(p));
-}
-
-// ---- mbarrier -----------------------------------------------------------------------------
-__device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count) : "memory");
-}
-__device__ __forceinline__ void fence_barrier_init() {
-  asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-}
-__device__ __forceinline__ void fence_proxy_async() {
-  asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-}
-__device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
-  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes)
-               : "memory");
-}
-// Wait on the phase parity; traps (instead of hanging the GPU) after ~2 s. The suspend-time hint lets the
-// hardware park the warp until the phase completes instead of returning to a software spin loop: with ~30
-// waiting warps per SM the spin instructions were competing with the epilogue for issue slots.
-#ifndef HEFL_MBAR_SUSPEND_NS
-#define HEFL_MBAR_SUSPEND_NS 1000000
-#endif
-constexpr uint32_t kMbarSuspendNs = HEFL_MBAR_SUSPEND_NS;
-__device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
-  const uint32_t addr = smem_u32(bar);
-  uint32_t done = 0;
-  long long start = 0;
-  uint32_t spins = 0;
-  while (true) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2, %3;\n\t"
-        "selp.u32 %0, 1, 0, p;\n\t}"
-        : "=r"(done)
-        : "r"(addr), "r"(parity), "r"(kMbarSuspendNs)
-        : "memory");
-    if (done) break;
-    if ((++spins & 0xFFFu) == 0) {
-      const long long now = clock64();
-      if (start == 0) start = now;
-      else if (now - start > 4000000000ll) __trap();
-    }
-  }
-}
-
-// ---- TMA ----------------------------------------------------------------------------------
-__device__ __forceinline__ void prefetch_tmap(const CUtensorMap* m) {
-  asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(m)) : "memory");
-}
-__device__ __forceinline__ void tma_load_2d(void* dst, const CUtensorMap* map, int c0, int c1,
-                                            uint64_t* bar) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3}], [%4];"
-      ::"r"(smem_u32(dst)), "l"(reinterpret_cast<uint64_t>(map)), "r"(c0), "r"(c1), "r"(smem_u32(bar))
-      : "memory");
-}
-
-__device__ __forceinline__ void tma_load_3d(void* dst, const CUtensorMap* map, int c0, int c1, int c2,
-                                            uint64_t* bar) {
-  asm volatile(
-      "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3, %4}], [%5];"
-      ::"r"(smem_u32(dst)), "l"(reinterpret_cast<uint64_t>(map)), "r"(c0), "r"(c1), "r"(c2), "r"(smem_u32(bar))
-      : "memory");
-}
-
-__device__ __forceinline__ void tma_load_4d(void* dst, const CUtensorMap* map, int c0, int c1, int c2, int c3,
-                                            uint64_t* bar) {
-  asm volatile(
-      "cp.async.bulk.tensor.4d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3, %4, %5}], [%6];"
-      ::"r"(smem_u32(dst)), "l"(reinterpret_cast<uint64_t>(map)), "r"(c0), "r"(c1), "r"(c2), "r"(c3),
-        "r"(smem_u32(bar))
-      : "memory");
-}
 
 // ---- warp-level tensor-core MMA on TMA-written shared-memory tiles (sm_90) ---------------------
 // TMA writes a tile with a swizzle span of SW bytes (32, 64 or 128, equal to the tile's row length): the 16-byte
@@ -153,12 +76,6 @@ __device__ __forceinline__ uint32_t pack_bf16x2(float lo, float hi) {
   uint32_t r;
   asm("cvt.rn.bf16x2.f32 %0, %1, %2;" : "=r"(r) : "f"(hi), "f"(lo));
   return r;
-}
-// One lane of a converged warp.
-__device__ __forceinline__ bool elect_one() {
-  uint32_t pred;
-  asm volatile("{\n\t.reg .pred p;\n\telect.sync _|p, 0xffffffff;\n\tselp.u32 %0, 1, 0, p;\n\t}" : "=r"(pred));
-  return pred != 0;
 }
 
 // Deterministic split-K reduction: returns sum over p = 0 .. parts-1 of ws[p * n + i] for element i = blockIdx.x * 32 +

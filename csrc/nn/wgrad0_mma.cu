@@ -34,7 +34,6 @@
 #include <cuda_bf16.h>
 
 #include <cstdlib>
-#include <stdexcept>
 
 #include "../he/kernels.h"
 #include "launch.cuh"
@@ -46,6 +45,7 @@ namespace nn {
 
 namespace {
 
+using namespace hefl::sm90;
 using namespace hefl::tc;
 
 constexpr int kT = 256;                 // 8 warps
@@ -60,20 +60,6 @@ constexpr int kSmem = kBarOff + 64;     // 104 KB -> 2 CTAs / SM
 constexpr int kPartStride = 40;         // floats per row of a parked accumulator tile (bank spread)
 constexpr int kPart = 48 * kPartStride + 32;   // one warp's tile + its bias sums
 static_assert(8 * kPart * 4 <= kBarOff, "parked tiles must fit in the operand buffers");
-
-__device__ __forceinline__ void bulk_load(uint32_t dst, const void* src, uint32_t bytes, uint64_t* bar) {
-  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-               ::"r"(dst), "l"(src), "r"(bytes), "r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void ldsm4t(uint32_t (&r)[4], uint32_t addr) {
-  asm volatile("ldmatrix.sync.aligned.m8n8.x4.trans.shared.b16 {%0,%1,%2,%3}, [%4];"
-               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]) : "r"(addr));
-}
-__device__ __forceinline__ void mma16816(float (&d)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
-  asm volatile("mma.sync.aligned.m16n8k16.row.col.f32.bf16.bf16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
-               : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
-               : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
-}
 
 __global__ void __launch_bounds__(kT, 2)
 wgrad0_mma_kernel(const __grid_constant__ CUtensorMap tmX, const __nv_bfloat16* __restrict__ g,
@@ -138,8 +124,8 @@ wgrad0_mma_kernel(const __grid_constant__ CUtensorMap tmX, const __nv_bfloat16* 
         mbar_expect_tx(&full[par], 4 * row_bytes + g_bytes + c_bytes);
 #pragma unroll
         for (int r = 0; r < 4; ++r) tma_load_2d(ring + r * kSlot, &tmX, 0, (b * H + 2 * i + r) * pairs, &full[par]);
-        bulk_load(smem_u32(gst + par * kGst), g + (size_t)s * Wp * 32, g_bytes, &full[par]);
-        bulk_load(smem_u32(cst + par * kCst), amax + (size_t)s * Wp * 32, c_bytes, &full[par]);
+        bulk_load_1d(gst + par * kGst, g + (size_t)s * Wp * 32, g_bytes, &full[par]);
+        bulk_load_1d(cst + par * kCst, amax + (size_t)s * Wp * 32, c_bytes, &full[par]);
       }
       if (pref_next) {                                       // the next strip: two new rows, its gradient and codes
         const int q = par ^ 1;
@@ -149,8 +135,8 @@ wgrad0_mma_kernel(const __grid_constant__ CUtensorMap tmX, const __nv_bfloat16* 
         mbar_expect_tx(&full[q], 2 * row_bytes + g_bytes + c_bytes);
         tma_load_2d(ring + sl4 * kSlot, &tmX, 0, (b * H + 2 * i + 4) * pairs, &full[q]);
         tma_load_2d(ring + sl5 * kSlot, &tmX, 0, (b * H + 2 * i + 5) * pairs, &full[q]);
-        bulk_load(smem_u32(gst + q * kGst), g + (size_t)(s + 1) * Wp * 32, g_bytes, &full[q]);
-        bulk_load(smem_u32(cst + q * kCst), amax + (size_t)(s + 1) * Wp * 32, c_bytes, &full[q]);
+        bulk_load_1d(gst + q * kGst, g + (size_t)(s + 1) * Wp * 32, g_bytes, &full[q]);
+        bulk_load_1d(cst + q * kCst, amax + (size_t)(s + 1) * Wp * 32, c_bytes, &full[q]);
       }
     }
     mbar_wait(&full[par], ((s - s0) >> 1) & 1);
@@ -196,18 +182,18 @@ wgrad0_mma_kernel(const __grid_constant__ CUtensorMap tmX, const __nv_bfloat16* 
       for (int c = 0; c < 4; ++c) {
         const int dy = c >> 1;
         uint32_t bq[2][4];
-        ldsm4t(bq[0], Gs_u + c * kGs + b_off0);
-        ldsm4t(bq[1], Gs_u + c * kGs + b_off2);
+        ldsm_x4_t(Gs_u + c * kGs + b_off0, bq[0]);
+        ldsm_x4_t(Gs_u + c * kGs + b_off2, bq[1]);
 #pragma unroll
         for (int r = 0; r < 3; ++r) {
           int slot = head + dy + r;
           slot = slot >= kRing ? slot - kRing : slot;
           uint32_t a[4];
-          ldsm4t(a, ring_u + slot * kSlot + ((c & 1) ? a_off1 : a_off0));
-          mma16816(acc[r][0], a, bq[0][0], bq[0][1]);
-          mma16816(acc[r][1], a, bq[0][2], bq[0][3]);
-          mma16816(acc[r][2], a, bq[1][0], bq[1][1]);
-          mma16816(acc[r][3], a, bq[1][2], bq[1][3]);
+          ldsm_x4_t(ring_u + slot * kSlot + ((c & 1) ? a_off1 : a_off0), a);
+          mma_bf16(acc[r][0], a, bq[0][0], bq[0][1]);
+          mma_bf16(acc[r][1], a, bq[0][2], bq[0][3]);
+          mma_bf16(acc[r][2], a, bq[1][0], bq[1][1]);
+          mma_bf16(acc[r][3], a, bq[1][2], bq[1][3]);
         }
       }
     }
@@ -250,32 +236,6 @@ wgrad0_mma_kernel(const __grid_constant__ CUtensorMap tmX, const __nv_bfloat16* 
   }
 }
 
-typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
-                                  const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
-                                  CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-
-// X viewed as [pixel pairs][2 x 16 channels]: one box = one image row, 64-byte swizzle
-CUtensorMap make_row_map(const void* X, uint64_t pairs_total, uint32_t pairs_per_row) {
-  static EncodeTiledFn fn = nullptr;
-  if (!fn) {
-    void* p = nullptr;
-    cudaDriverEntryPointQueryResult q;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &q) != cudaSuccess || !p)
-      throw std::runtime_error("cuTensorMapEncodeTiled not available");
-    fn = reinterpret_cast<EncodeTiledFn>(p);
-  }
-  CUtensorMap m;
-  cuuint64_t dims[2] = {32, pairs_total};
-  cuuint64_t strides[1] = {64};
-  cuuint32_t box[2] = {32, pairs_per_row};
-  cuuint32_t estr[2] = {1, 1};
-  const CUresult r = fn(&m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(X), dims, strides, box, estr,
-                        CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_64B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-                        CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) throw std::runtime_error("cuTensorMapEncodeTiled(wgrad0 rows) failed");
-  return m;
-}
-
 }  // namespace
 
 bool wgrad0_mma_supported(int W, int Wp, int CK, int Ci, int Co) {
@@ -295,9 +255,7 @@ __global__ void __launch_bounds__(256) wgrad0_reduce_kernel(const float* __restr
 }
 
 int wgrad0_parts(int B, int Hp) {
-  int dev = 0, sms = 0;
-  cudaGetDevice(&dev);
-  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+  const int sms = hefl::cuda::device_sm_count();
   return sms * 2 < B * Hp ? sms * 2 : B * Hp;
 }
 
@@ -308,15 +266,15 @@ void wgrad0_reduce(const float* ws, int parts, float* dW, cudaStream_t st) {
 
 void wgrad0_mma(const void* X, const void* g, const uint8_t* amax, float* dW, float* ws, int B, int H, int W, int Hp,
                 int Wp, cudaStream_t st) {
-  static int sms = 0;
-  if (!sms) {
-    int dev = 0;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+  static bool attrs_set = false;
+  if (!attrs_set) {
     cudaFuncSetAttribute(wgrad0_mma_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmem);
     cudaFuncSetAttribute(wgrad0_mma_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, 100);
+    attrs_set = true;
   }
-  const CUtensorMap tmX = make_row_map(X, (uint64_t)B * H * (W / 2), (uint32_t)(W / 2));
+  // X viewed as [pixel pairs][2 x 16 channels]: one box = one image row, 64-byte swizzle
+  const CUtensorMap tmX = tensor_map(X, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, {32, (uint64_t)B * H * (W / 2)}, {64},
+                                     {32, (uint32_t)(W / 2)}, CU_TENSOR_MAP_SWIZZLE_64B);
   const int grid = wgrad0_parts(B, Hp);
   launch_pdl(wgrad0_mma_kernel, dim3(grid), dim3(kT), kSmem, st, tmX, reinterpret_cast<const __nv_bfloat16*>(g), amax, ws,
              B, H, W, Hp, Wp);

@@ -60,9 +60,10 @@ BINDING_SOURCES = [
 
 
 def _headers_digest(subdirs) -> str:
-    """Digest of the headers a source directory can see: its own plus csrc/he (shared arithmetic)."""
+    """Digest of the headers a source directory can see: its own, csrc/he (shared arithmetic) and csrc/common
+    (Hopper plumbing)."""
     h = hashlib.sha256()
-    for sub in sorted(set(subdirs) | {"he"}):
+    for sub in sorted(set(subdirs) | {"he", "common"}):
         for p in sorted((CSRC / sub).rglob("*")):
             if p.suffix in (".h", ".cuh", ".hpp"):
                 h.update(p.read_bytes())

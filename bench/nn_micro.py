@@ -1,6 +1,8 @@
 """Per-kernel timing of one medical-CNN training step on the tcgen05 engine (CUDA events,
 warm-up, L2 flushed between iterations). Writes gpurun_out/nn_micro.json."""
-import json, os, sys
+# --in-channels 1 times the grayscale arm (rs-packed layer 1) and writes its report to --out, by default
+# bench_out/nn_micro_c1.json; --out also moves the RGB report.
+import argparse, json, os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch, torch.nn.functional as F
 from hefl_b200 import _ext
@@ -27,13 +29,18 @@ def timeit(fn, iters=10, warmup=3):
 
 
 def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--in-channels", type=int, choices=(1, 3), default=3)
+    ap.add_argument("--out", default=None, help="JSON report path")
+    args = ap.parse_args()
+    C = args.in_channels
     B = 32
-    cfg = FLConfig(model="medcnn", batch_size=B)
+    cfg = FLConfig(model="medcnn", batch_size=B, in_channels=C)
     dev = torch.device("cuda")
-    model = create_model("medcnn").to(dev)
+    model = create_model("medcnn", in_channels=C).to(dev)
     pack = ParamPack(model)
     eng = MedCNNEngine(model, pack, cfg, dev)
-    x = torch.randint(0, 256, (B, 256, 256, 3), dtype=torch.uint8, device="cuda")
+    x = torch.randint(0, 256, (B, 256, 256, C), dtype=torch.uint8, device="cuda")
     y = torch.randint(0, 2, (B,), device="cuda")
     out = torch.zeros(2, device="cuda")
     eng.train_step(x, y, out, augment=True)
@@ -43,17 +50,17 @@ def main():
     res["preprocess"] = timeit(lambda: ops.preprocess_u8(x, None, eng.X[0], 99, None, eng.spack0))
     for l in range(eng.n):
         h = eng.H[l]
-        res[f"fwd{l}"] = timeit(lambda l=l, h=h: ops.conv_fwd_pool(eng.X[l], eng._wf(l), eng.bias[l], eng.X[l + 1], eng.amax[l], B, h, h, eng.CK[l], eng.Co[l], eng.spack0 and l == 0))
+        res[f"fwd{l}"] = timeit(lambda l=l, h=h: ops.conv_fwd_pool(eng.X[l], eng._wf(l), eng.bias[l], eng.X[l + 1], eng.amax[l], B, h, h, eng.CK[l], eng.Co[l], eng.spack0 and l == 0, C))
         if l == 0 and eng.fwd_pair:
             res["fwd0(tap-GEMM, not used)"] = res["fwd0"]
-            res["fwd0"] = timeit(lambda: ops.conv_fwd_pool_pair(eng._x0_bufs[0], eng._wf(0), eng.bias[0], eng.X[1], eng.amax[0], B, h, h, eng.CK[0], eng.Co[0], eng.spack0))
+            res["fwd0"] = timeit(lambda: ops.conv_fwd_pool_pair(eng._x0_bufs[0], eng._wf(0), eng.bias[0], eng.X[1], eng.amax[0], B, h, h, eng.CK[0], eng.Co[0], eng.spack0, C))
     g = torch.randn(B, 512, device="cuda").to(torch.bfloat16).view_as(eng.X[eng.n]).contiguous()
     for l in range(eng.n - 1, -1, -1):
         h = eng.H[l]
         gin = g if l == eng.n - 1 else eng.gX[l + 1]
         if l == 0:
             res["wgrad0(gather from pooled grad)"] = timeit(lambda: ops.wgrad0_gather(eng._x0_bufs[0], gin, eng.amax[0], eng._dw(0), B, h, h))
-            res["wgrad0(masked GEMMs, mma.sync)"] = timeit(lambda: ops.wgrad0_gather(eng._x0_bufs[0], gin, eng.amax[0], eng._dw(0), B, h, h, eng.spack0))
+            res["wgrad0(masked GEMMs, mma.sync)"] = timeit(lambda: ops.wgrad0_gather(eng._x0_bufs[0], gin, eng.amax[0], eng._dw(0), B, h, h, eng.spack0, C))
             eng.dY[0] = torch.zeros(eng.P[0], eng.Co[0], dtype=torch.bfloat16, device="cuda")
         res[f"unpool{l}"] = timeit(lambda l=l, h=h, gin=gin: ops.unpool_relu(gin, eng.amax[l], eng.X[l + 1], eng.dY[l], B, h, h, eng.Co[l]))
         res[f"wgrad{l}(tcgen05)"] = timeit(lambda l=l, h=h: ops.conv_wgrad(eng.X[l], eng.dY[l], eng._dw(l), B, h, h, eng.CK[l], eng.Co[l]))
@@ -98,6 +105,11 @@ def main():
     for k, v in res.items():
         print(f"{k:24s} {v:9.1f} us")
     print(f"{'sum of parts':24s} {tot:9.1f} us")
+    out = args.out or (None if C == 3 else os.path.join("bench_out", f"nn_micro_c{C}.json"))
+    if out is not None:
+        os.makedirs(os.path.dirname(out) or ".", exist_ok=True)
+        json.dump(res, open(out, "w"), indent=1)
+        return
     os.makedirs("gpurun_out", exist_ok=True)
     json.dump(res, open("gpurun_out/nn_micro.json", "w"), indent=1)
 

@@ -60,7 +60,9 @@ static CUtensorMap make_map(const void* ptr, uint64_t inner, uint64_t outer, uin
 //             GEMM row m = k*W + w is column w of row 2(q0+k) + j (4-D tensor map, one TMA box per segment).
 //             The accumulators, taps and row offsets are the ones above, so every output gets the same MMAs
 //             in the same order (bit-identical results) on a fraction of the tiles.
-//   dgrad   : tile = 128 consecutive pixels; 3 segments starting at m0 - r*W - 2; tap (r,s)
+//   forward, rs-packed input (one-channel layer 1, TS = kTapsRS): the input already carries the 3x3 neighbourhood
+//             in its channels, so a tile is one tap on 2 halo segments (rows h, h+1), column or row-packed alike.
+//   dgrad   :tile = 128 consecutive pixels; 3 segments starting at m0 - r*W - 2; tap (r,s)
 //             reads segment r at row offset 2 - s.
 // L2->SM traffic drops from 9 tap tiles to ~2 (fwd) / ~3 (dgrad) tiles per output tile.
 // ------------------------------------------------------------------------------------------
@@ -103,13 +105,17 @@ __device__ __forceinline__ int fast_div(int n, int d, uint32_t magic) {
 // TS = filter taps along the image row that are separate GEMMs: 3 normally; 1 when the three horizontal taps
 // are packed into the channel dimension by the producer of the input (layer 1: 3 channels x 3 taps = 9 of the
 // 16 padded channels, written by preprocess_u8) — a third of the MMAs for the same bytes.
+// TS = kTapsRS (0): the whole 3x3 neighbourhood is packed (rs layout of a one-channel layer 1: channel 3r + s =
+// pixel (h + r, w + s)), so one GEMM per accumulator remains and a pooled tile needs only its own 2 image rows.
+constexpr int kTapsRS = 0;
+
 template <int CK, int CO, bool POOL, int TS = 3>
 struct TapGemmCfg {
-  static constexpr int NTAP = 3 * TS;
+  static constexpr int NTAP = TS ? 3 * TS : 1;
   static constexpr int KB = CK < 64 ? CK : 64;            // channels per k-block (one swizzle atom)
   static constexpr int NKB = CK / KB;
   static constexpr int ROW_BYTES = KB * 2;
-  static constexpr int NSEG = POOL ? 4 : 3;
+  static constexpr int NSEG = POOL ? (TS ? 4 : 2) : 3;
   static constexpr int NACC = POOL ? 2 : 1;
   static constexpr int SEG_ROWS = 136;                    // 130 used, multiple of 8
   static constexpr int SEG_BYTES = SEG_ROWS * ROW_BYTES;
@@ -272,7 +278,7 @@ tap_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
 #endif
 #pragma unroll 1
         for (int tap = 0; tap < Cfg::NTAP; ++tap) {
-          const int r = tap / TS, s = tap % TS;
+          const int r = TS ? tap / (TS ? TS : 1) : 0, s = TS ? tap % (TS ? TS : 1) : 0;
           const int shift = POOL ? s : (2 - s);
 #pragma unroll
           for (int kb = 0; kb < Cfg::NKB; ++kb) {
@@ -429,7 +435,7 @@ void conv_set_debug(int mask) {
 #endif
 
 void conv_fwd_pool(const void* X, const void* Wf, const float* bias, void* out, uint8_t* argmax, int B, int H,
-                   int W, int CK, int CO, int spack, cudaStream_t st) {
+                   int W, int CK, int CO, int spack, int in_channels, cudaStream_t st) {
   TapGemmArgs a{};
 #ifdef HEFL_CONV_DEBUG
   a.dbg = g_dbg;
@@ -463,7 +469,10 @@ void conv_fwd_pool(const void* X, const void* Wf, const float* bias, void* out, 
   while (co_blk % 64 == 0 && a.num_tiles * (CO / co_blk) < hefl::cuda::device_sm_count()) co_blk /= 2;
   const auto* x = reinterpret_cast<const __nv_bfloat16*>(X);
   const auto* w = reinterpret_cast<const __nv_bfloat16*>(Wf);
-  if (CK == 16 && spack) launch_tap_gemm<16, 32, true, 1>(x, w, a, st);
+  if (spack && !(CK == 16 && CO == 32 && (in_channels == 1 || in_channels == 3)))
+    throw std::runtime_error("conv_fwd_pool: packed input is the 1- or 3-channel first layer (CK=16, CO=32) only");
+  if (CK == 16 && spack && in_channels == 1) launch_tap_gemm<16, 32, true, kTapsRS>(x, w, a, st);
+  else if (CK == 16 && spack) launch_tap_gemm<16, 32, true, 1>(x, w, a, st);
   else if (CK == 16) launch_tap_gemm<16, 32, true>(x, w, a, st);
   else if (CK == 32 && co_blk == 32) launch_tap_gemm<32, 32, true>(x, w, a, st);
   else if (CK == 32) launch_tap_gemm<32, 64, true>(x, w, a, st);
@@ -511,10 +520,10 @@ void conv_dgrad(const void* dY, const void* Wd, void* dX, int B, int H, int W, i
 // shuffles, every lane stores a full 16-byte pooled pixel chunk. Restricted to CK <= 32 (one swizzle atom per
 // pair-row) and CO <= 64 (4 accumulators in registers).
 // ------------------------------------------------------------------------------------------
-template <int CK, int CO>
+template <int CK, int CO, int NSEG_ = 4>
 struct PairFwdCfg {
   static constexpr int ROW_BYTES = 2 * CK * 2;            // one pair-row: 2 pixels x CK channels, 64 or 128 B
-  static constexpr int NSEG = 4;                          // image rows 2hp .. 2hp+3
+  static constexpr int NSEG = NSEG_;                      // image rows 2hp .. 2hp+3 (2hp, 2hp+1 on the rs layout)
   static constexpr int SEG_ROWS = 136;                    // 130 pair-rows used (128 windows + shift 1 + slack)
   static constexpr int SEG_BYTES = SEG_ROWS * ROW_BYTES;
   static constexpr int HALO = NSEG * SEG_BYTES;
@@ -542,15 +551,25 @@ struct PairFwdArgs {
   uint8_t* argmax;      // may be null
 };
 
-// SP: s-packed layer-1 input (channels = pixels x, x+1, x+2): the three horizontal taps are already inside the 16
-// channels, so only the three filter rows remain — 3 MMAs per accumulator, column parity = K byte offset.
+// Input layouts (PK):
+//   kPairPlain : CK channels per pixel, 9 tap GEMMs;
+//   kPairS     : s-packed layer-1 input (channels = pixels x, x+1, x+2): the three horizontal taps are already inside
+//                the 16 channels, so only the three filter rows remain — 3 MMAs per accumulator, column parity = K
+//                byte offset;
+//   kPairRS    : rs-packed one-channel layer-1 input (channel 3r + s = pixel (y + r, x + s)): one filter row,
+//                acc(dy,dx)[j] = X[row 2hp+dy, pair-row j, half dx] . W — one MMA k-step per accumulator on a
+//                2-row halo.
 // Warp roles as in G1: warps 0..7 compute + epilogue (lane = window, quadrant = warp % 4, chunks by warp / 4),
 // warp 8 is the TMA producer.
-template <int CK, int CO, bool SP>
-__global__ void __launch_bounds__(288, PairFwdCfg<CK, CO>::OCC)
-pair_fwd_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmW,
-                const PairFwdArgs a) {
-  using Cfg = PairFwdCfg<CK, CO>;
+constexpr int kPairPlain = 0, kPairS = 1, kPairRS = 2;
+
+template <int CK, int CO, int PK>
+using PairCfgOf = PairFwdCfg<CK, CO, PK == kPairRS ? 2 : 4>;
+
+template <int CK, int CO, int PK>
+__device__ __forceinline__ void pair_fwd_body(const CUtensorMap& tmA, const CUtensorMap& tmW, const PairFwdArgs& a) {
+  using Cfg = PairCfgOf<CK, CO, PK>;
+  constexpr bool SP = PK == kPairS;
   constexpr int RB = Cfg::ROW_BYTES;
   constexpr int WB = Cfg::W_ROW;
   extern __shared__ uint8_t smem_raw[];
@@ -575,7 +594,7 @@ pair_fwd_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
   __syncthreads();
   pdl_trigger();
   if (warp == 8 && elect_one()) {
-    constexpr int NTAPW = SP ? 3 : 9;
+    constexpr int NTAPW = PK == kPairRS ? 1 : (SP ? 3 : 9);
     mbar_expect_tx(wfull, NTAPW * Cfg::W_TAP);
     for (int tap = 0; tap < NTAPW; ++tap) tma_load_2d(sW + tap * Cfg::W_TAP, &tmW, 0, tap * CO, wfull);
   }
@@ -623,7 +642,21 @@ pair_fwd_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
             for (int mt = 0; mt < 2; ++mt)
 #pragma unroll
               for (int q = 0; q < 4; ++q) acc[x][i][mt][q] = 0.f;
-        if constexpr (SP) {
+        if constexpr (PK == kPairRS) {
+          uint32_t bf[4];
+          ld_b_kmajor<WB>(w_base, c0 * 8, (c0 + 2) * 8, 0, lane, bf);
+#pragma unroll
+          for (int dy = 0; dy < 2; ++dy)
+#pragma unroll
+            for (int dx = 0; dx < 2; ++dx)
+#pragma unroll
+              for (int mt = 0; mt < 2; ++mt) {
+                uint32_t af[4];
+                ld_a_kmajor<RB>(a_base + dy * Cfg::SEG_BYTES, qd * 32 + mt * 16, dx * CK * 2, lane, af);
+                mma_bf16(acc[dy * 2 + dx][0][mt], af, bf[0], bf[1]);
+                mma_bf16(acc[dy * 2 + dx][1][mt], af, bf[2], bf[3]);
+              }
+        } else if constexpr (SP) {
 #pragma unroll
           for (int r = 0; r < 3; ++r) {
             uint32_t bf[4];
@@ -711,13 +744,30 @@ pair_fwd_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
   }
 }
 
-template <int CK, int CO, bool SP = false>
+template <int CK, int CO, bool SP>
+__global__ void __launch_bounds__(288, PairFwdCfg<CK, CO>::OCC)
+pair_fwd_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmW,
+                const PairFwdArgs a) {
+  pair_fwd_body<CK, CO, SP ? kPairS : kPairPlain>(tmA, tmW, a);
+}
+
+// the one-channel layer 1 on the rs-packed input (CK = 16, CO = 32)
+__global__ void __launch_bounds__(288, PairCfgOf<16, 32, kPairRS>::OCC)
+pair_fwd_rs_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmW,
+                   const PairFwdArgs a) {
+  pair_fwd_body<16, 32, kPairRS>(tmA, tmW, a);
+}
+
+template <int CK, int CO, int PK = kPairPlain>
 static void launch_pair_fwd(const __nv_bfloat16* X, const __nv_bfloat16* Wt, PairFwdArgs a, cudaStream_t st) {
-  using Cfg = PairFwdCfg<CK, CO>;
+  using Cfg = PairCfgOf<CK, CO, PK>;
   const uint64_t pair_rows = ((uint64_t)a.B * a.H * a.W) / 2;
   const CUtensorMap tmA = make_map(X, 2 * CK, pair_rows, (uint64_t)Cfg::ROW_BYTES, 2 * CK, Cfg::SEG_ROWS);
-  const CUtensorMap tmW = make_map(Wt, CK, (uint64_t)(SP ? 3 : 9) * CO, (uint64_t)CK * 2, CK, CO);
-  auto kern = pair_fwd_kernel<CK, CO, SP>;
+  const int ntap = PK == kPairRS ? 1 : (PK == kPairS ? 3 : 9);
+  const CUtensorMap tmW = make_map(Wt, CK, (uint64_t)ntap * CO, (uint64_t)CK * 2, CK, CO);
+  void (*kern)(const CUtensorMap, const CUtensorMap, const PairFwdArgs);
+  if constexpr (PK == kPairRS) kern = pair_fwd_rs_kernel;
+  else kern = pair_fwd_kernel<CK, CO, PK == kPairS>;
   cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM);
   int gx = hefl::cuda::device_sm_count() * Cfg::OCC;
   if (gx > a.num_tiles) gx = a.num_tiles;
@@ -729,10 +779,10 @@ bool conv_fwd_pool_pair_supported(int H, int W, int CK, int CO) {
   return H == W && (W % 2) == 0 && (W - 2) / 2 <= 128 && (CK == 16 || CK == 32) && (CO == 32 || CO == 64);
 }
 
-// Same contract as conv_fwd_pool (plain 9-tap weight layout [9][CO][CK], or [3][CO][16] with the s-packed input);
-// see G1b above.
+// Same contract as conv_fwd_pool (plain 9-tap weight layout [9][CO][CK], [3][CO][16] with the s-packed input,
+// [1][CO][16] with the rs-packed one-channel input); see G1b above.
 void conv_fwd_pool_pair(const void* X, const void* Wf, const float* bias, void* out, uint8_t* argmax, int B, int H,
-                        int W, int CK, int CO, int spack, cudaStream_t st) {
+                        int W, int CK, int CO, int spack, int in_channels, cudaStream_t st) {
   if (!conv_fwd_pool_pair_supported(H, W, CK, CO)) throw std::runtime_error("conv_fwd_pool_pair: unsupported shape");
   PairFwdArgs a{};
   a.B = B; a.H = H; a.W = W;
@@ -744,7 +794,10 @@ void conv_fwd_pool_pair(const void* X, const void* Wf, const float* bias, void* 
   const auto* x = reinterpret_cast<const __nv_bfloat16*>(X);
   const auto* w = reinterpret_cast<const __nv_bfloat16*>(Wf);
   if (spack && !(CK == 16 && CO == 32)) throw std::runtime_error("conv_fwd_pool_pair: s-packed input is CK=16, CO=32 only");
-  if (CK == 16 && CO == 32 && spack) launch_pair_fwd<16, 32, true>(x, w, a, st);
+  if (spack && in_channels != 1 && in_channels != 3)
+    throw std::runtime_error("conv_fwd_pool_pair: packed input has 1 or 3 channels");
+  if (CK == 16 && CO == 32 && spack && in_channels == 1) launch_pair_fwd<16, 32, kPairRS>(x, w, a, st);
+  else if (CK == 16 && CO == 32 && spack) launch_pair_fwd<16, 32, kPairS>(x, w, a, st);
   else if (CK == 16 && CO == 32) launch_pair_fwd<16, 32>(x, w, a, st);
   else if (CK == 32 && CO == 32) launch_pair_fwd<32, 32>(x, w, a, st);
   else if (CK == 32 && CO == 64) launch_pair_fwd<32, 64>(x, w, a, st);

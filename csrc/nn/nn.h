@@ -14,11 +14,13 @@ void adam_step(float* p, float* g, float* m, float* v, void* shadow_bf16, int64_
                float beta2, float eps, cudaStream_t st);
 
 // ---- tensor-core implicit-GEMM convolution (conv_tcgen05.cu) ----
+// spack: the layer-1 input is packed by preprocess_u8 — s-packed when in_channels == 3 (weights [3][CO][16]),
+// rs-packed when in_channels == 1 (weights [1][CO][16]); in_channels is not read without spack.
 void conv_fwd_pool(const void* X, const void* Wf, const float* bias, void* out, uint8_t* argmax, int B, int H,
-                   int W, int CK, int CO, int spack, cudaStream_t st);
+                   int W, int CK, int CO, int spack, int in_channels, cudaStream_t st);
 bool conv_fwd_pool_pair_supported(int H, int W, int CK, int CO);
 void conv_fwd_pool_pair(const void* X, const void* Wf, const float* bias, void* out, uint8_t* argmax, int B, int H,
-                        int W, int CK, int CO, int spack, cudaStream_t st);
+                        int W, int CK, int CO, int spack, int in_channels, cudaStream_t st);
 void conv_set_debug(int mask);
 void conv_dgrad(const void* dY, const void* Wd, void* dX, int B, int H, int W, int CK, int CO, const uint8_t* up_amax,
                 int up_W, cudaStream_t st);
@@ -46,10 +48,11 @@ int wgrad0_parts(int B, int Hp);
 void wgrad0_reduce(const float* ws, int parts, float* dW, cudaStream_t st);
 void wgrad0_gather(const void* X, const void* g, const uint8_t* amax, float* dW, float* ws, int B, int H, int W, int Hp,
                    int Wp, cudaStream_t st);
-// the same gradient as four masked GEMMs on the tensor cores (wgrad0_mma.cu); needs the s-packed layer-1 input
+// the same gradient as four masked GEMMs on the tensor cores (wgrad0_mma.cu); needs the packed layer-1 input
+// (s-packed for in_channels == 3, rs-packed for in_channels == 1)
 bool wgrad0_mma_supported(int W, int Wp, int CK, int Ci, int Co);
 void wgrad0_mma(const void* X, const void* g, const uint8_t* amax, float* dW, float* ws, int B, int H, int W, int Hp,
-                int Wp, cudaStream_t st);
+                int Wp, int in_channels, cudaStream_t st);
 // ---- general tensor-core GEMMs for the ResNet convolutions (gemm_tcgen05.cu) ----
 // C[rows_out, N] (bf16) = sum_{t < taps} A[m + shifts[t], K] . B[t*N + n, K]^T. padded != 0: A rows index a zero-padded
 // [Bn][H+2][W+2] grid and only interior pixels are written (to the dense [Bn*H*W, N] output). fp8: A and B hold e4m3
@@ -87,7 +90,8 @@ struct ConvLayerTable {
   int64_t wf_off[kMaxConvLayers], wd_off[kMaxConvLayers];     // offsets (elements) into the bf16 Wf / Wd buffers
   int64_t dw_off[kMaxConvLayers];                             // offsets (elements) into the fp32 dW32 buffer
 };
-void preprocess_u8(const uint8_t* x, const float* theta, void* X, int B, int H, int W, uint64_t aug_seed,
+// x: uint8 [B,H,W,C] with C = 3 or 1
+void preprocess_u8(const uint8_t* x, const float* theta, void* X, int B, int H, int W, int C, uint64_t aug_seed,
                    const int64_t* step, int spack, cudaStream_t st);
 void unpool_relu(const void* g, const uint8_t* amax, const void* ypool, void* dY, int B, int H, int W, int Hp,
                  int Wp, int Co, cudaStream_t st);

@@ -76,13 +76,20 @@ inline void chk_bf16(const Tensor& t, const char* n) {
   TORCH_CHECK(t.is_cuda() && t.scalar_type() == at::kBFloat16 && t.is_contiguous(), n, " must be a contiguous CUDA bf16 tensor");
 }
 
+// in_channels: channels of the packed first-layer input (spack): 3 = s-packed, 1 = rs-packed (preprocess_u8)
+inline int packed_taps(bool spack, int64_t in_channels) {
+  TORCH_CHECK(in_channels == 1 || in_channels == 3, "in_channels must be 1 or 3, got ", in_channels);
+  return spack ? (in_channels == 1 ? 1 : 3) : 9;
+}
+
 void conv_fwd_pool(const Tensor& X, const Tensor& Wf, const Tensor& bias, Tensor out,
                    const c10::optional<Tensor>& argmax, int64_t B, int64_t H, int64_t W, int64_t CK, int64_t CO,
-                   bool spack) {
+                   bool spack, int64_t in_channels) {
   chk_bf16(X, "X"); chk_bf16(Wf, "Wf"); chk_bf16(out, "out");
   TORCH_CHECK(X.numel() == B * H * W * CK, "X must be [B*H*W, CK]");
-  TORCH_CHECK(Wf.numel() >= (spack ? 3 : 9) * CO * CK, "Wf must be [9, CO, CK] ([3, CO, CK] s-packed)");
-  TORCH_CHECK(!spack || (CK == 16 && CO == 32), "s-packed input is the 3-channel first layer only");
+  TORCH_CHECK(Wf.numel() >= packed_taps(spack, in_channels) * CO * CK,
+              "Wf must be [9, CO, CK] ([3, CO, CK] s-packed, [1, CO, CK] rs-packed)");
+  TORCH_CHECK(!spack || (CK == 16 && CO == 32), "packed input is the 1- or 3-channel first layer only");
   TORCH_CHECK(bias.is_cuda() && bias.scalar_type() == at::kFloat && bias.numel() == CO, "bias must be float32 [CO]");
   const int64_t Hp = (H - 2) / 2, Wp = (W - 2) / 2;
   TORCH_CHECK(out.numel() == B * Hp * Wp * CO, "out must be [B,Hp,Wp,CO]");
@@ -92,7 +99,7 @@ void conv_fwd_pool(const Tensor& X, const Tensor& Wf, const Tensor& bias, Tensor
     am = argmax->data_ptr<uint8_t>();
   }
   hefl::nn::conv_fwd_pool(X.data_ptr(), Wf.data_ptr(), bias.data_ptr<float>(), out.data_ptr(), am, (int)B, (int)H,
-                          (int)W, (int)CK, (int)CO, spack ? 1 : 0, cur());
+                          (int)W, (int)CK, (int)CO, spack ? 1 : 0, (int)in_channels, cur());
 }
 
 // up_amax given: the un-pooling of the previous layer is fused into the epilogue — dX is then that layer's
@@ -100,10 +107,10 @@ void conv_fwd_pool(const Tensor& X, const Tensor& Wf, const Tensor& bias, Tensor
 // Pair-row forward kernel (conv_tcgen05.cu G1b): same contract as conv_fwd_pool with the plain [9, CO, CK] weights.
 void conv_fwd_pool_pair(const Tensor& X, const Tensor& Wf, const Tensor& bias, Tensor out,
                         const c10::optional<Tensor>& argmax, int64_t B, int64_t H, int64_t W, int64_t CK, int64_t CO,
-                        bool spack) {
+                        bool spack, int64_t in_channels) {
   chk_bf16(X, "X"); chk_bf16(Wf, "Wf"); chk_bf16(out, "out");
-  TORCH_CHECK(X.numel() >= B * H * W * CK && Wf.numel() >= (spack ? 3 : 9) * CO * CK, "shape mismatch");
-  TORCH_CHECK(!spack || (CK == 16 && CO == 32), "s-packed input is the 3-channel first layer only");
+  TORCH_CHECK(X.numel() >= B * H * W * CK && Wf.numel() >= packed_taps(spack, in_channels) * CO * CK, "shape mismatch");
+  TORCH_CHECK(!spack || (CK == 16 && CO == 32), "packed input is the 1- or 3-channel first layer only");
   TORCH_CHECK(hefl::nn::conv_fwd_pool_pair_supported((int)H, (int)W, (int)CK, (int)CO), "conv_fwd_pool_pair: unsupported shape");
   const int64_t Hp = (H - 2) / 2, Wp = (W - 2) / 2;
   TORCH_CHECK(out.numel() == B * Hp * Wp * CO, "out must be [B,Hp,Wp,CO]");
@@ -113,7 +120,7 @@ void conv_fwd_pool_pair(const Tensor& X, const Tensor& Wf, const Tensor& bias, T
     am = argmax->data_ptr<uint8_t>();
   }
   hefl::nn::conv_fwd_pool_pair(X.data_ptr(), Wf.data_ptr(), bias.data_ptr<float>(), out.data_ptr(), am, (int)B, (int)H,
-                               (int)W, (int)CK, (int)CO, spack ? 1 : 0, cur());
+                               (int)W, (int)CK, (int)CO, spack ? 1 : 0, (int)in_channels, cur());
 }
 
 void conv_dgrad(const Tensor& dY, const Tensor& Wd, Tensor dX, int64_t B, int64_t H, int64_t W, int64_t CK,
@@ -144,7 +151,8 @@ void conv_wgrad(const Tensor& X, const Tensor& DY, Tensor dW32, int64_t B, int64
 
 void preprocess_u8(const Tensor& x, const c10::optional<Tensor>& theta, Tensor X, int64_t aug_seed,
                    const c10::optional<Tensor>& step, bool spack) {
-  TORCH_CHECK(x.is_cuda() && x.scalar_type() == at::kByte && x.is_contiguous() && x.dim() == 4 && x.size(3) == 3, "x must be uint8 [B,H,W,3]");
+  TORCH_CHECK(x.is_cuda() && x.scalar_type() == at::kByte && x.is_contiguous() && x.dim() == 4 && (x.size(3) == 3 || x.size(3) == 1),
+              "x must be uint8 [B,H,W,3] or [B,H,W,1]");
   chk_bf16(X, "X");
   const int64_t B = x.size(0), H = x.size(1), W = x.size(2);
   TORCH_CHECK(X.numel() == B * H * W * 16, "X must be [B*H*W, 16]");
@@ -158,7 +166,8 @@ void preprocess_u8(const Tensor& x, const c10::optional<Tensor>& theta, Tensor X
     TORCH_CHECK(step->is_cuda() && step->scalar_type() == at::kLong && step->numel() == 1, "step must be a CUDA int64 scalar tensor");
     sp = step->data_ptr<int64_t>();
   }
-  hefl::nn::preprocess_u8(x.data_ptr<uint8_t>(), th, X.data_ptr(), (int)B, (int)H, (int)W, (uint64_t)aug_seed, sp, spack ? 1 : 0, cur());
+  hefl::nn::preprocess_u8(x.data_ptr<uint8_t>(), th, X.data_ptr(), (int)B, (int)H, (int)W, (int)x.size(3), (uint64_t)aug_seed, sp,
+                          spack ? 1 : 0, cur());
 }
 
 void unpool_relu(const Tensor& g, const Tensor& amax, const Tensor& ypool, Tensor dY, int64_t B, int64_t H,
@@ -240,16 +249,19 @@ void bn_backward(const Tensor& dy, const Tensor& x, const Tensor& y, const Tenso
 
 // Layer-1 weight gradient from the pooled gradient (see wgrad_gather.cu). X: [B*H*W(+slack), 16] bf16,
 // g: [B,Hp,Wp,32] bf16, amax: [B,Hp,Wp,32] u8 (bits 0-1 position, bit 2 active), dW32: [9*16+1, 32] fp32 (+=).
-void wgrad0_gather(const Tensor& X, const Tensor& g, const Tensor& amax, Tensor dW32, int64_t B, int64_t H, int64_t W, bool spack) {
+// spack: X is the packed input of in_channels channels (s-packed for 3, rs-packed for 1) -> masked GEMMs.
+void wgrad0_gather(const Tensor& X, const Tensor& g, const Tensor& amax, Tensor dW32, int64_t B, int64_t H, int64_t W, bool spack,
+                   int64_t in_channels) {
   chk_bf16(X, "X"); chk_bf16(g, "g");
+  packed_taps(spack, in_channels);
   const int64_t Hp = (H - 2) / 2, Wp = (W - 2) / 2;
   TORCH_CHECK(hefl::nn::wgrad0_gather_supported((int)W, (int)Wp, 16, 3, 32), "wgrad0_gather: unsupported shape");
   TORCH_CHECK(X.numel() >= B * H * W * 16 && g.numel() == B * Hp * Wp * 32 && amax.numel() == g.numel(), "shape mismatch");
   TORCH_CHECK(amax.scalar_type() == at::kByte && dW32.scalar_type() == at::kFloat && dW32.numel() >= (9 * 16 + 1) * 32, "dtype / size");
   Tensor ws = at::empty({(int64_t)hefl::nn::wgrad0_parts((int)B, (int)Hp) * hefl::nn::kWgrad0Part}, dW32.options());
-  if (spack && hefl::nn::wgrad0_mma_supported((int)W, (int)Wp, 16, 3, 32)) {      // s-packed input: masked GEMMs on the tensor cores
+  if (spack && hefl::nn::wgrad0_mma_supported((int)W, (int)Wp, 16, 3, 32)) {      // packed input: masked GEMMs on the tensor cores
     hefl::nn::wgrad0_mma(X.data_ptr(), g.data_ptr(), amax.data_ptr<uint8_t>(), dW32.data_ptr<float>(), ws.data_ptr<float>(),
-                         (int)B, (int)H, (int)W, (int)Hp, (int)Wp, cur());
+                         (int)B, (int)H, (int)W, (int)Hp, (int)Wp, (int)in_channels, cur());
     return;
   }
   hefl::nn::wgrad0_gather(X.data_ptr(), g.data_ptr(), amax.data_ptr<uint8_t>(), dW32.data_ptr<float>(), ws.data_ptr<float>(),
@@ -424,8 +436,8 @@ void conv_grad_finalize(Tensor dW32, const Tensor& table, Tensor grad, int64_t l
 TORCH_LIBRARY_FRAGMENT(hefl, m) {
   m.def("adam_step_(Tensor(a!) p, Tensor(b!) g, Tensor(c!) m, Tensor(d!) v, Tensor? shadow, Tensor step, Tensor? lr_scale, float lr, float decay, float beta1, float beta2, float eps) -> ()", &adam_step_);
   m.def("gather_h2d_(Tensor(a!) dst, Tensor src, Tensor indices) -> ()", &gather_h2d_);
-  m.def("conv_fwd_pool(Tensor X, Tensor Wf, Tensor bias, Tensor(a!) out, Tensor(b!)? argmax, int B, int H, int W, int CK, int CO, bool spack=False) -> ()", &conv_fwd_pool);
-  m.def("conv_fwd_pool_pair(Tensor X, Tensor Wf, Tensor bias, Tensor(a!) out, Tensor(b!)? argmax, int B, int H, int W, int CK, int CO, bool spack=False) -> ()", &conv_fwd_pool_pair);
+  m.def("conv_fwd_pool(Tensor X, Tensor Wf, Tensor bias, Tensor(a!) out, Tensor(b!)? argmax, int B, int H, int W, int CK, int CO, bool spack=False, int in_channels=3) -> ()", &conv_fwd_pool);
+  m.def("conv_fwd_pool_pair(Tensor X, Tensor Wf, Tensor bias, Tensor(a!) out, Tensor(b!)? argmax, int B, int H, int W, int CK, int CO, bool spack=False, int in_channels=3) -> ()", &conv_fwd_pool_pair);
   m.def("conv_dgrad(Tensor dY, Tensor Wd, Tensor(a!) dX, int B, int H, int W, int CK, int CO, Tensor? up_amax=None, int up_W=0) -> ()", &conv_dgrad);
   m.def("conv_wgrad(Tensor X, Tensor DY, Tensor(a!) dW32, int B, int H, int W, int CK, int Co) -> ()", &conv_wgrad);
   m.def("preprocess_u8(Tensor x, Tensor? theta, Tensor(a!) X, int aug_seed, Tensor? step, bool spack=False) -> ()", &preprocess_u8);
@@ -435,7 +447,7 @@ TORCH_LIBRARY_FRAGMENT(hefl, m) {
   m.def("conv_set_debug(int mask) -> ()", &conv_set_debug);
   m.def("set_head_cluster(int on) -> ()", [](int64_t on) { g_head_cluster = (int)on; });
   m.def("set_pdl(int on) -> ()", [](int64_t on) { hefl::nn::set_pdl((int)on); });
-  m.def("wgrad0_gather(Tensor X, Tensor g, Tensor amax, Tensor(a!) dW32, int B, int H, int W, bool spack=False) -> ()", &wgrad0_gather);
+  m.def("wgrad0_gather(Tensor X, Tensor g, Tensor amax, Tensor(a!) dW32, int B, int H, int W, bool spack=False, int in_channels=3) -> ()", &wgrad0_gather);
   m.def("fp8_quantize(Tensor x, Tensor(a!) q, Tensor scale, Tensor(b!) amax) -> ()", &fp8_quantize);
   m.def("gemm_taps(Tensor A, Tensor B, Tensor(a!) out, int N, int K, int[] shifts, int padded, int Bn, int H, int W, Tensor? scale_a, Tensor? scale_b) -> ()", &gemm_taps);
   m.def("wgrad_taps(Tensor DY, Tensor X, Tensor(a!) dW, int taps, int Wp) -> ()", &wgrad_taps);

@@ -57,22 +57,16 @@ void adam_step(float* p, float* g, float* m, float* v, void* shadow_bf16, int64_
 namespace hefl {
 namespace nn {
 
-// uint8 NHWC (3 channels) -> bf16 [P,16] (channels 3..15 zero), with 1/255 rescale and an optional per-sample affine warp (Keras shear/zoom/flip,
-// FLPyfhelin.py:80-86) sampled bilinearly with border clamp (torch.grid_sample semantics,
-// align_corners=False).
-__global__ void preprocess_u8_kernel(const uint8_t* __restrict__ x, const float* __restrict__ theta,
-                                     __nv_bfloat16* __restrict__ X, int B, int H, int W, uint64_t aug_seed,
-                                     const int64_t* __restrict__ step, int spack) {
-  pdl_prologue();
-  const int b = blockIdx.y;
-  float tl[6];
+// Per-sample affine warp of the pre-processing: theta[b] if given, else (aug_seed != 0) Keras
+// ImageDataGenerator(shear_range=0.2 deg, zoom_range=0.2, horizontal_flip) drawn per sample from a counter-based
+// generator keyed by (seed, optimiser step, sample). Returns false when the image is not warped.
+__device__ __forceinline__ bool preprocess_theta(const float* __restrict__ theta, uint64_t aug_seed,
+                                                 const int64_t* __restrict__ step, int b, float tl[6]) {
   bool warp_img = theta != nullptr;
   if (theta) {
 #pragma unroll
     for (int i = 0; i < 6; ++i) tl[i] = theta[b * 6 + i];
   } else if (aug_seed != 0) {
-    // Keras ImageDataGenerator(shear_range=0.2 deg, zoom_range=0.2, horizontal_flip) drawn per sample
-    // from a counter-based generator keyed by (seed, optimiser step, sample).
     const uint64_t st = step ? (uint64_t)*step : 0ull;
     const Philox4 r = philox4x32_10((uint32_t)b, (uint32_t)st, (uint32_t)(st >> 32), 7u, (uint32_t)aug_seed,
                                     (uint32_t)(aug_seed >> 32));
@@ -84,6 +78,19 @@ __global__ void preprocess_u8_kernel(const uint8_t* __restrict__ x, const float*
     tl[3] = 0.f; tl[4] = cosf(sh) * zy; tl[5] = 0.f;
     warp_img = true;
   }
+  return warp_img;
+}
+
+// uint8 NHWC (3 channels) -> bf16 [P,16] (channels 3..15 zero), with 1/255 rescale and an optional per-sample affine warp (Keras shear/zoom/flip,
+// FLPyfhelin.py:80-86) sampled bilinearly with border clamp (torch.grid_sample semantics,
+// align_corners=False).
+__global__ void preprocess_u8_kernel(const uint8_t* __restrict__ x, const float* __restrict__ theta,
+                                     __nv_bfloat16* __restrict__ X, int B, int H, int W, uint64_t aug_seed,
+                                     const int64_t* __restrict__ step, int spack) {
+  pdl_prologue();
+  const int b = blockIdx.y;
+  float tl[6];
+  const bool warp_img = preprocess_theta(theta, aug_seed, step, b, tl);
   // One warp = one run of consecutive pixels of an image row. With `spack` (s-packed layer-1 input: channels
   // 0-2 = this pixel, 3-5 = pixel w+1, 6-8 = pixel w+2, so the three horizontal filter taps become part of the
   // GEMM K dimension) a warp stores 30 pixels and lanes 30/31 only feed their values to the shuffles.
@@ -137,14 +144,81 @@ __global__ void preprocess_u8_kernel(const uint8_t* __restrict__ x, const float*
   }
 }
 
-void preprocess_u8(const uint8_t* x, const float* theta, void* X, int B, int H, int W, uint64_t aug_seed,
+// One-channel (grayscale) input: the same scaling, warp and Philox keying as preprocess_u8_kernel. With `spack`
+// it writes the rs-packed layer-1 input: channel 3r + s holds pixel (h + r, w + s), 0 past the bottom or right
+// edge, channels 9..15 zero — the whole 3x3 neighbourhood, so layer 1 is a single K = 16 GEMM. Without it,
+// channel 0 = pixel and the rest zero. Each warp samples its own three rows (h, h+1, h+2) with the code that
+// samples row h + r as channel 0, so channel 3r + s is bit-identical to channel 0 of pixel (h + r, w + s).
+__global__ void preprocess_u8_gray_kernel(const uint8_t* __restrict__ x, const float* __restrict__ theta,
+                                          __nv_bfloat16* __restrict__ X, int B, int H, int W, uint64_t aug_seed,
+                                          const int64_t* __restrict__ step, int spack) {
+  pdl_prologue();
+  const int b = blockIdx.y;
+  float tl[6];
+  const bool warp_img = preprocess_theta(theta, aug_seed, step, b, tl);
+  const int lane = threadIdx.x & 31;
+  const int PW = spack ? 30 : 32;
+  const int NR = spack ? 3 : 1;
+  const int chunks = (W + PW - 1) / PW;
+  const int tasks = H * chunks;
+  const int wpb = blockDim.x >> 5;
+  const uint8_t* img = x + (int64_t)b * H * W;
+  for (int task = blockIdx.x * wpb + (threadIdx.x >> 5); task < tasks; task += gridDim.x * wpb) {
+    const int h = task / chunks;
+    const int w = (task - h * chunks) * PW + lane;
+    const int wc = w < W ? w : W - 1;
+    uint32_t v[3] = {0u, 0u, 0u};                            // bf16 bits of pixel (h + r, w)
+#pragma unroll
+    for (int r = 0; r < 3; ++r) {
+      const int hh = h + r;
+      if (r >= NR || hh >= H) continue;                      // rows below the image: zero
+      float c;
+      if (warp_img) {
+        const float xn = (2.f * wc + 1.f) / W - 1.f, yn = (2.f * hh + 1.f) / H - 1.f;
+        const float sx = tl[0] * xn + tl[1] * yn + tl[2], sy = tl[3] * xn + tl[4] * yn + tl[5];
+        float ix = ((sx + 1.f) * W - 1.f) * 0.5f, iy = ((sy + 1.f) * H - 1.f) * 0.5f;
+        ix = fminf(fmaxf(ix, 0.f), (float)(W - 1));
+        iy = fminf(fmaxf(iy, 0.f), (float)(H - 1));
+        const int x0 = (int)floorf(ix), y0 = (int)floorf(iy);
+        const int x1 = min(x0 + 1, W - 1), y1 = min(y0 + 1, H - 1);
+        const float fx = ix - x0, fy = iy - y0;
+        const float v00 = img[(int64_t)y0 * W + x0], v01 = img[(int64_t)y0 * W + x1];
+        const float v10 = img[(int64_t)y1 * W + x0], v11 = img[(int64_t)y1 * W + x1];
+        c = ((v00 * (1.f - fx) + v01 * fx) * (1.f - fy) + (v10 * (1.f - fx) + v11 * fx) * fy) * (1.f / 255.f);
+      } else {
+        c = (float)img[(int64_t)hh * W + wc] * (1.f / 255.f);
+      }
+      v[r] = w < W ? (uint32_t)__bfloat16_as_ushort(__float2bfloat16(c)) : 0u;   // past the row end: zero
+    }
+    if (spack) {
+      uint32_t k[9];                                         // channel 3r + s = pixel (h + r, w + s)
+#pragma unroll
+      for (int r = 0; r < 3; ++r) {
+        k[3 * r] = v[r];
+        k[3 * r + 1] = __shfl_down_sync(0xffffffffu, v[r], 1);
+        k[3 * r + 2] = __shfl_down_sync(0xffffffffu, v[r], 2);
+      }
+      if (lane < PW && w < W) {
+        uint4* dst = reinterpret_cast<uint4*>(X + ((int64_t)(b * H + h) * W + w) * 16);
+        dst[0] = make_uint4(k[0] | (k[1] << 16), k[2] | (k[3] << 16), k[4] | (k[5] << 16), k[6] | (k[7] << 16));
+        dst[1] = make_uint4(k[8], 0u, 0u, 0u);
+      }
+    } else if (w < W) {
+      uint4* dst = reinterpret_cast<uint4*>(X + ((int64_t)(b * H + h) * W + w) * 16);
+      dst[0] = make_uint4(v[0], 0u, 0u, 0u);
+      dst[1] = make_uint4(0u, 0u, 0u, 0u);
+    }
+  }
+}
+
+void preprocess_u8(const uint8_t* x, const float* theta, void* X, int B, int H, int W, int C, uint64_t aug_seed,
                    const int64_t* step, int spack, cudaStream_t st) {
   const int tasks = H * ((W + (spack ? 29 : 31)) / (spack ? 30 : 32));
   int bx = (tasks + 7) / 8;
   if (bx > 64) bx = 64;
   dim3 grid(bx, B);
-  launch_pdl(preprocess_u8_kernel, dim3(grid), dim3(256), 0, st, x, theta, reinterpret_cast<__nv_bfloat16*>(X), B, H, W,
-             aug_seed, step, spack);
+  launch_pdl(C == 1 ? preprocess_u8_gray_kernel : preprocess_u8_kernel, dim3(grid), dim3(256), 0, st, x, theta,
+             reinterpret_cast<__nv_bfloat16*>(X), B, H, W, aug_seed, step, spack);
   hefl::cuda::note_launch();
 }
 
@@ -222,6 +296,15 @@ __global__ void conv_weight_relayout_kernel(const __nv_bfloat16* __restrict__ sh
   const int l = blockIdx.y + l0;
   const int Ci = t.Ci[l], CK = t.CK[l], Co = t.Co[l];
   const __nv_bfloat16* w = shadow + t.w_off[l];
+  if (l == 0 && spack0 && Ci == 1) {
+    // rs-packed one-channel layer 1: Wf [1][Co][CK], k = 3r + s (the input carries the whole 3x3 neighbourhood)
+    const int nf = Co * CK;
+    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < nf; i += gridDim.x * blockDim.x) {
+      const int k = i % CK, co = i / CK;
+      Wf[t.wf_off[l] + i] = k < 9 ? w[co * 9 + k] : __float2bfloat16(0.f);
+    }
+    return;
+  }
   if (l == 0 && spack0) {
     // s-packed layer 1: Wf [3 filter rows][Co][CK], k = s*Ci + ci (the input carries pixels w, w+1, w+2)
     const int nf = 3 * Co * CK;

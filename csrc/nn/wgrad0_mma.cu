@@ -28,6 +28,10 @@
 //     the split-K buffer the other weight-gradient kernels use. The bias gradient is the sum of the active g,
 //     taken in the mask pass.
 //
+// With the rs-packed one-channel input (channel 3r + s = pixel (h + r, w + s), nn_kernels.cu) the 16 channels of pixel
+// (2i + dy, 2j + dx) already are all nine taps, so each code's GEMM has M = 16 (9 rows used) and a pooled row needs
+// input rows 2i and 2i+1 only (wgrad0_mma_rs_kernel); the partial rows tap * 3 + 0 carry the result.
+//
 // (Why mma.sync and not tcgen05 here: the B operand is produced by the CUDA cores, M x N is 48 x 32 and the
 // kernel is bound by the 116 MB it reads; the legacy tensor path needs no TMEM / descriptor round trip for that.)
 // Reference semantics: Keras Conv2D/MaxPooling2D backward of the first block (FLPyfhelin.py:120-121).
@@ -61,9 +65,14 @@ constexpr int kPartStride = 40;         // floats per row of a parked accumulato
 constexpr int kPart = 48 * kPartStride + 32;   // one warp's tile + its bias sums
 static_assert(8 * kPart * 4 <= kBarOff, "parked tiles must fit in the operand buffers");
 
-__global__ void __launch_bounds__(kT, 2)
-wgrad0_mma_kernel(const __grid_constant__ CUtensorMap tmX, const __nv_bfloat16* __restrict__ g,
-                  const uint8_t* __restrict__ amax, float* __restrict__ ws, int B, int H, int W, int Hp, int Wp) {
+// FR = filter rows that are separate GEMMs: 3 on the s-packed input (M = 3 x 16, a strip reads input rows 2i .. 2i+3),
+// 1 on the rs-packed one-channel input (channel 3r + s = pixel (h + r, w + s): M = 16 with 9 rows used, a strip reads
+// rows 2i and 2i+1 only, so consecutive strips share none).
+template <int FR>
+__device__ __forceinline__ void wgrad0_mma_body(const CUtensorMap& tmX, const __nv_bfloat16* __restrict__ g,
+                                                const uint8_t* __restrict__ amax, float* __restrict__ ws, int B, int H,
+                                                int W, int Hp, int Wp) {
+  constexpr int NR = FR + 1;            // input rows under one pooled row
   extern __shared__ __align__(1024) uint8_t sm[];
   uint8_t* ring = sm;
   uint8_t* gst = ring + kRing * kSlot;
@@ -89,9 +98,9 @@ wgrad0_mma_kernel(const __grid_constant__ CUtensorMap tmX, const __nv_bfloat16* 
   const uint32_t row_bytes = (uint32_t)W * 32u, g_bytes = (uint32_t)Wp * 64u, c_bytes = (uint32_t)Wp * 32u;
   const int pairs = W >> 1;
 
-  float acc[3][4][4];
+  float acc[FR][4][4];
 #pragma unroll
-  for (int r = 0; r < 3; ++r)
+  for (int r = 0; r < FR; ++r)
 #pragma unroll
     for (int n = 0; n < 4; ++n) acc[r][n][0] = acc[r][n][1] = acc[r][n][2] = acc[r][n][3] = 0.f;
   float bsum[8];
@@ -121,20 +130,20 @@ wgrad0_mma_kernel(const __grid_constant__ CUtensorMap tmX, const __nv_bfloat16* 
     const bool pref_next = (s + 1 < s1) && (i + 1 < Hp);
     if (tid == 0) {
       if (!pref) {                                           // first strip of the CTA or of an image: all of it, now
-        mbar_expect_tx(&full[par], 4 * row_bytes + g_bytes + c_bytes);
+        mbar_expect_tx(&full[par], NR * row_bytes + g_bytes + c_bytes);
 #pragma unroll
-        for (int r = 0; r < 4; ++r) tma_load_2d(ring + r * kSlot, &tmX, 0, (b * H + 2 * i + r) * pairs, &full[par]);
+        for (int r = 0; r < NR; ++r) tma_load_2d(ring + r * kSlot, &tmX, 0, (b * H + 2 * i + r) * pairs, &full[par]);
         bulk_load_1d(gst + par * kGst, g + (size_t)s * Wp * 32, g_bytes, &full[par]);
         bulk_load_1d(cst + par * kCst, amax + (size_t)s * Wp * 32, c_bytes, &full[par]);
       }
       if (pref_next) {                                       // the next strip: two new rows, its gradient and codes
         const int q = par ^ 1;
-        int sl4 = head + 4, sl5 = head + 5;
+        int sl4 = head + NR, sl5 = head + NR + 1;
         sl4 = sl4 >= kRing ? sl4 - kRing : sl4;
         sl5 = sl5 >= kRing ? sl5 - kRing : sl5;
         mbar_expect_tx(&full[q], 2 * row_bytes + g_bytes + c_bytes);
-        tma_load_2d(ring + sl4 * kSlot, &tmX, 0, (b * H + 2 * i + 4) * pairs, &full[q]);
-        tma_load_2d(ring + sl5 * kSlot, &tmX, 0, (b * H + 2 * i + 5) * pairs, &full[q]);
+        tma_load_2d(ring + sl4 * kSlot, &tmX, 0, (b * H + 2 * i + NR) * pairs, &full[q]);
+        tma_load_2d(ring + sl5 * kSlot, &tmX, 0, (b * H + 2 * i + NR + 1) * pairs, &full[q]);
         bulk_load_1d(gst + q * kGst, g + (size_t)(s + 1) * Wp * 32, g_bytes, &full[q]);
         bulk_load_1d(cst + q * kCst, amax + (size_t)(s + 1) * Wp * 32, c_bytes, &full[q]);
       }
@@ -185,7 +194,7 @@ wgrad0_mma_kernel(const __grid_constant__ CUtensorMap tmX, const __nv_bfloat16* 
         ldsm_x4_t(Gs_u + c * kGs + b_off0, bq[0]);
         ldsm_x4_t(Gs_u + c * kGs + b_off2, bq[1]);
 #pragma unroll
-        for (int r = 0; r < 3; ++r) {
+        for (int r = 0; r < FR; ++r) {
           int slot = head + dy + r;
           slot = slot >= kRing ? slot - kRing : slot;
           uint32_t a[4];
@@ -208,7 +217,7 @@ wgrad0_mma_kernel(const __grid_constant__ CUtensorMap tmX, const __nv_bfloat16* 
     float* mine = part + warp * kPart;
     const int gq = lane >> 2, tq = lane & 3;
 #pragma unroll
-    for (int r = 0; r < 3; ++r)
+    for (int r = 0; r < FR; ++r)
 #pragma unroll
       for (int n = 0; n < 4; ++n) {
         const int col = n * 8 + 2 * tq;
@@ -228,12 +237,30 @@ wgrad0_mma_kernel(const __grid_constant__ CUtensorMap tmX, const __nv_bfloat16* 
   for (int idx = tid; idx < 28 * 32; idx += kT) {
     const int row = idx >> 5, co = idx & 31;
     // partial row = tap * 3 + ci (as in wgrad0_reduce_kernel), 27 = bias
-    const int src = row < 27 ? ((row / 9) * 16 + row % 9) * kPartStride + co : 48 * kPartStride + co;
     float v = 0.f;
+    if (FR == 3) {
+      const int src = row < 27 ? ((row / 9) * 16 + row % 9) * kPartStride + co : 48 * kPartStride + co;
 #pragma unroll
-    for (int w = 0; w < 8; ++w) v += part[w * kPart + src];
+      for (int w = 0; w < 8; ++w) v += part[w * kPart + src];
+    } else if (row >= 27 || row % 3 == 0) {               // rs: tile row 3r + s holds tap 3r + s of channel 0
+      const int src = row < 27 ? (row / 3) * kPartStride + co : 48 * kPartStride + co;
+#pragma unroll
+      for (int w = 0; w < 8; ++w) v += part[w * kPart + src];
+    }
     ws[(size_t)blockIdx.x * kWgrad0Part + idx] = v;
   }
+}
+
+__global__ void __launch_bounds__(kT, 2)
+wgrad0_mma_kernel(const __grid_constant__ CUtensorMap tmX, const __nv_bfloat16* __restrict__ g,
+                  const uint8_t* __restrict__ amax, float* __restrict__ ws, int B, int H, int W, int Hp, int Wp) {
+  wgrad0_mma_body<3>(tmX, g, amax, ws, B, H, W, Hp, Wp);
+}
+
+__global__ void __launch_bounds__(kT, 2)
+wgrad0_mma_rs_kernel(const __grid_constant__ CUtensorMap tmX, const __nv_bfloat16* __restrict__ g,
+                     const uint8_t* __restrict__ amax, float* __restrict__ ws, int B, int H, int W, int Hp, int Wp) {
+  wgrad0_mma_body<1>(tmX, g, amax, ws, B, H, W, Hp, Wp);
 }
 
 }  // namespace
@@ -265,19 +292,21 @@ void wgrad0_reduce(const float* ws, int parts, float* dW, cudaStream_t st) {
 }
 
 void wgrad0_mma(const void* X, const void* g, const uint8_t* amax, float* dW, float* ws, int B, int H, int W, int Hp,
-                int Wp, cudaStream_t st) {
+                int Wp, int in_channels, cudaStream_t st) {
   static bool attrs_set = false;
   if (!attrs_set) {
-    cudaFuncSetAttribute(wgrad0_mma_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmem);
-    cudaFuncSetAttribute(wgrad0_mma_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, 100);
+    for (auto* k : {wgrad0_mma_kernel, wgrad0_mma_rs_kernel}) {
+      cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmem);
+      cudaFuncSetAttribute(k, cudaFuncAttributePreferredSharedMemoryCarveout, 100);
+    }
     attrs_set = true;
   }
   // X viewed as [pixel pairs][2 x 16 channels]: one box = one image row, 64-byte swizzle
   const CUtensorMap tmX = tensor_map(X, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, {32, (uint64_t)B * H * (W / 2)}, {64},
                                      {32, (uint32_t)(W / 2)}, CU_TENSOR_MAP_SWIZZLE_64B);
   const int grid = wgrad0_parts(B, Hp);
-  launch_pdl(wgrad0_mma_kernel, dim3(grid), dim3(kT), kSmem, st, tmX, reinterpret_cast<const __nv_bfloat16*>(g), amax, ws,
-             B, H, W, Hp, Wp);
+  launch_pdl(in_channels == 1 ? wgrad0_mma_rs_kernel : wgrad0_mma_kernel, dim3(grid), dim3(kT), kSmem, st, tmX,
+             reinterpret_cast<const __nv_bfloat16*>(g), amax, ws, B, H, W, Hp, Wp);
   hefl::cuda::note_launch();
   wgrad0_reduce(ws, grid, dW, st);
 }

@@ -3,8 +3,8 @@
 Replaces Keras' ``model.fit`` compute path (FLPyfhelin.py:118-136, :193) for the medical CNN:
 
   input     preprocess_u8 (uint8 -> bf16 NHWC [P,16], 1/255, Philox affine augmentation; layer-1 input
-            carries pixels w, w+1, w+2 in its channels) into one of two X0 slots — the trainer stages
-            batch i+1 on a side stream while step i runs
+            carries pixels w, w+1, w+2 in its channels for RGB, the whole 3x3 neighbourhood for grayscale)
+            into one of two X0 slots — the trainer stages batch i+1 on a side stream while step i runs
   forward   6 x conv_fwd_pool  (TMA-fed tensor-core tap GEMMs, bias + ReLU + 2x2 max-pool + 3-bit
                                 arg-max/active code fused in the epilogue; only pooled tensors
                                 reach HBM; layer 1 on the pair-row variant: the whole pooling window
@@ -17,7 +17,8 @@ Replaces Keras' ``model.fit`` compute path (FLPyfhelin.py:118-136, :193) for the
             layer 1: wgrad0_gather straight from the pooled gradient (no un-pool, no dY tensor): four
                      masked GEMMs on the tensor cores (wgrad0_mma.cu), FP32-pipe gather as the fallback
   update    conv_grad_finalize + Adam + conv_weight_relayout: layers 2..6 and the head on the side
-            stream under the layer-1 kernel, the 896 layer-1 parameters in the tail (``opt`` hooks)
+            stream under the layer-1 kernel, the 896 (RGB) or 320 (grayscale) layer-1 parameters in the
+            tail (``opt`` hooks)
 
 All buffers are allocated once; a step is CUDA-graph capturable (one graph per input slot); every
 kernel uses programmatic dependent launch (csrc/nn/launch.cuh).
@@ -50,10 +51,12 @@ class MedCNNEngine:
         self.ops.set_pdl(0 if os.environ.get("HEFL_PDL", "1") == "0" else 1)   # programmatic dependent launch
         self.model, self.pack, self.cfg, self.device = model, pack, cfg, device
         B, S = cfg.batch_size, cfg.image_size
-        if cfg.in_channels != 3:
-            raise ValueError("engine expects 3-channel uint8 images")
+        if cfg.in_channels not in (1, 3):
+            raise ValueError(f"the tcgen05 engine supports 1- or 3-channel uint8 images, got in_channels={cfg.in_channels}")
         self.B = B
         convs = list(model.convs)
+        if convs[0].in_channels != cfg.in_channels:
+            raise ValueError(f"model has {convs[0].in_channels} input channels, config {cfg.in_channels}")
         self.n = len(convs)
         offs = {k: o for k, _, o, _ in pack.entries}
         keys = [k for k in pack.keras_order_keys()]
@@ -74,8 +77,9 @@ class MedCNNEngine:
             self.Co.append(co)
             h = (h - 2) // 2
         self.H.append(h)                 # feature map side
-        # layer-1 input carries pixels (w, w+1, w+2) in its 16 channels: 3 tap-GEMMs instead of 9 (conv_tcgen05.cu TS=1)
-        self.spack0 = (os.environ.get("HEFL_SPACK0", "1") != "0" and self.Ci[0] == 3 and self.CK[0] == 16
+        # packed layer-1 input: RGB carries pixels (w, w+1, w+2) in its 16 channels, 3 tap-GEMMs instead of 9
+        # (conv_tcgen05.cu TS=1); grayscale carries the whole 3x3 neighbourhood, one GEMM (rs layout, TS=kTapsRS)
+        self.spack0 = (os.environ.get("HEFL_SPACK0", "1") != "0" and self.Ci[0] in (1, 3) and self.CK[0] == 16
                        and self.Co[0] == 32)
         # un-pool inside the dgrad epilogue: correct (bit-exact test) but measured 10 us/step SLOWER than the
         # separate un-pool kernels (the epilogue is issue-bound; 4x the stores), so off by default
@@ -196,7 +200,7 @@ class MedCNNEngine:
         if train and augment:
             seed = (self.aug_seed + 0x9E3779B97F4A7C15 * (self.prep_count + 1)) & 0x7FFFFFFFFFFFFFFF or 1
             self.prep_count += 1
-        self.ops.preprocess_u8(x_u8, None, self.X0[slot], seed, None, self.spack0)
+        self.ops.preprocess_u8(x_u8, None, self.X0[slot], seed, None, self.spack0)     # channels from x_u8
 
     def forward_convs(self, slot: int, train: bool) -> torch.Tensor:
         x = self.X0[slot]
@@ -205,12 +209,12 @@ class MedCNNEngine:
             if l < self.fwd_pair and h % 2 == 0 and (h - 2) // 2 <= 128 and self.CK[l] <= 32 and self.Co[l] <= 64:
                 self.ops.conv_fwd_pool_pair(x if l else self._x0_bufs[slot], self._wf(l), self.bias[l], self.X[l + 1],
                                             self.amax[l] if train else None, self.B, h, h, self.CK[l], self.Co[l],
-                                            self.spack0 and l == 0)
+                                            self.spack0 and l == 0, self.Ci[0])
                 x = self.X[l + 1]
                 continue
             self.ops.conv_fwd_pool(x, self._wf(l), self.bias[l], self.X[l + 1],
                                    self.amax[l] if train else None, self.B, h, h, self.CK[l], self.Co[l],
-                                   self.spack0 and l == 0)
+                                   self.spack0 and l == 0, self.Ci[0])
             x = self.X[l + 1]
         return self.X[self.n]
 
@@ -236,7 +240,7 @@ class MedCNNEngine:
         ``opt`` (optional) applies the parameter update: ``opt.bump()`` advances the step counter and
         ``opt.apply(lo, hi)`` runs Adam on flat parameters [lo, hi). With two streams, everything but
         layer 1 is updated on the side stream while layer 1's weight-gradient kernel still runs; only
-        the 896 layer-1 parameters are left for the tail of the step."""
+        the layer-1 parameters (896 for RGB, 320 for grayscale) are left for the tail of the step."""
         feat_bf = self.forward_convs(slot, True)
         if self.fused_head:
             self.ops.head_forward_backward(feat_bf, self.pack.flat, self.pack.grad, self.head_offs, y, self.dfeat,
@@ -267,8 +271,9 @@ class MedCNNEngine:
                         self.ops.conv_grad_finalize(self.dW32, self.table, self.pack.grad, 1, self.n)
                         opt.apply(self.p0, self.pack.n_trainable)
                         self.ops.conv_weight_relayout(self.shadow, self.table, self.Wf, self.Wd, 1, self.n)
-                # 3-channel layer: weight gradient gathered straight from the pooled gradient
-                self.ops.wgrad0_gather(self._x0_bufs[slot], g, self.amax[0], self._dw(0), self.B, h, h, self.spack0)
+                # 1- or 3-channel layer: weight gradient gathered straight from the pooled gradient
+                self.ops.wgrad0_gather(self._x0_bufs[slot], g, self.amax[0], self._dw(0), self.B, h, h, self.spack0,
+                                       self.Ci[0])
                 break
             xin = self.X0[slot] if l == 0 else self.X[l]
             if self.dY[l] is None:

@@ -9,9 +9,10 @@ namespace nn {
 // Fused Adam with Keras' legacy time-based decay (FLPyfhelin.py:140):
 //   lr_t = lr * lr_scale / (1 + decay * (t-1)),  t = *step (already incremented)
 // Updates p, m, v in place, zeroes g, optionally writes a bf16 shadow of p.
+// FedProx: with an fp32 anchor (the round's global model) and mu != 0, the gradient is g + mu * (p - anchor).
 void adam_step(float* p, float* g, float* m, float* v, void* shadow_bf16, int64_t n,
                const int64_t* step, const float* lr_scale, float lr, float decay, float beta1,
-               float beta2, float eps, cudaStream_t st);
+               float beta2, float eps, const float* anchor, float mu, cudaStream_t st);
 
 // ---- tensor-core implicit-GEMM convolution (conv_tcgen05.cu) ----
 // spack: the layer-1 input is packed by preprocess_u8 — s-packed when in_channels == 3 (weights [3][CO][16]),
@@ -100,7 +101,8 @@ void conv_weight_relayout(const void* shadow, const ConvLayerTable& t, void* Wf,
 void conv_grad_finalize(float* dW32, const ConvLayerTable& t, float* grad, int l0, int l1, cudaStream_t st);
 void fused_update(float* dW32, const ConvLayerTable& t, float* flat, float* grad, float* m, float* v, void* shadow,
                   void* Wf, void* Wd, const int64_t* step, const float* lr_scale, float lr, float decay, float beta1,
-                  float beta2, float eps, int64_t dense_off, int64_t n_trainable, cudaStream_t st);
+                  float beta2, float eps, int64_t dense_off, int64_t n_trainable, const float* anchor, float mu,
+                  cudaStream_t st);
 
 }  // namespace nn
 }  // namespace hefl

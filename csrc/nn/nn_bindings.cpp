@@ -13,11 +13,18 @@ using at::Tensor;
 
 void adam_step_(Tensor p, Tensor g, Tensor m, Tensor v, const c10::optional<Tensor>& shadow,
                 const Tensor& step, const c10::optional<Tensor>& lr_scale, double lr, double decay,
-                double beta1, double beta2, double eps) {
+                double beta1, double beta2, double eps, const c10::optional<Tensor>& anchor, double mu) {
   TORCH_CHECK(p.scalar_type() == at::kFloat && p.is_contiguous(), "p must be contiguous float32");
   TORCH_CHECK(g.numel() == p.numel() && m.numel() == p.numel() && v.numel() == p.numel(), "size mismatch");
   TORCH_CHECK(step.scalar_type() == at::kLong && step.numel() == 1, "step must be a 1-element int64 tensor");
   const int64_t n = p.numel();
+  // FedProx: the proximal gradient mu * (p - anchor) joins g only with an anchor and mu != 0
+  const float* ap = nullptr;
+  if (anchor.has_value() && (float)mu != 0.0f) {
+    TORCH_CHECK(anchor->scalar_type() == at::kFloat && anchor->is_contiguous() && anchor->numel() == n &&
+                anchor->device() == p.device(), "anchor must be a contiguous float32 tensor like p");
+    ap = anchor->data_ptr<float>();
+  }
   if (p.is_cuda()) {
     void* sh = nullptr;
     if (shadow.has_value()) {
@@ -27,7 +34,7 @@ void adam_step_(Tensor p, Tensor g, Tensor m, Tensor v, const c10::optional<Tens
     hefl::nn::adam_step(p.data_ptr<float>(), g.data_ptr<float>(), m.data_ptr<float>(), v.data_ptr<float>(),
                         sh, n, step.data_ptr<int64_t>(),
                         lr_scale.has_value() ? lr_scale->data_ptr<float>() : nullptr, (float)lr,
-                        (float)decay, (float)beta1, (float)beta2, (float)eps,
+                        (float)decay, (float)beta1, (float)beta2, (float)eps, ap, (float)mu,
                         at::cuda::getCurrentCUDAStream().stream());
     return;
   }
@@ -39,8 +46,10 @@ void adam_step_(Tensor p, Tensor g, Tensor m, Tensor v, const c10::optional<Tens
   float* gp = g.data_ptr<float>();
   float* mp = m.data_ptr<float>();
   float* vp = v.data_ptr<float>();
+  const float muf = (float)mu;
   for (int64_t i = 0; i < n; ++i) {
-    const float gi = gp[i];
+    float gi = gp[i];
+    if (ap) gi += muf * (pp[i] - ap[i]);
     mp[i] = (float)beta1 * mp[i] + (1.0f - (float)beta1) * gi;
     vp[i] = (float)beta2 * vp[i] + (1.0f - (float)beta2) * gi * gi;
     pp[i] -= alpha * mp[i] / (std::sqrt(vp[i]) + (float)eps);
@@ -379,15 +388,23 @@ void fp8_quantize(const Tensor& x, Tensor q, const Tensor& scale, Tensor amax) {
 
 void fused_update(Tensor dW32, const Tensor& table, Tensor flat, Tensor grad, Tensor m, Tensor v, Tensor shadow, Tensor Wf,
                   Tensor Wd, const Tensor& step, const c10::optional<Tensor>& lr_scale, double lr, double decay,
-                  double beta1, double beta2, double eps, int64_t dense_off, int64_t n_trainable) {
+                  double beta1, double beta2, double eps, int64_t dense_off, int64_t n_trainable,
+                  const c10::optional<Tensor>& anchor, double mu) {
   chk_bf16(shadow, "shadow"); chk_bf16(Wf, "Wf"); chk_bf16(Wd, "Wd");
   TORCH_CHECK(flat.scalar_type() == at::kFloat && grad.scalar_type() == at::kFloat && m.scalar_type() == at::kFloat &&
               v.scalar_type() == at::kFloat && dW32.scalar_type() == at::kFloat, "float32 buffers required");
   TORCH_CHECK(step.is_cuda() && step.scalar_type() == at::kLong, "step must be a CUDA int64 tensor");
+  const float* ap = nullptr;
+  if (anchor.has_value() && (float)mu != 0.0f) {
+    TORCH_CHECK(anchor->is_cuda() && anchor->scalar_type() == at::kFloat && anchor->is_contiguous() &&
+                anchor->numel() >= n_trainable, "anchor must be a contiguous float32 CUDA tensor of n_trainable values");
+    ap = anchor->data_ptr<float>();
+  }
   hefl::nn::fused_update(dW32.data_ptr<float>(), table_from(table), flat.data_ptr<float>(), grad.data_ptr<float>(),
                          m.data_ptr<float>(), v.data_ptr<float>(), shadow.data_ptr(), Wf.data_ptr(), Wd.data_ptr(),
                          step.data_ptr<int64_t>(), lr_scale.has_value() ? lr_scale->data_ptr<float>() : nullptr,
-                         (float)lr, (float)decay, (float)beta1, (float)beta2, (float)eps, dense_off, n_trainable, cur());
+                         (float)lr, (float)decay, (float)beta1, (float)beta2, (float)eps, dense_off, n_trainable,
+                         ap, (float)mu, cur());
 }
 
 Tensor umma_shift_probe(const Tensor& A, const Tensor& Bm, int64_t CK, int64_t shift_rows) {
@@ -434,7 +451,7 @@ void conv_grad_finalize(Tensor dW32, const Tensor& table, Tensor grad, int64_t l
 }  // namespace
 
 TORCH_LIBRARY_FRAGMENT(hefl, m) {
-  m.def("adam_step_(Tensor(a!) p, Tensor(b!) g, Tensor(c!) m, Tensor(d!) v, Tensor? shadow, Tensor step, Tensor? lr_scale, float lr, float decay, float beta1, float beta2, float eps) -> ()", &adam_step_);
+  m.def("adam_step_(Tensor(a!) p, Tensor(b!) g, Tensor(c!) m, Tensor(d!) v, Tensor? shadow, Tensor step, Tensor? lr_scale, float lr, float decay, float beta1, float beta2, float eps, Tensor? anchor=None, float mu=0.0) -> ()", &adam_step_);
   m.def("gather_h2d_(Tensor(a!) dst, Tensor src, Tensor indices) -> ()", &gather_h2d_);
   m.def("conv_fwd_pool(Tensor X, Tensor Wf, Tensor bias, Tensor(a!) out, Tensor(b!)? argmax, int B, int H, int W, int CK, int CO, bool spack=False, int in_channels=3) -> ()", &conv_fwd_pool);
   m.def("conv_fwd_pool_pair(Tensor X, Tensor Wf, Tensor bias, Tensor(a!) out, Tensor(b!)? argmax, int B, int H, int W, int CK, int CO, bool spack=False, int in_channels=3) -> ()", &conv_fwd_pool_pair);
@@ -443,7 +460,7 @@ TORCH_LIBRARY_FRAGMENT(hefl, m) {
   m.def("preprocess_u8(Tensor x, Tensor? theta, Tensor(a!) X, int aug_seed, Tensor? step, bool spack=False) -> ()", &preprocess_u8);
   m.def("unpool_relu(Tensor g, Tensor amax, Tensor ypool, Tensor(a!) dY, int B, int H, int W, int Co) -> ()", &unpool_relu);
   m.def("head_forward_backward(Tensor feat, Tensor flat, Tensor(a!) grad, int[] offs, Tensor y, Tensor(b!) dfeat, Tensor(c!) h1_buf, Tensor(d!) dh1_buf, Tensor(e!) out, Tensor(f!)? step, int B, int F, int H1, int H2, int C, bool train) -> ()", &head_forward_backward);
-  m.def("fused_update(Tensor(a!) dW32, Tensor table, Tensor(b!) flat, Tensor(c!) grad, Tensor(d!) m, Tensor(e!) v, Tensor(f!) shadow, Tensor(g!) Wf, Tensor(h!) Wd, Tensor step, Tensor? lr_scale, float lr, float decay, float beta1, float beta2, float eps, int dense_off, int n_trainable) -> ()", &fused_update);
+  m.def("fused_update(Tensor(a!) dW32, Tensor table, Tensor(b!) flat, Tensor(c!) grad, Tensor(d!) m, Tensor(e!) v, Tensor(f!) shadow, Tensor(g!) Wf, Tensor(h!) Wd, Tensor step, Tensor? lr_scale, float lr, float decay, float beta1, float beta2, float eps, int dense_off, int n_trainable, Tensor? anchor=None, float mu=0.0) -> ()", &fused_update);
   m.def("conv_set_debug(int mask) -> ()", &conv_set_debug);
   m.def("set_head_cluster(int on) -> ()", [](int64_t on) { g_head_cluster = (int)on; });
   m.def("set_pdl(int on) -> ()", [](int64_t on) { hefl::nn::set_pdl((int)on); });

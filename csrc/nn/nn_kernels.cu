@@ -13,10 +13,14 @@ namespace nn {
 int g_pdl = 1;
 void set_pdl(int on) { g_pdl = on; }
 
+// PROX: FedProx local objective, the gradient of (mu/2)*||p - anchor||^2 is added to g before the moments
+// (anchor = the round's global model). The extra arguments come last so that <false> keeps today's code.
+template <bool PROX>
 __global__ void adam_kernel(float* __restrict__ p, float* __restrict__ g, float* __restrict__ m,
                             float* __restrict__ v, __nv_bfloat16* __restrict__ shadow, int64_t n,
                             const int64_t* __restrict__ step, const float* __restrict__ lr_scale,
-                            float lr, float decay, float beta1, float beta2, float eps) {
+                            float lr, float decay, float beta1, float beta2, float eps,
+                            const float* __restrict__ anchor, float mu) {
   pdl_wait();   // parameter writer: no early trigger (see launch.cuh)
   const float t = (float)(*step);
   const float lr_t = lr * (lr_scale ? *lr_scale : 1.0f) / (1.0f + decay * (t - 1.0f));
@@ -25,7 +29,8 @@ __global__ void adam_kernel(float* __restrict__ p, float* __restrict__ g, float*
   const float alpha = lr_t * sqrtf(bc2) / bc1;
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n;
        i += (int64_t)gridDim.x * blockDim.x) {
-    const float gi = g[i];
+    float gi = g[i];
+    if (PROX) gi += mu * (p[i] - anchor[i]);
     const float mi = beta1 * m[i] + (1.0f - beta1) * gi;
     const float vi = beta2 * v[i] + (1.0f - beta2) * gi * gi;
     const float pi = p[i] - alpha * mi / (sqrtf(vi) + eps);
@@ -39,12 +44,12 @@ __global__ void adam_kernel(float* __restrict__ p, float* __restrict__ g, float*
 
 void adam_step(float* p, float* g, float* m, float* v, void* shadow_bf16, int64_t n,
                const int64_t* step, const float* lr_scale, float lr, float decay, float beta1,
-               float beta2, float eps, cudaStream_t st) {
+               float beta2, float eps, const float* anchor, float mu, cudaStream_t st) {
   if (n == 0) return;
   int blocks = (int)((n + 255) / 256);
   if (blocks > hefl::cuda::device_sm_count() * 8) blocks = hefl::cuda::device_sm_count() * 8;
-  launch_pdl(adam_kernel, dim3(blocks), dim3(256), 0, st, p, g, m, v, reinterpret_cast<__nv_bfloat16*>(shadow_bf16), n,
-                                      step, lr_scale, lr, decay, beta1, beta2, eps);
+  launch_pdl(anchor && mu != 0.0f ? adam_kernel<true> : adam_kernel<false>, dim3(blocks), dim3(256), 0, st, p, g, m, v,
+             reinterpret_cast<__nv_bfloat16*>(shadow_bf16), n, step, lr_scale, lr, decay, beta1, beta2, eps, anchor, mu);
   hefl::cuda::note_launch();
 }
 
@@ -393,12 +398,14 @@ __device__ __forceinline__ float adam_one(float p, float g, float& mi, float& vi
   return p - alpha * mi / (sqrtf(vi) + eps);
 }
 
+// PROX: the FedProx term of adam_kernel<true>, applied to the conv entries and the dense tail alike.
+template <bool PROX>
 __global__ void fused_update_kernel(float* __restrict__ dW32, const ConvLayerTable t, float* __restrict__ flat,
                                     float* __restrict__ grad, float* __restrict__ m, float* __restrict__ v,
                                     __nv_bfloat16* __restrict__ shadow, __nv_bfloat16* __restrict__ Wf,
                                     __nv_bfloat16* __restrict__ Wd, const int64_t* __restrict__ step,
                                     const float* __restrict__ lr_scale, AdamHyper h, int64_t dense_off,
-                                    int64_t n_trainable) {
+                                    int64_t n_trainable, const float* __restrict__ anchor, float mu) {
   pdl_wait();   // parameter writer: no early trigger (see launch.cuh)
   const float tt = (float)(*step);
   const float lr_t = h.lr * (lr_scale ? *lr_scale : 1.f) / (1.f + h.decay * (tt - 1.f));
@@ -410,7 +417,7 @@ __global__ void fused_update_kernel(float* __restrict__ dW32, const ConvLayerTab
     const int total = (9 * CK + 1) * Co;
     for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < total; i += gridDim.x * blockDim.x) {
       const int R = i / Co, co = i - R * Co;
-      const float g = src[i];
+      float g = src[i];
       src[i] = 0.f;
       int64_t pi;
       int tap = 0, ci = 0;
@@ -422,6 +429,7 @@ __global__ void fused_update_kernel(float* __restrict__ dW32, const ConvLayerTab
         if (ci >= Ci) continue;                      // zero-padded input channels of layer 1
         pi = t.w_off[l] + ((int64_t)co * Ci + ci) * 9 + tap;
       }
+      if (PROX) g += mu * (flat[pi] - anchor[pi]);
       float mi = m[pi], vi = v[pi];
       const float p = adam_one(flat[pi], g, mi, vi, alpha, h.beta1, h.beta2, h.eps);
       flat[pi] = p; m[pi] = mi; v[pi] = vi;
@@ -436,7 +444,9 @@ __global__ void fused_update_kernel(float* __restrict__ dW32, const ConvLayerTab
     for (int64_t i = dense_off + (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n_trainable;
          i += (int64_t)gridDim.x * blockDim.x) {
       float mi = m[i], vi = v[i];
-      const float p = adam_one(flat[i], grad[i], mi, vi, alpha, h.beta1, h.beta2, h.eps);
+      float gi = grad[i];
+      if (PROX) gi += mu * (flat[i] - anchor[i]);
+      const float p = adam_one(flat[i], gi, mi, vi, alpha, h.beta1, h.beta2, h.eps);
       flat[i] = p; m[i] = mi; v[i] = vi;
       grad[i] = 0.f;
       shadow[i] = __float2bfloat16(p);
@@ -446,12 +456,13 @@ __global__ void fused_update_kernel(float* __restrict__ dW32, const ConvLayerTab
 
 void fused_update(float* dW32, const ConvLayerTable& t, float* flat, float* grad, float* m, float* v, void* shadow,
                   void* Wf, void* Wd, const int64_t* step, const float* lr_scale, float lr, float decay, float beta1,
-                  float beta2, float eps, int64_t dense_off, int64_t n_trainable, cudaStream_t st) {
+                  float beta2, float eps, int64_t dense_off, int64_t n_trainable, const float* anchor, float mu,
+                  cudaStream_t st) {
   dim3 grid(48, t.n + 1);
   AdamHyper h{lr, decay, beta1, beta2, eps};
-  launch_pdl(fused_update_kernel, dim3(grid), dim3(256), 0, st, dW32, t, flat, grad, m, v, reinterpret_cast<__nv_bfloat16*>(shadow),
-                                            reinterpret_cast<__nv_bfloat16*>(Wf), reinterpret_cast<__nv_bfloat16*>(Wd),
-                                            step, lr_scale, h, dense_off, n_trainable);
+  launch_pdl(anchor && mu != 0.0f ? fused_update_kernel<true> : fused_update_kernel<false>, dim3(grid), dim3(256), 0, st,
+             dW32, t, flat, grad, m, v, reinterpret_cast<__nv_bfloat16*>(shadow), reinterpret_cast<__nv_bfloat16*>(Wf),
+             reinterpret_cast<__nv_bfloat16*>(Wd), step, lr_scale, h, dense_off, n_trainable, anchor, mu);
   hefl::cuda::note_launch();
 }
 

@@ -6,11 +6,14 @@ process (one process per GPU under ``torchrun``; a single process on CPU or one 
     # CPU plumbing config (BASELINE.json configs[0])
     python -m hefl_b200 --device cpu --model cnn2 --image-size 28 --in-channels 1 --num-classes 10 \\
         --he-preset n2048_l1 --nn-backend cudnn --dtype fp32 --rounds 2
+    # non-IID hospitals: Dirichlet(0.3) label-skew shards, sample-weighted FedAvg, FedProx mu = 0.01
+    torchrun --nproc-per-node 8 -m hefl_b200 --dirichlet-alpha 0.3 --fedavg-weighting samples --fedprox-mu 0.01
 
 Every ``FLConfig`` field is a flag (``--local-epochs 10``) or an environment variable
 (``HEFL_LOCAL_EPOCHS=10``); the reference hard-codes all of them (FLPyfhelin.py:31-36, notebook N:24-32).
 Extra flags: ``--data-dir DIR`` (the reference's ``image/Train`` layout ``DIR/<label>/<file>``: every rank decodes
-its own IID contiguous shard, 10 % of it validates; without it a synthetic set of the configured shape is used),
+its own IID contiguous shard, or with ``--dirichlet-alpha`` its label-skew part of the folder, 10 % of it validates;
+without it a synthetic set of the configured shape is used),
 ``--test-dir DIR`` (same layout; after the last round rank 0 prints the reference's four metrics — weighted
 precision / recall / F1 and accuracy, notebook N:267-270 — of the aggregated model),
 ``--checkpoint PATH`` (written by rank 0 after every round, resumed from if it exists),
@@ -77,7 +80,8 @@ def main(argv=None) -> int:
         from .fl.data import ImageFolderDataset
 
         dataset = ImageFolderDataset(ns.data_dir, cfg.image_size, cfg.in_channels, index=rank, num_clients=world,
-                                     shuffle_seed=cfg.seed, stream=ns.stream_decode)
+                                     shuffle_seed=cfg.seed, stream=ns.stream_decode,
+                                     dirichlet_alpha=cfg.dirichlet_alpha, min_train=cfg.batch_size)
         cfg.num_classes = max(cfg.num_classes, dataset.classes)
     run = FederatedRunner(cfg, rank=rank, world=world, device=device, dataset=dataset)
     if ns.checkpoint and os.path.exists(ns.checkpoint):

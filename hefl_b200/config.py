@@ -70,6 +70,10 @@ class FLConfig:
     debug_precision: bool = False             # also all-reduce the PLAINTEXT updates and record the CKKS error of the
                                               # round (debug only: it defeats the privacy the ciphertext path provides)
     debug_poison: bool = False                # overwrite ciphertext / scratch buffers with a poison pattern between rounds
+    # non-IID clients (DESIGN.md §7)
+    dirichlet_alpha: float = 0.0              # 0: equal IID shards; > 0: Dirichlet(alpha) label-skew shards of one pool
+    fedavg_weighting: str = "uniform"         # uniform (1/K) | samples (n_k / N, McMahan et al.'s FedAvg)
+    fedprox_mu: float = 0.0                   # FedProx coefficient: local loss + (mu/2)*||w - w_global||^2; 0 = plain Adam
     # HE
     he_preset: str = "n4096_l3"
     packing: str = "slots"            # slots (canonical embedding, N/2 per ct) | coeff (N per ct)

@@ -5,7 +5,8 @@
   uint8 NHWC images in pinned host memory with a label-dependent pattern so that training
   has signal.
 * ``shard_range`` is the reference's IID contiguous shard (:75-78, remainder dropped, Q9);
-  ``split_train_val`` is Keras' ``validation_split=0.1`` (:85 — the first 10 % validate).
+  ``split_train_val`` is Keras' ``validation_split=0.1`` (:85 — the first 10 % validate);
+  ``dirichlet_partition`` gives non-IID label-skew shards of unequal size instead.
 * ``BatchFeeder`` streams batches host->device from pinned memory on a copy stream
   (double-buffered), which is what the end-to-end benchmark times.
 """
@@ -45,6 +46,35 @@ def split_train_val(start: int, end: int, val_frac: float = 0.1) -> Tuple[range,
     return range(start + nval, end), range(start, start + nval)
 
 
+def dirichlet_partition(labels, num_clients: int, alpha: float, seed: int, min_train: int = 1,
+                        val_frac: float = 0.1, max_draws: int = 100) -> List[torch.Tensor]:
+    """Label-skew shards: for every class, its indices are permuted and split among the clients at the cut
+    points of proportions drawn from Dirichlet(alpha, ..., alpha). Small alpha gives each client a few dominant
+    classes and unequal sizes; large alpha approaches the pool's class mix. Every client must keep at least
+    ``min_train`` training samples after the ``val_frac`` validation split; otherwise the whole partition is
+    drawn again with ``seed + attempt``. The result depends only on (labels, num_clients, alpha, seed), so every
+    rank computes the same partition without communication. Returns one sorted int64 index tensor per client."""
+    if alpha <= 0:
+        raise ValueError(f"dirichlet_alpha must be > 0 for a label-skew partition, got {alpha}")
+    labels = np.asarray(labels.cpu() if isinstance(labels, torch.Tensor) else labels).reshape(-1)
+    sizes: List[int] = []
+    for attempt in range(max_draws):
+        rng = np.random.default_rng(seed + attempt)
+        parts: List[List[np.ndarray]] = [[] for _ in range(num_clients)]
+        for c in np.unique(labels):
+            idx = rng.permutation(np.flatnonzero(labels == c))
+            cuts = (np.cumsum(rng.dirichlet([alpha] * num_clients))[:-1] * len(idx)).astype(np.int64)
+            for k, piece in enumerate(np.split(idx, cuts)):
+                parts[k].append(piece)
+        out = [np.sort(np.concatenate(p)) for p in parts]
+        sizes = [len(o) for o in out]
+        if all(n - int(n * val_frac) >= min_train for n in sizes):
+            return [torch.from_numpy(o.astype(np.int64)) for o in out]
+    raise ValueError(f"dirichlet_partition: no draw of {max_draws} gave every one of {num_clients} clients "
+                     f"{min_train} training samples (alpha={alpha}, {len(labels)} samples; last client sizes "
+                     f"{sizes}); raise alpha or the pool size, or lower the client count")
+
+
 class SyntheticImageDataset:
     """``n`` uint8 images [n, H, W, C] (pinned when CUDA is present) and int64 labels."""
 
@@ -69,6 +99,15 @@ class SyntheticImageDataset:
         self.n = n
         self.classes = classes
 
+    def subset(self, idx: torch.Tensor, pin: Optional[bool] = None) -> "SyntheticImageDataset":
+        """A dataset of rows ``idx`` of this one (a client's shard of a pooled set)."""
+        out = object.__new__(SyntheticImageDataset)
+        out.images, out.labels = self.images[idx], self.labels[idx]
+        if torch.cuda.is_available() if pin is None else pin:
+            out.images, out.labels = out.images.pin_memory(), out.labels.pin_memory()
+        out.n, out.classes = len(idx), self.classes
+        return out
+
     def __len__(self) -> int:
         return self.n
 
@@ -78,11 +117,13 @@ class ImageFolderDataset:
     this client's IID contiguous shard (:75-78) is decoded once (PIL, bilinear resize to the model's input
     size, :104; a thread pool decodes in parallel) into pinned uint8 NHWC memory, from where ``BatchFeeder``
     streams it to the GPU. Same attributes as ``SyntheticImageDataset``. Class indices come from the sorted
-    label names of the WHOLE folder, so every client agrees on them."""
+    label names of the WHOLE folder, so every client agrees on them. ``dirichlet_alpha > 0`` replaces the
+    contiguous shard by client ``index``'s part of a ``dirichlet_partition`` of the whole shuffled folder's labels
+    (each part keeps at least ``min_train`` training images); only that part is decoded."""
 
     def __init__(self, folder: str, image_size: int = 256, channels: int = 3, index: int = 0, num_clients: int = 1,
                  shuffle_seed: Optional[int] = 0, workers: int = 8, pin: Optional[bool] = None,
-                 stream: bool = False):
+                 stream: bool = False, dirichlet_alpha: float = 0.0, min_train: int = 1):
         from concurrent.futures import ThreadPoolExecutor
 
         df = prep_df(folder, shuffle=shuffle_seed is not None, seed=shuffle_seed)
@@ -90,8 +131,13 @@ class ImageFolderDataset:
             raise FileNotFoundError(f"no images under {folder}/<label>/")
         names = sorted(set(df["Label"]))
         self.class_indices = {l: i for i, l in enumerate(names)}
-        lo, hi = shard_range(len(df), index, num_clients)
-        rows = df.iloc[lo:hi]
+        if dirichlet_alpha > 0:
+            all_labels = np.array([self.class_indices[l] for l in df["Label"]], dtype=np.int64)
+            part = dirichlet_partition(all_labels, num_clients, dirichlet_alpha, shuffle_seed or 0, min_train)[index]
+            rows = df.iloc[part.numpy()]
+        else:
+            lo, hi = shard_range(len(df), index, num_clients)
+            rows = df.iloc[lo:hi]
         self.filenames = list(rows["Path"])
         n = len(self.filenames)
         self.image_size, self.channels = image_size, channels

@@ -9,7 +9,9 @@ One round = what the reference's notebook cell 3 does once (N:233-272):
   single-process simulation),
 * there is an outer round loop (the reference runs exactly one, Q2),
 * the pickle-file "network" and the server loop are replaced by the ciphertext all-reduce,
-* averaging is a sum in ciphertext space with 1/K folded into the decode scale.
+* averaging is a sum in ciphertext space with 1/K folded into the decode scale; with
+  ``fedavg_weighting="samples"`` each client also folds K·n_k/N into its encode scale, so the
+  decrypted result is McMahan et al.'s sample-weighted FedAvg.
 
 Roles: every rank holds the public context; the secret key is generated (OS entropy) and kept by
 the key-holder rank alone (default rank 0), which owns no chunk of the fused all-reduce, decrypts
@@ -32,13 +34,26 @@ from ..he.context import CKKSContext, CtBatch
 from ..models import ParamPack, create_model
 from ..parallel import LoopbackTransport, make_transport
 from ..utils import DeviceTimer, JsonlLogger, StageTimes
-from .data import BatchFeeder, SyntheticImageDataset, shard_range, split_train_val
+from .data import BatchFeeder, SyntheticImageDataset, dirichlet_partition, shard_range, split_train_val
 from .trainer import LocalTrainer
+
+FEDAVG_WEIGHTINGS = ("uniform", "samples")
+
+
+def check_noniid_options(cfg: FLConfig) -> None:
+    """Reject out-of-range non-IID settings (they arrive from flags and environment variables)."""
+    if not cfg.dirichlet_alpha >= 0:
+        raise ValueError(f"dirichlet_alpha must be >= 0 (0 = IID shards), got {cfg.dirichlet_alpha}")
+    if not cfg.fedprox_mu >= 0:
+        raise ValueError(f"fedprox_mu must be >= 0 (0 = plain local Adam), got {cfg.fedprox_mu}")
+    if cfg.fedavg_weighting not in FEDAVG_WEIGHTINGS:
+        raise ValueError(f"fedavg_weighting must be one of {FEDAVG_WEIGHTINGS}, got {cfg.fedavg_weighting!r}")
 
 
 class FederatedRunner:
     def __init__(self, cfg: FLConfig, rank: int = 0, world: int = 1, group=None,
                  device: Optional[torch.device] = None, samples_per_client: Optional[int] = None, dataset=None):
+        check_noniid_options(cfg)
         self.cfg = cfg
         self.rank, self.world, self.group = rank, world, group
         self.device = device or torch.device(cfg.device if torch.cuda.is_available() or cfg.device == "cpu" else "cpu")
@@ -73,11 +88,25 @@ class FederatedRunner:
             self.dataset = dataset
             per = len(dataset)
             nval = int(per * 0.1)
+        elif cfg.dirichlet_alpha > 0:
+            # label-skew shard: this client's Dirichlet part of one pooled set of world x per samples (the pool
+            # and the partition are the same on every rank); 10 % of the part validates
+            per = samples_per_client or (cfg.steps_per_epoch * cfg.batch_size + cfg.val_steps * cfg.batch_size)
+            pool = SyntheticImageDataset(world * per, cfg.image_size, cfg.in_channels, cfg.num_classes,
+                                         seed=cfg.seed, pin=False)
+            part = dirichlet_partition(pool.labels, world, cfg.dirichlet_alpha, cfg.seed, cfg.batch_size)[rank]
+            self.dataset = pool.subset(part)
+            del pool
+            per = len(self.dataset)
+            nval = int(per * 0.1)
         else:
             per = samples_per_client or (cfg.steps_per_epoch * cfg.batch_size + cfg.val_steps * cfg.batch_size)
             self.dataset = SyntheticImageDataset(per, cfg.image_size, cfg.in_channels, cfg.num_classes,
                                                  seed=cfg.seed + 17 * rank)
             nval = cfg.val_steps * cfg.batch_size
+        self.n_train = per - nval                # n_k of sample-weighted FedAvg
+        self.label_counts = torch.bincount(self.dataset.labels[nval:per].long(),
+                                           minlength=int(getattr(self.dataset, "classes", cfg.num_classes))).tolist()
         self.train_feed = BatchFeeder(self.dataset, range(nval, per), cfg.batch_size, self.device,
                                       shuffle=True, seed=cfg.seed + rank)
         self.val_feed = BatchFeeder(self.dataset, range(0, nval), cfg.batch_size, self.device,
@@ -85,6 +114,7 @@ class FederatedRunner:
         self.round = 0
         self.participating = True        # set False to sit a round out (needs cfg.allow_dropouts on every rank)
         self._active = None              # contributors of the current round when dropouts are allowed
+        self._n_total = None             # N = sum of n_k over the round's contributors (sample-weighted FedAvg)
         self.timer = DeviceTimer(self.device)
         self.log = JsonlLogger(cfg.log_jsonl, rank)
         self.global_flat = self.pack.flat.clone()
@@ -165,23 +195,47 @@ class FederatedRunner:
         return float(self.transport.contributors())
 
     def _agree_on_participants(self) -> None:
+        """One all-reduce of [participating, n_k] (float64): the participant count K when dropouts are allowed
+        and the round's total of training samples N for sample-weighted FedAvg."""
         self._active = None
-        if not self.cfg.allow_dropouts or isinstance(self.transport, LoopbackTransport):
+        self._n_total = None
+        weighted = self.cfg.fedavg_weighting == "samples"
+        if not (self.cfg.allow_dropouts or weighted) or isinstance(self.transport, LoopbackTransport):
             return
-        t = torch.tensor([1.0 if self.participating else 0.0], dtype=torch.float32, device=self.device)
+        t = torch.tensor([1.0 if self._takes_part() else 0.0, float(self._my_samples())], dtype=torch.float64,
+                         device=self.device)
         if self.world > 1:
             dist.all_reduce(t, op=dist.ReduceOp.SUM, group=self.group)
-        self._active = int(round(float(t)))
+        t = t.tolist()
+        if self.cfg.allow_dropouts:
+            self._active = int(round(t[0]))
+        if weighted:
+            self._n_total = t[1]
+
+    def _takes_part(self) -> bool:
+        return self.participating or not self.cfg.allow_dropouts
+
+    def _my_samples(self) -> int:
+        """n_k: this client's training samples, 0 when it sits the round out."""
+        return self.n_train if self._takes_part() else 0
+
+    def fedavg_weight(self) -> float:
+        """w_k = K·n_k / N, folded into the encode scale (1.0 for uniform FedAvg). Σ w_k = K, so the aggregate has
+        the magnitude bound of uniform FedAvg; equal shards give exactly 1.0."""
+        n = self._my_samples()
+        if not self._n_total or n == 0:
+            return 1.0
+        return self._contributors() * n / self._n_total
 
     def _my_update(self) -> torch.Tensor:
-        return self.pack.flat if (self.participating or not self.cfg.allow_dropouts) else torch.zeros_like(self.pack.flat)
+        return self.pack.flat if self._takes_part() else torch.zeros_like(self.pack.flat)
 
     def encrypt_update(self) -> CtBatch:
         self._agree_on_participants()
         with self.timer.stage("encrypt"):
             buf = self.transport.buffer(self.ct_numel)
             ct = self.ctx.encrypt(self._my_update(), self.pk, seed=self._encrypt_seed(), packing=self.cfg.packing,
-                                  out=buf)
+                                  out=buf, weight=self.fedavg_weight())
             self._mask(ct.data)
             return ct
 
@@ -222,6 +276,7 @@ class FederatedRunner:
         k = self._contributors()
         if k == 0:
             return
+        weight = self.fedavg_weight()
         seed = self._encrypt_seed()
         # the three streams live as long as the runner: the caching allocator keeps one pool per stream, so
         # fresh streams every round meant fresh cudaMallocs (and cudaFree stalls) every round
@@ -268,7 +323,8 @@ class FederatedRunner:
                 with torch.cuda.stream(s_enc):
                     if timeline is not None:
                         rec["enc0"] = mark(s_enc)
-                    ct = ctx.encrypt(vals, self.pk, seed=seed, packing=self.cfg.packing, out=view, ct_offset=c0)
+                    ct = ctx.encrypt(vals, self.pk, seed=seed, packing=self.cfg.packing, out=view, ct_offset=c0,
+                                     weight=weight)
                     self._mask(ct.data, chunk=ci)
                     ev_enc.append(mark(s_enc))
                 with torch.cuda.stream(s_comm):
@@ -319,12 +375,14 @@ class FederatedRunner:
         if self.cfg.debug_precision and not isinstance(self.transport, LoopbackTransport):
             # plaintext FedAvg oracle (SURVEY.md §5.5 "CKKS precision: max abs error vs plaintext FedAvg")
             # the oracle averages what the encrypted path averages: sitting-out clients contribute zeros and
-            # K is the agreed participant count
+            # K is the agreed participant count; with sample weighting it is sum(n_k x_k) / N
             self._agree_on_participants()
             plain_mean = self._my_update().detach().clone().double()
+            if self._n_total is not None:
+                plain_mean *= self._my_samples()
             if self.world > 1:
                 dist.all_reduce(plain_mean, op=dist.ReduceOp.SUM, group=self.group)
-            kk = self._contributors()
+            kk = self._n_total if self._n_total is not None else self._contributors()
             plain_mean = plain_mean / kk if kk > 0 else None
         if pipelined is None:
             pipelined = self.device.type == "cuda" and self.n_ct > 512 and self.transport.name in ("fused", "nccl", "gloo")
@@ -345,7 +403,8 @@ class FederatedRunner:
             self.guard_finite()
         rec = {"round": self.round, "rank": self.rank, "stage_ms": times,
                "loss": hist[-1].loss if hist else None, "accuracy": hist[-1].accuracy if hist else None,
-               "transport": self.transport.name, "n_ct": self.n_ct, "ct_bytes": self.ct_numel * 8}
+               "transport": self.transport.name, "n_ct": self.n_ct, "ct_bytes": self.ct_numel * 8,
+               "n_train": self.n_train, "fedavg_weight": self.fedavg_weight(), "label_counts": self.label_counts}
         if plain_mean is not None:
             err = float((self.pack.flat.double() - plain_mean).abs().max())
             rec["ckks_max_abs_err"] = err
@@ -443,7 +502,10 @@ def simulate_clients(cfg: FLConfig, device: Optional[torch.device] = None, round
                      drop_client: Optional[int] = None) -> Dict:
     """Single-process simulation of ``cfg.clients`` clients through the loopback transport — the
     reference's own structure (clients = loop iterations, FLPyfhelin.py:184) and our fake
-    backend for tests. Returns the encrypted-FedAvg result and the plaintext FedAvg oracle."""
+    backend for tests. Returns the encrypted-FedAvg result and the plaintext FedAvg oracle. With
+    ``dirichlet_alpha > 0`` the clients hold Dirichlet label-skew parts of the pool; with
+    ``fedavg_weighting="samples"`` client k is weighted by n_k / N in both."""
+    check_noniid_options(cfg)
     device = device or torch.device("cpu")
     torch.manual_seed(cfg.seed)
     hp = cfg.he_params()
@@ -456,6 +518,17 @@ def simulate_clients(cfg: FLConfig, device: Optional[torch.device] = None, round
     K = cfg.clients
     total = K * (cfg.steps_per_epoch + cfg.val_steps) * cfg.batch_size
     ds = SyntheticImageDataset(total, cfg.image_size, cfg.in_channels, cfg.num_classes, seed=cfg.seed, pin=False)
+    if cfg.dirichlet_alpha > 0:
+        splits = []
+        for part in dirichlet_partition(ds.labels, K, cfg.dirichlet_alpha, cfg.seed, cfg.batch_size):
+            nval = int(len(part) * 0.1)
+            splits.append((part[nval:].tolist(), part[:nval].tolist()))
+    else:
+        splits = [split_train_val(*shard_range(total, i, K)) for i in range(K)]
+    kept_ids = [i for i in range(K) if not (drop_client is not None and i == drop_client)]
+    n_k = [len(splits[i][0]) for i in range(K)]
+    n_total = sum(n_k[i] for i in kept_ids)
+    weights = [len(kept_ids) * n_k[i] / n_total if cfg.fedavg_weighting == "samples" else 1.0 for i in range(K)]
     lb = LoopbackTransport(ctx, K)
     global_flat = pack.flat.clone()
     result = {}
@@ -466,13 +539,13 @@ def simulate_clients(cfg: FLConfig, device: Optional[torch.device] = None, round
             if not cfg.compat_sequential_clients:
                 pack.load_flat(global_flat)          # true FedAvg: same starting point
                 trainer.reset_optimizer()
-            s, e = shard_range(total, i, K)
-            tr, va = split_train_val(s, e)
+            tr, va = splits[i]
             tf = BatchFeeder(ds, tr, cfg.batch_size, device, seed=cfg.seed + i)
             vf = BatchFeeder(ds, va, cfg.batch_size, device, seed=cfg.seed + i) if len(va) else None
             trainer.fit(tf, vf, cfg.local_epochs)
             plain.append(pack.flat.clone())
-            ct = ctx.encrypt(pack.flat, pk, seed=cfg.seed * 7919 + rnd * 131 + i, packing=cfg.packing)
+            ct = ctx.encrypt(pack.flat, pk, seed=cfg.seed * 7919 + rnd * 131 + i, packing=cfg.packing,
+                             weight=weights[i])
             if drop_client is not None and i == drop_client:
                 lb.drop(i)
             else:
@@ -480,12 +553,14 @@ def simulate_clients(cfg: FLConfig, device: Optional[torch.device] = None, round
         agg = CtBatch(lb.reduce(), ctx.scale, pack.numel, cfg.packing)
         k = lb.contributors()
         avg = ctx.decrypt(agg, sk, divide_by=float(k))
-        kept = [p for i, p in enumerate(plain) if not (drop_client is not None and i == drop_client)]
-        oracle = torch.stack(kept).mean(0)
+        if cfg.fedavg_weighting == "samples":
+            oracle = (sum(n_k[i] * plain[i].double() for i in kept_ids) / n_total).float()
+        else:
+            oracle = torch.stack([plain[i] for i in kept_ids]).mean(0)
         global_flat = avg.clone()
         pack.load_flat(global_flat)
-        result = {"encrypted_avg": avg, "plain_avg": oracle, "contributors": k,
-                  "max_abs_err": float((avg - oracle).abs().max())}
+        result = {"encrypted_avg": avg, "plain_avg": oracle, "contributors": k, "n_train": n_k,
+                  "fedavg_weights": weights, "max_abs_err": float((avg - oracle).abs().max())}
     result["model"] = model
     result["pack"] = pack
     result["ctx"] = ctx

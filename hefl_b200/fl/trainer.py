@@ -59,6 +59,10 @@ class LocalTrainer:
         self.v = torch.zeros(n, dtype=torch.float32, device=device)
         self.step_t = torch.zeros(1, dtype=torch.int64, device=device)
         self.lr_scale = torch.ones(1, dtype=torch.float32, device=device)
+        # FedProx: the model at the start of fit() (the round's global model); the Adam kernels add mu*(w - anchor)
+        # to the gradient. Allocated once, so captured graphs keep a valid pointer to it.
+        self.mu = float(cfg.fedprox_mu)
+        self.anchor = torch.zeros(n, dtype=torch.float32, device=device) if self.mu > 0 else None
         # "fp8": bf16 autocast + e4m3 GEMMs for the 1x1 convolutions of the ResNets (ops/fp8.py)
         self.amp_dtype = {"bf16": torch.bfloat16, "fp16": torch.float16, "fp32": torch.float32,
                           "fp8": torch.bfloat16}[cfg.dtype]
@@ -151,17 +155,19 @@ class LocalTrainer:
         if hi <= lo:
             return
         self.ops.adam_step_(self.pack.trainable()[lo:hi], self.pack.grad[lo:hi], self.m[lo:hi], self.v[lo:hi],
-                            self.engine.shadow[lo:hi], self.step_t, self.lr_scale, c.lr, c.lr_decay, 0.9, 0.999, 1e-7)
+                            self.engine.shadow[lo:hi], self.step_t, self.lr_scale, c.lr, c.lr_decay, 0.9, 0.999, 1e-7,
+                            self.anchor[lo:hi] if self.anchor is not None else None, self.mu)
 
     def _optimizer_step(self) -> None:
         c = self.cfg
         if self.engine is not None and self.engine.fused_step:
-            self.engine.fused_update(self.m, self.v, self.step_t, self.lr_scale, c)   # step counter bumped by the head kernel
+            # step counter bumped by the head kernel
+            self.engine.fused_update(self.m, self.v, self.step_t, self.lr_scale, c, self.anchor, self.mu)
             return
         self.step_t += 1
         self.ops.adam_step_(self.pack.trainable(), self.pack.grad, self.m, self.v,
                             self.engine.shadow if self.engine is not None else None,
-                            self.step_t, self.lr_scale, c.lr, c.lr_decay, 0.9, 0.999, 1e-7)
+                            self.step_t, self.lr_scale, c.lr, c.lr_decay, 0.9, 0.999, 1e-7, self.anchor, self.mu)
         if self.engine is not None:
             self.engine.after_update()
 
@@ -334,7 +340,10 @@ class LocalTrainer:
             checkpoint_path: Optional[str] = None,
             on_epoch: Optional[Callable[[int, EpochStats], None]] = None) -> List[EpochStats]:
         """The reference's ``model.fit(train_ds, validation_data=val_ds, callbacks=[checkpoint,
-        early, lr_red], epochs=epoch)`` (FLPyfhelin.py:193)."""
+        early, lr_red], epochs=epoch)`` (FLPyfhelin.py:193). With ``fedprox_mu > 0`` the model at entry is the
+        proximal anchor of every update; the reported losses stay the data loss."""
+        if self.anchor is not None:
+            self.anchor.copy_(self.pack.trainable())
         hist: List[EpochStats] = []
         best_loss, best_acc, wait_es, wait_lr = float("inf"), -1.0, 0, 0
         best_weights = None

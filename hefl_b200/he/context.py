@@ -206,10 +206,12 @@ class CKKSContext:
         raise ValueError(f"unknown packing {packing}")
 
     def encrypt(self, vals: torch.Tensor, pk: torch.Tensor, seed: int, packing: str = "slots",
-                out: Optional[torch.Tensor] = None, ct_offset: int = 0) -> CtBatch:
-        """encode + public-key encrypt; ``out`` may be a view of a symmetric-memory buffer."""
+                out: Optional[torch.Tensor] = None, ct_offset: int = 0, weight: float = 1.0) -> CtBatch:
+        """encode + public-key encrypt; ``out`` may be a view of a symmetric-memory buffer. ``weight`` multiplies
+        the values inside the encode (scale Δ·weight) at no cost: the ciphertext carries weight·vals at scale Δ
+        (sample-weighted FedAvg). ``weight=1.0`` encodes exactly as without it."""
         nvals = vals.numel()
-        msg = self.encode(vals, packing)
+        msg = self.encode(vals, packing, scale=self.scale * float(weight))
         C = msg.shape[0]
         if out is None:
             data = self.ops.encrypt(msg, pk, C, self.L, self.logn, self.tables, self.consts, None,

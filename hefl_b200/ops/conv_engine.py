@@ -316,11 +316,13 @@ class MedCNNEngine:
             opt.apply(0, self.pack.n_trainable)
             self.after_update()
 
-    def fused_update(self, m: torch.Tensor, v: torch.Tensor, step: torch.Tensor, lr_scale: torch.Tensor, cfg) -> None:
-        """finalize + Adam + bf16 shadow + tensor-core weight layouts + dW32 clear, one launch."""
+    def fused_update(self, m: torch.Tensor, v: torch.Tensor, step: torch.Tensor, lr_scale: torch.Tensor, cfg,
+                     anchor: Optional[torch.Tensor] = None, mu: float = 0.0) -> None:
+        """finalize + Adam + bf16 shadow + tensor-core weight layouts + dW32 clear, one launch. ``anchor`` and
+        ``mu``: the FedProx term, as in ``adam_step_``."""
         self.ops.fused_update(self.dW32, self.table, self.pack.flat, self.pack.grad, m, v, self.shadow, self.Wf, self.Wd,
                               step, lr_scale, cfg.lr, cfg.lr_decay, 0.9, 0.999, 1e-7, self.dense_off,
-                              self.pack.n_trainable)
+                              self.pack.n_trainable, anchor, mu)
         if self.spack0:
             self.ops.conv_weight_relayout(self.shadow, self.table, self.Wf, self.Wd, 0, 1, True)
 

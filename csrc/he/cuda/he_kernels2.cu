@@ -238,7 +238,7 @@ struct EncArgs {
   uint32_t ct_offset;
   int L;
   int64_t C;
-  uint64_t* scratch;        // N = 16384 only: [grid][N] words for u_hat
+  uint64_t* scratch;        // N = 16384 only: [grid][N] words for u_hat, private to the launch
 };
 
 __device__ __forceinline__ uint32_t pack_e(int e0, int e1) { return ((uint32_t)e0 & 0xFFu) | (((uint32_t)e1 & 0xFFu) << 8); }
@@ -597,16 +597,7 @@ void launch_encrypt2(EncArgs a, cudaStream_t st) {
   const CUtensorMap tmap = rows128_map(a.tw2, (uint64_t)a.L * 2 * N * 16, tw_rows(LOGN) / 2);
   auto k = encrypt2_kernel<LOGN>;
   set_smem(k, Smem<LOGN, NBUF>::kTotal);
-  const int grid = grid_ctas(1);
-  if (LOGN >= 14) {
-    // u_hat of the ciphertext in flight: one row per CTA, allocated once per device (about 17 MB for 132 CTAs), L2 resident
-    static uint64_t* scratch[16] = {nullptr};
-    int dev = 0;
-    cudaGetDevice(&dev);
-    if (!scratch[dev & 15]) cudaMalloc(&scratch[dev & 15], (size_t)device_sm_count() * N * 8);
-    a.scratch = scratch[dev & 15];
-  }
-  k<<<grid, kThreads, Smem<LOGN, NBUF>::kTotal, st>>>(tmap, a);
+  k<<<grid_ctas(1), kThreads, Smem<LOGN, NBUF>::kTotal, st>>>(tmap, a);
 }
 
 template <int LOGN, unsigned CORR>
@@ -668,11 +659,14 @@ bool ntt2(uint64_t* data, int64_t rows, int L, int logn, const uint64_t* tw2, co
   return ok;
 }
 
+int64_t encrypt2_scratch_words(int logn) { return logn >= 14 ? (int64_t)grid_ctas(1) << logn : 0; }
+
 bool encrypt2(const int64_t* msg, const uint64_t* pkx, uint64_t* ct, int64_t C, int L, int logn, const uint64_t* tw2,
               const uint64_t* consts, const uint64_t* msg_scale, uint64_t seed, uint32_t ct_offset, int qbits,
-              cudaStream_t st) {
+              uint64_t* scratch, cudaStream_t st) {
   if (C == 0) return true;
   if (!ntt2_supported(logn, L, qbits)) return false;
+  if (logn >= 14 && scratch == nullptr) return false;
   {
     // A persistent CTA wants at least two units of 8192 coefficients: below that (the 109
     // ciphertexts of the medical CNN) the one-CTA-per-(ciphertext, limb) kernel fills the GPU
@@ -681,7 +675,7 @@ bool encrypt2(const int64_t* msg, const uint64_t* pkx, uint64_t* ct, int64_t C, 
     const int64_t workers = (grid_ctas(1) / 2 / L) * 2;
     if (units < 2 * workers) return false;
   }
-  const EncArgs a{msg, pkx, ct, tw2, consts, msg_scale, seed, ct_offset, L, C, nullptr};
+  const EncArgs a{msg, pkx, ct, tw2, consts, msg_scale, seed, ct_offset, L, C, scratch};
   switch (logn) {
     case 10: launch_encrypt2<10>(a, st); break;
     case 11: launch_encrypt2<11>(a, st); break;

@@ -312,8 +312,12 @@ void encrypt_out(const c10::optional<Tensor>& msg, const Tensor& pk, int64_t C, 
       const TableExt& te = table_ext(tables, consts);
       if (hefl::cuda::ntt2_supported((int)logn, (int)L, te.qbits) && logn <= 14) {
         const Tensor& pkx = key_ext(pk, consts, L);
+        // per-launch scratch from the caching allocator on this stream (as ckks_encode's N = 32768 scratch)
+        Tensor scratch;
+        if (const int64_t words = hefl::cuda::encrypt2_scratch_words((int)logn)) scratch = at::empty({words}, pk.options());
         if (hefl::cuda::encrypt2(mp, u64(pkx), u64(ct), C, (int)L, (int)logn, u64(te.tw2), u64(consts),
-                                 u64o(msg_scale), (uint64_t)seed, (uint32_t)ct_offset, te.qbits, cur_stream()))
+                                 u64o(msg_scale), (uint64_t)seed, (uint32_t)ct_offset, te.qbits,
+                                 scratch.defined() ? u64(scratch) : nullptr, cur_stream()))
           return;
       }
     }

@@ -63,9 +63,13 @@ bool ntt2_supported(int logn, int L, int qbits);
 void set_cta_limits(int ntt, int enc, int dec);
 bool ntt2(uint64_t* data, int64_t rows, int L, int logn, const uint64_t* tw2, const uint64_t* consts, int qbits,
           bool inverse, cudaStream_t st);
+// At N = 16384 the ciphertext in flight keeps NTT(u) in a global row per CTA: `scratch` holds
+// encrypt2_scratch_words(logn) words (0 below N = 16384) and belongs to this launch alone, so that
+// encrypts on different streams cannot overwrite each other's rows.
+int64_t encrypt2_scratch_words(int logn);
 bool encrypt2(const int64_t* msg, const uint64_t* pkx, uint64_t* ct, int64_t C, int L, int logn, const uint64_t* tw2,
               const uint64_t* consts, const uint64_t* msg_scale, uint64_t seed, uint32_t ct_offset, int qbits,
-              cudaStream_t st);
+              uint64_t* scratch, cudaStream_t st);
 bool decrypt2(const uint64_t* ct, const uint64_t* skx, uint64_t* out, int64_t C, int Lct, int k, int logn,
               const uint64_t* tw2, const uint64_t* consts, int Ltab, int qbits, cudaStream_t st);
 

@@ -370,12 +370,46 @@ void crt_center(const uint64_t* res, int64_t C, int k, int n, uint64_t q0, uint6
   note_launch();
 }
 
+// One server-optimizer step on a decoded average a (fp64) at flat index g (DESIGN.md §8). fp32 throughout
+// after d = (float)(a - x); __fmul_rn / __fadd_rn keep nvcc from contracting into FMAs, so the step rounds
+// exactly like its host twin (host::ckks_decode_server_step). sqrtf and '/' are IEEE (no fast-math).
+template <int OPT>
+__device__ __forceinline__ float server_step_one(double a, int64_t g, const ServerStep& s) {
+  if (g >= s.n_trainable) return (float)a;              // BatchNorm running statistics: plain FedAvg
+  const float x = s.x_t[g];
+  const float d = (float)(a - (double)x);
+  float m = s.m[g];
+  if (OPT == kFedAvgM) {
+    m = __fadd_rn(__fmul_rn(s.beta1, m), d);
+    s.m[g] = m;
+    return __fadd_rn(x, __fmul_rn(s.lr, m));
+  }
+  m = __fadd_rn(__fmul_rn(s.beta1, m), __fmul_rn(__fsub_rn(1.0f, s.beta1), d));
+  const float d2 = __fmul_rn(d, d);
+  float v = s.v[g];
+  if (OPT == kFedAdagrad) {
+    v = __fadd_rn(v, d2);
+  } else if (OPT == kFedYogi) {
+    const float t = __fsub_rn(v, d2);
+    const float sg = t > 0.0f ? 1.0f : (t < 0.0f ? -1.0f : 0.0f);
+    v = __fsub_rn(v, __fmul_rn(__fmul_rn(__fsub_rn(1.0f, s.beta2), d2), sg));
+  } else {                                              // kFedAdam
+    v = __fadd_rn(__fmul_rn(s.beta2, v), __fmul_rn(__fsub_rn(1.0f, s.beta2), d2));
+  }
+  s.m[g] = m;
+  s.v[g] = v;
+  return __fadd_rn(x, __fdiv_rn(__fmul_rn(s.lr, m), __fadd_rn(__fsqrt_rn(v), s.tau)));
+}
+
 // Decode straight from decrypted residues: CRT centre -> /(scale*K) -> special FFT -> real part.
-__global__ void __launch_bounds__(1024)
-ckks_decode_res_kernel(const uint64_t* __restrict__ res, const double* __restrict__ coeffs,
-                       int logn, CrtParams p, double inv_scale, const int32_t* __restrict__ rot,
-                       const double2* __restrict__ ksi, float* __restrict__ out_f32,
-                       double* __restrict__ out_f64, int64_t nvals, double2* __restrict__ scratch) {
+// OPT = 0 writes the average; OPT = 1..4 (FedAvgM, FedAdagrad, FedYogi, FedAdam) apply the server step to it
+// in the same pass, so the average itself never goes to memory unless ServerStep::avg_* asks for it.
+template <int OPT>
+__device__ __forceinline__ void decode_res_body(const uint64_t* __restrict__ res, const double* __restrict__ coeffs,
+                                                int logn, const CrtParams& p, double inv_scale,
+                                                const int32_t* __restrict__ rot, const double2* __restrict__ ksi,
+                                                float* __restrict__ out_f32, double* __restrict__ out_f64,
+                                                int64_t nvals, double2* __restrict__ scratch, const ServerStep& sv) {
   extern __shared__ double2 fsm[];
   const int n = 1 << logn, nh = n >> 1, lognh = logn - 1;
   const int64_t c = blockIdx.x;
@@ -396,13 +430,43 @@ ckks_decode_res_kernel(const uint64_t* __restrict__ res, const double* __restric
   }
   __syncthreads();
   fft_special_dev(v, lognh, 2 * n, rot, ksi);
-  for (int i = threadIdx.x; i < nh; i += blockDim.x) {
-    const int64_t g = c * nh + i;
-    if (g < nvals) {
-      if (out_f32) out_f32[g] = (float)v[i].x;
-      if (out_f64) out_f64[g] = v[i].x;
+  if constexpr (OPT == 0) {
+    for (int i = threadIdx.x; i < nh; i += blockDim.x) {
+      const int64_t g = c * nh + i;
+      if (g < nvals) {
+        if (out_f32) out_f32[g] = (float)v[i].x;
+        if (out_f64) out_f64[g] = v[i].x;
+      }
+    }
+  } else {
+    for (int i = threadIdx.x; i < nh; i += blockDim.x) {
+      const int64_t g = c * nh + i;
+      if (g < nvals) {
+        const double a = v[i].x;
+        const int64_t gg = sv.g0 + g;
+        if (sv.avg_f32) sv.avg_f32[gg] = (float)a;
+        if (sv.avg_f64) sv.avg_f64[gg] = a;
+        sv.x_new[gg] = server_step_one<OPT>(a, gg, sv);
+      }
     }
   }
+}
+
+__global__ void __launch_bounds__(1024)
+ckks_decode_res_kernel(const uint64_t* __restrict__ res, const double* __restrict__ coeffs,
+                       int logn, CrtParams p, double inv_scale, const int32_t* __restrict__ rot,
+                       const double2* __restrict__ ksi, float* __restrict__ out_f32,
+                       double* __restrict__ out_f64, int64_t nvals, double2* __restrict__ scratch) {
+  decode_res_body<kFedAvg>(res, coeffs, logn, p, inv_scale, rot, ksi, out_f32, out_f64, nvals, scratch, ServerStep{});
+}
+
+// The decode with a server-optimizer step (OPT = 1..4) in its output loop.
+template <int OPT>
+__global__ void __launch_bounds__(1024)
+ckks_decode_step_kernel(const uint64_t* __restrict__ res, int logn, CrtParams p, double inv_scale,
+                        const int32_t* __restrict__ rot, const double2* __restrict__ ksi, int64_t nvals,
+                        double2* __restrict__ scratch, ServerStep sv) {
+  decode_res_body<OPT>(res, nullptr, logn, p, inv_scale, rot, ksi, nullptr, nullptr, nvals, scratch, sv);
 }
 
 void ckks_decode_residues(const uint64_t* res, int64_t C, int k, int logn, uint64_t q0, uint64_t q1,
@@ -416,6 +480,33 @@ void ckks_decode_residues(const uint64_t* res, int64_t C, int k, int logn, uint6
   ckks_decode_res_kernel<<<(unsigned)C, fft_threads(logn), smem, st>>>(
       res, nullptr, logn, p, inv_scale, rot_group, reinterpret_cast<const double2*>(ksi), out,
       nullptr, nvals_total, logn <= 14 ? nullptr : reinterpret_cast<double2*>(scratch));
+  note_launch();
+}
+
+template <int OPT>
+static void launch_decode_step(const uint64_t* res, int64_t C, int logn, const CrtParams& p, double inv_scale,
+                               const int32_t* rot_group, const double* ksi, int64_t nvals, double* scratch,
+                               const ServerStep& sv, cudaStream_t st) {
+  const size_t smem = logn <= 14 ? (size_t)(1 << (logn - 1)) * 16 : 0;
+  set_smem(ckks_decode_step_kernel<OPT>, smem);
+  ckks_decode_step_kernel<OPT><<<(unsigned)C, fft_threads(logn), smem, st>>>(
+      res, logn, p, inv_scale, rot_group, reinterpret_cast<const double2*>(ksi), nvals,
+      logn <= 14 ? nullptr : reinterpret_cast<double2*>(scratch), sv);
+}
+
+void ckks_decode_server_step(const uint64_t* res, int64_t C, int k, int logn, uint64_t q0, uint64_t q1,
+                             uint64_t q1_ratio_lo, uint64_t q1_ratio_hi, uint64_t q0_inv_q1,
+                             double inv_scale, const int32_t* rot_group, const double* ksi,
+                             int64_t nvals, const ServerStep& sv, int opt, double* scratch, cudaStream_t st) {
+  if (C == 0) return;
+  CrtParams p{q0, q1, q1_ratio_lo, q1_ratio_hi, q0_inv_q1, k};
+  switch (opt) {
+    case kFedAvgM: launch_decode_step<kFedAvgM>(res, C, logn, p, inv_scale, rot_group, ksi, nvals, scratch, sv, st); break;
+    case kFedAdagrad: launch_decode_step<kFedAdagrad>(res, C, logn, p, inv_scale, rot_group, ksi, nvals, scratch, sv, st); break;
+    case kFedYogi: launch_decode_step<kFedYogi>(res, C, logn, p, inv_scale, rot_group, ksi, nvals, scratch, sv, st); break;
+    case kFedAdam: launch_decode_step<kFedAdam>(res, C, logn, p, inv_scale, rot_group, ksi, nvals, scratch, sv, st); break;
+    default: throw std::invalid_argument("ckks_decode_server_step: opt must be 1..4, got " + std::to_string(opt));
+  }
   note_launch();
 }
 

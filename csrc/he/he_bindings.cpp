@@ -293,6 +293,76 @@ Tensor ckks_decode_residues(const Tensor& res, const Tensor& consts_cpu, int64_t
   return full.reshape({-1}).slice(0, 0, nvals).contiguous();
 }
 
+// Decrypted residues [C,k,N] of flat values g0 .. g0 + nvals - 1 -> one server-optimizer step (DESIGN.md §8):
+// x_new = step(x_t, average), m and v updated in place for the indices below n_trainable. One launch on CUDA
+// (ckks_decode_step_kernel<opt>); on CPU the host twin. avg_out (fp32 or fp64) also receives
+// the decoded average.
+void ckks_decode_server_step_(const Tensor& res, const Tensor& consts_cpu, int64_t q0_inv_q1, int64_t logn,
+                              double inv_scale, const Tensor& rot, const Tensor& ksi, int64_t nvals, int64_t g0,
+                              int64_t n_trainable, const Tensor& x_t, Tensor x_new, Tensor m, Tensor v, int64_t opt,
+                              double lr, double beta1, double beta2, double tau,
+                              const c10::optional<Tensor>& avg_out) {
+  TORCH_CHECK(res.dim() == 3, "res must be [C,k,N]");
+  const int64_t C = res.size(0), k = res.size(1), n = res.size(2);
+  TORCH_CHECK(k == 1 || k == 2, "the decode supports 1 or 2 limbs");
+  TORCH_CHECK(n == (1ll << logn), "N mismatch");
+  TORCH_CHECK(consts_cpu.is_cpu(), "consts_cpu must live on the CPU");
+  same_device(res, rot);
+  same_device(res, ksi);
+  TORCH_CHECK(opt >= hefl::kFedAvgM && opt <= hefl::kFedAdam, "opt must be 1 (fedavgm), 2 (fedadagrad), 3 (fedyogi) or 4 (fedadam), got ", opt);
+  TORCH_CHECK(nvals >= 0 && nvals <= C * n / 2, "nvals too large");
+  TORCH_CHECK(g0 >= 0 && n_trainable >= 0, "g0 and n_trainable must be >= 0");
+  const int64_t end = g0 + nvals;
+  const int64_t n_state = std::max<int64_t>(0, std::min(n_trainable, end));
+  auto check_f32 = [&](const Tensor& t, const char* name, int64_t need) {
+    same_device(res, t);
+    TORCH_CHECK(t.scalar_type() == at::kFloat && t.is_contiguous(), name, " must be contiguous float32");
+    TORCH_CHECK(t.numel() >= need, name, " has ", t.numel(), " elements, needs ", need);
+  };
+  check_f32(x_t, "x_t", end);
+  check_f32(x_new, "x_new", end);
+  check_f32(m, "m", n_state);
+  check_f32(v, "v", n_state);
+  hefl::ServerStep sv;
+  sv.x_t = x_t.data_ptr<float>();
+  sv.x_new = x_new.data_ptr<float>();
+  sv.m = m.data_ptr<float>();
+  sv.v = v.data_ptr<float>();
+  if (avg_out.has_value()) {
+    same_device(res, *avg_out);
+    const bool f64 = avg_out->scalar_type() == at::kDouble;
+    TORCH_CHECK((f64 || avg_out->scalar_type() == at::kFloat) && avg_out->is_contiguous(),
+                "avg_out must be contiguous float32 or float64");
+    TORCH_CHECK(avg_out->numel() >= end, "avg_out has ", avg_out->numel(), " elements, needs ", end);
+    if (f64) sv.avg_f64 = avg_out->data_ptr<double>();
+    else sv.avg_f32 = avg_out->data_ptr<float>();
+  }
+  sv.g0 = g0;
+  sv.n_trainable = n_trainable;
+  sv.lr = (float)lr;
+  sv.beta1 = (float)beta1;
+  sv.beta2 = (float)beta2;
+  sv.tau = (float)tau;
+  if (nvals == 0) return;
+  if (res.is_cuda()) {
+    const uint64_t* cc = u64(consts_cpu);
+    Tensor scratch;
+    double* sp = nullptr;
+    if (logn > 14) {
+      scratch = at::empty({C, n / 2, 2}, res.options().dtype(at::kDouble));
+      sp = scratch.data_ptr<double>();
+    }
+    hefl::cuda::ckks_decode_server_step(u64(res), C, (int)k, (int)logn, cc[0], k > 1 ? cc[8] : 1,
+                                        k > 1 ? cc[9] : 0, k > 1 ? cc[10] : 0, (uint64_t)q0_inv_q1, inv_scale,
+                                        rot.data_ptr<int32_t>(), ksi.data_ptr<double>(), nvals, sv, (int)opt, sp,
+                                        cur_stream());
+    return;
+  }
+  Tensor coeffs = crt_center(res, consts_cpu, q0_inv_q1);
+  hefl::host::ckks_decode_server_step(coeffs.data_ptr<double>(), C, (int)logn, inv_scale, rot.data_ptr<int32_t>(),
+                                      ksi.data_ptr<double>(), nvals, sv, (int)opt);
+}
+
 void encrypt_out(const c10::optional<Tensor>& msg, const Tensor& pk, int64_t C, int64_t L, int64_t logn,
                  const Tensor& tables, const Tensor& consts, const c10::optional<Tensor>& msg_scale,
                  int64_t seed, int64_t ct_offset, Tensor ct) {
@@ -525,6 +595,7 @@ TORCH_LIBRARY_FRAGMENT(hefl, m) {
   m.def("crt_center(Tensor res, Tensor consts_cpu, int q0_inv_q1) -> Tensor", &crt_center);
   m.def("ckks_decode(Tensor coeffs, int logn, float inv_scale, Tensor rot, Tensor ksi, bool as_f64) -> Tensor", &ckks_decode);
   m.def("ckks_decode_residues(Tensor res, Tensor consts_cpu, int q0_inv_q1, int logn, float inv_scale, Tensor rot, Tensor ksi, int nvals) -> Tensor", &ckks_decode_residues);
+  m.def("ckks_decode_server_step_(Tensor res, Tensor consts_cpu, int q0_inv_q1, int logn, float inv_scale, Tensor rot, Tensor ksi, int nvals, int g0, int n_trainable, Tensor x_t, Tensor(a!) x_new, Tensor(b!) m, Tensor(c!) v, int opt, float lr, float beta1, float beta2, float tau, Tensor(d!)? avg_out=None) -> ()", &ckks_decode_server_step_);
   m.def("encrypt(Tensor? msg, Tensor pk, int C, int L, int logn, Tensor tables, Tensor consts, Tensor? msg_scale, int seed, int ct_offset) -> Tensor", &encrypt);
   m.def("encrypt_out(Tensor? msg, Tensor pk, int C, int L, int logn, Tensor tables, Tensor consts, Tensor? msg_scale, int seed, int ct_offset, Tensor(a!) out) -> ()", &encrypt_out);
   m.def("decrypt(Tensor ct, Tensor sk, int k, int logn, Tensor tables, Tensor consts) -> Tensor", &decrypt);

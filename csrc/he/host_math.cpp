@@ -321,6 +321,52 @@ void ckks_decode(const double* coeffs, int64_t C, int logn, double inv_scale,
   }
 }
 
+// fp32 step of one value, in the order of server_step_one (he_kernels.cu); fp-contract=off keeps g++ from fusing
+// a multiply-add on targets that have FMA, where the kernel rounds every product and sum on its own.
+__attribute__((optimize("fp-contract=off")))
+static float server_step_one(double a, int64_t g, const ServerStep& s, int opt) {
+  if (g >= s.n_trainable) return (float)a;
+  const float x = s.x_t[g];
+  const float d = (float)(a - (double)x);
+  float m = s.m[g];
+  if (opt == kFedAvgM) {
+    m = s.beta1 * m + d;
+    s.m[g] = m;
+    return x + s.lr * m;
+  }
+  m = s.beta1 * m + (1.0f - s.beta1) * d;
+  const float d2 = d * d;
+  float v = s.v[g];
+  if (opt == kFedAdagrad) {
+    v = v + d2;
+  } else if (opt == kFedYogi) {
+    const float t = v - d2;
+    const float sg = t > 0.0f ? 1.0f : (t < 0.0f ? -1.0f : 0.0f);
+    v = v - ((1.0f - s.beta2) * d2) * sg;
+  } else {
+    v = s.beta2 * v + (1.0f - s.beta2) * d2;
+  }
+  s.m[g] = m;
+  s.v[g] = v;
+  return x + (s.lr * m) / (std::sqrt(v) + s.tau);
+}
+
+void ckks_decode_server_step(const double* coeffs, int64_t C, int logn, double inv_scale,
+                             const int32_t* rot_group, const double* ksi, int64_t nvals,
+                             const ServerStep& sv, int opt) {
+  const int64_t nh = (1ll << logn) / 2;
+  std::vector<double> avg((size_t)(C * nh));
+  ckks_decode(coeffs, C, logn, inv_scale, rot_group, ksi, nullptr, avg.data());
+#pragma omp parallel for schedule(static)
+  for (int64_t g = 0; g < nvals; ++g) {
+    const double a = avg[g];
+    const int64_t gg = sv.g0 + g;
+    if (sv.avg_f32) sv.avg_f32[gg] = (float)a;
+    if (sv.avg_f64) sv.avg_f64[gg] = a;
+    sv.x_new[gg] = server_step_one(a, gg, sv, opt);
+  }
+}
+
 void coeff_encode(const float* vals, int64_t C, int64_t nvals_total, int n, double scale,
                   int64_t* msg) {
 #pragma omp parallel for schedule(static)

@@ -10,6 +10,8 @@
 #include <cstdint>
 #include <vector>
 
+#include "server_step.h"
+
 namespace hefl {
 namespace host {
 
@@ -40,6 +42,11 @@ void ckks_encode(const float* vals_f32, const double* vals_f64, int64_t C, int64
                  int logn, double scale, const int32_t* rot_group, const double* ksi, int64_t* msg);
 void ckks_decode(const double* coeffs, int64_t C, int logn, double inv_scale,
                  const int32_t* rot_group, const double* ksi, float* out_f32, double* out_f64);
+// Twin of cuda::ckks_decode_server_step on CRT-centred coefficients [C][N]: ckks_decode to fp64, then the
+// server step of the first nvals values in the kernel's operation order (opt 1..4, server_step.h).
+void ckks_decode_server_step(const double* coeffs, int64_t C, int logn, double inv_scale,
+                             const int32_t* rot_group, const double* ksi, int64_t nvals,
+                             const ServerStep& sv, int opt);
 void coeff_encode(const float* vals, int64_t C, int64_t nvals_total, int n, double scale,
                   int64_t* msg);
 void encrypt(const int64_t* msg, const uint64_t* pk, uint64_t* ct, int64_t C, int L, int logn,

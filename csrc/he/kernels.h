@@ -8,6 +8,8 @@
 #include <cstdint>
 #include <cuda_runtime.h>
 
+#include "server_step.h"
+
 namespace hefl {
 namespace cuda {
 
@@ -27,6 +29,12 @@ void ckks_decode_residues(const uint64_t* res, int64_t C, int k, int logn, uint6
 void ckks_decode(const double* coeffs, int64_t C, int logn, double inv_scale,
                  const int32_t* rot_group, const double* ksi, float* out_f32, double* out_f64,
                  double* scratch, cudaStream_t st);
+
+// Decode + server-optimizer step (server_step.h, DESIGN.md §8) in one launch; opt 1..4 (ServerOpt).
+void ckks_decode_server_step(const uint64_t* res, int64_t C, int k, int logn, uint64_t q0, uint64_t q1,
+                             uint64_t q1_ratio_lo, uint64_t q1_ratio_hi, uint64_t q0_inv_q1,
+                             double inv_scale, const int32_t* rot_group, const double* ksi,
+                             int64_t nvals, const ServerStep& sv, int opt, double* scratch, cudaStream_t st);
 void coeff_encode(const float* vals, int64_t C, int64_t nvals_total, int n, double scale,
                   int64_t* msg, cudaStream_t st);
 void encrypt(const int64_t* msg, const uint64_t* pk, uint64_t* ct, int64_t C, int L, int logn,

@@ -8,6 +8,8 @@ process (one process per GPU under ``torchrun``; a single process on CPU or one 
         --he-preset n2048_l1 --nn-backend cudnn --dtype fp32 --rounds 2
     # non-IID hospitals: Dirichlet(0.3) label-skew shards, sample-weighted FedAvg, FedProx mu = 0.01
     torchrun --nproc-per-node 8 -m hefl_b200 --dirichlet-alpha 0.3 --fedavg-weighting samples --fedprox-mu 0.01
+    # ... with a server optimizer: FedAdam (eta 0.1, beta1 0.9, beta2 0.99, tau 1e-3) fused into the CKKS decode
+    torchrun --nproc-per-node 8 -m hefl_b200 --dirichlet-alpha 0.3 --server-opt fedadam --server-lr 0.1
 
 Every ``FLConfig`` field is a flag (``--local-epochs 10``) or an environment variable
 (``HEFL_LOCAL_EPOCHS=10``); the reference hard-codes all of them (FLPyfhelin.py:31-36, notebook N:24-32).
@@ -64,7 +66,11 @@ def main(argv=None) -> int:
     if ns.simulate:
         res = simulate_clients(cfg, device=device, rounds=cfg.rounds)
         err = float(res["max_abs_err"]) if "max_abs_err" in res else None
-        print(json.dumps({"mode": "simulate", "clients": cfg.clients, "rounds": cfg.rounds, "max_abs_err_vs_plaintext": err}))
+        out = {"mode": "simulate", "clients": cfg.clients, "rounds": cfg.rounds, "max_abs_err_vs_plaintext": err}
+        if "global" in res:
+            out["server_opt"] = cfg.server_opt
+            out["max_abs_err_global_vs_oracle"] = float((res["global"].double() - res["global_oracle"]).abs().max())
+        print(json.dumps(out))
         return 0
 
     if world > 1:

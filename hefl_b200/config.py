@@ -74,6 +74,12 @@ class FLConfig:
     dirichlet_alpha: float = 0.0              # 0: equal IID shards; > 0: Dirichlet(alpha) label-skew shards of one pool
     fedavg_weighting: str = "uniform"         # uniform (1/K) | samples (n_k / N, McMahan et al.'s FedAvg)
     fedprox_mu: float = 0.0                   # FedProx coefficient: local loss + (mu/2)*||w - w_global||^2; 0 = plain Adam
+    # server optimizer (DESIGN.md §8): the key holder steps the global model along avg - x_t, fused into the decode
+    server_opt: str = "fedavg"                # fedavg (the model becomes the average) | fedavgm | fedadagrad | fedyogi | fedadam
+    server_lr: float = 1.0                    # eta
+    server_momentum: float = 0.9              # beta1
+    server_beta2: float = 0.99                # beta2 (fedyogi, fedadam)
+    server_tau: float = 1e-3                  # tau: adaptivity / epsilon term; v starts at tau^2
     # HE
     he_preset: str = "n4096_l3"
     packing: str = "slots"            # slots (canonical embedding, N/2 per ct) | coeff (N per ct)

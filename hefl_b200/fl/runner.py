@@ -35,6 +35,7 @@ from ..models import ParamPack, create_model
 from ..parallel import LoopbackTransport, make_transport
 from ..utils import DeviceTimer, JsonlLogger, StageTimes
 from .data import BatchFeeder, SyntheticImageDataset, dirichlet_partition, shard_range, split_train_val
+from .server_opt import ServerOptimizer, check_server_options, reference_step
 from .trainer import LocalTrainer
 
 FEDAVG_WEIGHTINGS = ("uniform", "samples")
@@ -54,6 +55,7 @@ class FederatedRunner:
     def __init__(self, cfg: FLConfig, rank: int = 0, world: int = 1, group=None,
                  device: Optional[torch.device] = None, samples_per_client: Optional[int] = None, dataset=None):
         check_noniid_options(cfg)
+        check_server_options(cfg)
         self.cfg = cfg
         self.rank, self.world, self.group = rank, world, group
         self.device = device or torch.device(cfg.device if torch.cuda.is_available() or cfg.device == "cpu" else "cpu")
@@ -117,7 +119,12 @@ class FederatedRunner:
         self._n_total = None             # N = sum of n_k over the round's contributors (sample-weighted FedAvg)
         self.timer = DeviceTimer(self.device)
         self.log = JsonlLogger(cfg.log_jsonl, rank)
-        self.global_flat = self.pack.flat.clone()
+        self.global_flat = self.pack.flat.clone()       # x_t: the global model of the round, snapshot by run_round
+        # server optimizer (DESIGN.md §8): the state lives with whoever decrypts -- the key holder, or every rank
+        # when every rank holds sk (each then applies the same deterministic step)
+        self.server_opt = (ServerOptimizer.from_config(cfg, self.pack.n_trainable, self.device)
+                           if cfg.server_opt != "fedavg" and self.has_sk else None)
+        self._avg_out = None                  # debug_precision with a server step: the decoded average of the round
         self.history: List[Dict] = []
 
     # ------------------------------------------------------------------ keys and randomness
@@ -249,13 +256,19 @@ class FederatedRunner:
             k = self._contributors()
             if k == 0:                                       # nobody took part: keep the current global model
                 return
-            if self.has_sk:
+            if self.server_opt is not None:
+                # x_{t+1} = step(x_t, average): decoded and stepped in one launch, broadcast where the average was
+                avg = torch.empty_like(self.pack.flat)
+                self.server_opt.step(self.ctx, agg, self.sk, float(k), self.global_flat, avg, avg_out=self._avg_out)
+            elif self.has_sk:
                 avg = self.ctx.decrypt(agg, self.sk, divide_by=float(k))
             else:
                 avg = torch.empty_like(self.pack.flat)
             if self.key_holder >= 0:
                 avg = avg.to(self.pack.flat.dtype).contiguous()
                 dist.broadcast(avg, src=self.key_holder, group=self.group)
+                if self._avg_out is not None:
+                    dist.broadcast(self._avg_out, src=self.key_holder, group=self.group)
             self.pack.load_flat(avg)
             if self.trainer.engine is not None:
                 self.trainer.engine.after_restore()
@@ -278,6 +291,8 @@ class FederatedRunner:
             return
         weight = self.fedavg_weight()
         seed = self._encrypt_seed()
+        if self.server_opt is not None:
+            self.server_opt.ensure_state()               # on the current stream, before the three streams fork
         # the three streams live as long as the runner: the caching allocator keeps one pool per stream, so
         # fresh streams every round meant fresh cudaMallocs (and cudaFree stalls) every round
         if getattr(self, "_pipe_streams", None) is None:
@@ -337,7 +352,10 @@ class FederatedRunner:
                     s_dec.wait_event(ev_comm[ci])
                     if timeline is not None:
                         rec["dec0"] = mark(s_dec)
-                    if self.has_sk:
+                    if self.server_opt is not None:
+                        self.server_opt.step(ctx, CtBatch(data, ct.scale, ct.nvals, ct.packing), self.sk, k,
+                                             self.global_flat, out, offset=c0 * vpc, avg_out=self._avg_out)
+                    elif self.has_sk:
                         avg = ctx.decrypt(CtBatch(data, ct.scale, ct.nvals, ct.packing), self.sk, divide_by=k)
                         out[c0 * vpc: c0 * vpc + avg.numel()].copy_(avg)
                     if timeline is not None:
@@ -361,6 +379,8 @@ class FederatedRunner:
                                    "unit": "ms since the start of the FedAvg stage", "chunks": rows}, f, indent=1)
             if self.key_holder >= 0:
                 dist.broadcast(out, src=self.key_holder, group=self.group)
+                if self._avg_out is not None:
+                    dist.broadcast(self._avg_out, src=self.key_holder, group=self.group)
             self.pack.load_flat(out)
 
     def guard_finite(self) -> None:
@@ -370,8 +390,10 @@ class FederatedRunner:
 
     # ------------------------------------------------------------------ round
     def run_round(self, check: bool = False, pipelined: Optional[bool] = None) -> Dict:
+        self.global_flat.copy_(self.pack.flat)       # x_t of the server step
         hist = self.local_train()
         plain_mean = None
+        self._avg_out = None
         if self.cfg.debug_precision and not isinstance(self.transport, LoopbackTransport):
             # plaintext FedAvg oracle (SURVEY.md §5.5 "CKKS precision: max abs error vs plaintext FedAvg")
             # the oracle averages what the encrypted path averages: sitting-out clients contribute zeros and
@@ -384,6 +406,9 @@ class FederatedRunner:
                 dist.all_reduce(plain_mean, op=dist.ReduceOp.SUM, group=self.group)
             kk = self._n_total if self._n_total is not None else self._contributors()
             plain_mean = plain_mean / kk if kk > 0 else None
+            if plain_mean is not None and self.cfg.server_opt != "fedavg":
+                # the error is the decoded average's, not the stepped model's: the decode also writes it here
+                self._avg_out = torch.empty_like(self.pack.flat)
         if pipelined is None:
             pipelined = self.device.type == "cuda" and self.n_ct > 512 and self.transport.name in ("fused", "nccl", "gloo")
         if pipelined:
@@ -404,9 +429,11 @@ class FederatedRunner:
         rec = {"round": self.round, "rank": self.rank, "stage_ms": times,
                "loss": hist[-1].loss if hist else None, "accuracy": hist[-1].accuracy if hist else None,
                "transport": self.transport.name, "n_ct": self.n_ct, "ct_bytes": self.ct_numel * 8,
-               "n_train": self.n_train, "fedavg_weight": self.fedavg_weight(), "label_counts": self.label_counts}
+               "n_train": self.n_train, "fedavg_weight": self.fedavg_weight(), "label_counts": self.label_counts,
+               "server_opt": self.cfg.server_opt}
         if plain_mean is not None:
-            err = float((self.pack.flat.double() - plain_mean).abs().max())
+            avg = self._avg_out if self._avg_out is not None else self.pack.flat
+            err = float((avg.double() - plain_mean).abs().max())
             rec["ckks_max_abs_err"] = err
             rec["ckks_precision_bits"] = float(-math.log2(err)) if err > 0 else float("inf")
         self.history.append(rec)
@@ -459,7 +486,8 @@ class FederatedRunner:
         if self.rank == 0:
             torch.save({"round": self.round, "flat": self.pack.flat.detach().cpu(), "config": self.cfg.to_json()}, path)
         torch.save({"round": self.round, "opt": self.trainer.state_dict(), "rng": torch.get_rng_state(),
-                    "cuda_rng": torch.cuda.get_rng_state(self.device) if self.device.type == "cuda" else None},
+                    "cuda_rng": torch.cuda.get_rng_state(self.device) if self.device.type == "cuda" else None,
+                    "server": self.server_opt.state_dict() if self.server_opt is not None else None},
                    f"{path}.rank{self.rank}")
 
     def load_checkpoint(self, path: str) -> None:
@@ -473,8 +501,15 @@ class FederatedRunner:
             torch.set_rng_state(st["rng"])
             if st.get("cuda_rng") is not None and self.device.type == "cuda":
                 torch.cuda.set_rng_state(st["cuda_rng"], self.device)
+            if self.server_opt is not None:          # the server state sits in the key holder's own file
+                if st.get("server") is not None:
+                    self.server_opt.load_state_dict(st["server"])
+                else:
+                    self.server_opt.reset()
         else:                                       # no state of this rank (e.g. a different world size): start it fresh
             self.trainer.reset_optimizer()
+            if self.server_opt is not None:
+                self.server_opt.reset()
         if self.trainer.engine is not None:
             self.trainer.engine.after_restore()
 
@@ -504,8 +539,12 @@ def simulate_clients(cfg: FLConfig, device: Optional[torch.device] = None, round
     reference's own structure (clients = loop iterations, FLPyfhelin.py:184) and our fake
     backend for tests. Returns the encrypted-FedAvg result and the plaintext FedAvg oracle. With
     ``dirichlet_alpha > 0`` the clients hold Dirichlet label-skew parts of the pool; with
-    ``fedavg_weighting="samples"`` client k is weighted by n_k / N in both."""
+    ``fedavg_weighting="samples"`` client k is weighted by n_k / N in both. With a ``server_opt`` other than
+    fedavg the fused decode steps the global model along the average: ``global`` is the new model and
+    ``global_oracle`` the float64 step (``server_opt.reference_step``) of the plaintext average from the same x_t;
+    ``encrypted_avg`` / ``plain_avg`` / ``max_abs_err`` keep describing the average."""
     check_noniid_options(cfg)
+    check_server_options(cfg)
     device = device or torch.device("cpu")
     torch.manual_seed(cfg.seed)
     hp = cfg.he_params()
@@ -531,6 +570,10 @@ def simulate_clients(cfg: FLConfig, device: Optional[torch.device] = None, round
     weights = [len(kept_ids) * n_k[i] / n_total if cfg.fedavg_weighting == "samples" else 1.0 for i in range(K)]
     lb = LoopbackTransport(ctx, K)
     global_flat = pack.flat.clone()
+    sopt = ServerOptimizer.from_config(cfg, pack.n_trainable, device) if cfg.server_opt != "fedavg" else None
+    if sopt is not None:
+        ref_m = torch.zeros(pack.n_trainable, dtype=torch.float64, device=device)
+        ref_v = torch.full((pack.n_trainable,), sopt.hp["tau"] ** 2, dtype=torch.float64, device=device)
     result = {}
     for rnd in range(rounds):
         lb.reset()
@@ -552,15 +595,27 @@ def simulate_clients(cfg: FLConfig, device: Optional[torch.device] = None, round
                 lb.contribute(i, ct.data)
         agg = CtBatch(lb.reduce(), ctx.scale, pack.numel, cfg.packing)
         k = lb.contributors()
-        avg = ctx.decrypt(agg, sk, divide_by=float(k))
+        if sopt is None:
+            avg = ctx.decrypt(agg, sk, divide_by=float(k))
+        else:
+            avg = torch.empty_like(global_flat)
+            new = torch.empty_like(global_flat)
+            sopt.step(ctx, agg, sk, float(k), global_flat, new, avg_out=avg)
         if cfg.fedavg_weighting == "samples":
             oracle = (sum(n_k[i] * plain[i].double() for i in kept_ids) / n_total).float()
         else:
             oracle = torch.stack([plain[i] for i in kept_ids]).mean(0)
-        global_flat = avg.clone()
+        step_info = {}
+        if sopt is not None:
+            # the oracle of the step: float64, on the plaintext average, from the same x_t
+            g_oracle = reference_step(cfg.server_opt, sopt.hp, global_flat, oracle, ref_m, ref_v, pack.n_trainable)
+            step_info = {"global": new, "global_oracle": g_oracle}
+            global_flat = new.clone()
+        else:
+            global_flat = avg.clone()
         pack.load_flat(global_flat)
         result = {"encrypted_avg": avg, "plain_avg": oracle, "contributors": k, "n_train": n_k,
-                  "fedavg_weights": weights, "max_abs_err": float((avg - oracle).abs().max())}
+                  "fedavg_weights": weights, "max_abs_err": float((avg - oracle).abs().max()), **step_info}
     result["model"] = model
     result["pack"] = pack
     result["ctx"] = ctx

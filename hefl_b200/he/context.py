@@ -244,6 +244,27 @@ class CKKSContext:
         coeffs = self.ops.crt_center(res, self.consts_cpu, self.q0_inv_q1)
         return (coeffs.reshape(-1)[: ct.nvals] * inv).float()
 
+    def decrypt_server_step(self, ct: CtBatch, sk: torch.Tensor, divide_by: float, x_t: torch.Tensor,
+                            x_new: torch.Tensor, m: torch.Tensor, v: torch.Tensor, opt, hp, n_trainable: int,
+                            offset: int = 0, avg_out: Optional[torch.Tensor] = None) -> None:
+        """``decrypt`` fused with a server-optimizer step (hefl_b200.fl.server_opt, DESIGN.md §8): the batch holds
+        flat values ``offset .. offset + ct.nvals - 1`` of a model; for each, the decoded average ``a`` and the
+        round's starting weight ``x_t[g]`` give ``x_new[g]``, and ``m`` / ``v`` (``n_trainable`` fp32 entries) are
+        updated in place. ``opt`` is a name or code of ``SERVER_OPTS`` (not fedavg); ``hp`` holds lr, beta1,
+        beta2 and tau. ``avg_out`` (fp32 or fp64, indexed like ``x_new``) also receives the average."""
+        if ct.packing != "slots":
+            raise ValueError("the server-optimizer step is fused into the slot decode; coefficient packing is "
+                             "not supported")
+        if isinstance(opt, str):
+            from ..fl.server_opt import SERVER_OPTS
+            opt = SERVER_OPTS[opt]
+        res = self.decrypt_residues(ct, sk)
+        inv = 1.0 / (ct.scale * divide_by)
+        self.ops.ckks_decode_server_step_(res, self.consts_cpu, self.q0_inv_q1, self.logn, inv, self.rot, self.ksi,
+                                          ct.nvals, int(offset), int(n_trainable), x_t, x_new, m, v, int(opt),
+                                          float(hp["lr"]), float(hp["beta1"]), float(hp["beta2"]), float(hp["tau"]),
+                                          avg_out)
+
     def decode(self, coeffs: torch.Tensor, scale: float, as_f64: bool = False) -> torch.Tensor:
         return self.ops.ckks_decode(coeffs.contiguous(), self.logn, 1.0 / scale, self.rot, self.ksi, as_f64)
 

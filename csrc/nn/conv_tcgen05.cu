@@ -520,19 +520,19 @@ void conv_dgrad(const void* dY, const void* Wd, void* dX, int B, int H, int W, i
 // shuffles, every lane stores a full 16-byte pooled pixel chunk. Restricted to CK <= 32 (one swizzle atom per
 // pair-row) and CO <= 64 (4 accumulators in registers).
 // ------------------------------------------------------------------------------------------
-template <int CK, int CO, int NSEG_ = 4>
+template <int CK, int CO, int NSEG_ = 4, int SEG_BYTES_ = 136 * 2 * CK * 2, int NBUF_ = 2>
 struct PairFwdCfg {
   static constexpr int ROW_BYTES = 2 * CK * 2;            // one pair-row: 2 pixels x CK channels, 64 or 128 B
   static constexpr int NSEG = NSEG_;                      // image rows 2hp .. 2hp+3 (2hp, 2hp+1 on the rs layout)
   static constexpr int SEG_ROWS = 136;                    // 130 pair-rows used (128 windows + shift 1 + slack)
-  static constexpr int SEG_BYTES = SEG_ROWS * ROW_BYTES;
+  static constexpr int SEG_BYTES = SEG_BYTES_;
   static constexpr int HALO = NSEG * SEG_BYTES;
   static constexpr int W_ROW = CK * 2;                    // weight rows: [tap][CO][CK], 32 or 64 B (as G1)
   static constexpr int W_TAP = CO * W_ROW;
   static constexpr int W_BYTES = 9 * W_TAP;
   static constexpr int BAR_BYTES = 384;
   static constexpr int SCR_BYTES = 8 * 1024;
-  static constexpr int NBUF = 2;
+  static constexpr int NBUF = NBUF_;
   static constexpr int SMEM = W_BYTES + NBUF * HALO + SCR_BYTES + BAR_BYTES + 1024;
   static constexpr int NACC = 4;
   static constexpr int NG = 2;                            // 8-channel chunks per warp and pass
@@ -559,15 +559,27 @@ struct PairFwdArgs {
 //   kPairRS    : rs-packed one-channel layer-1 input (channel 3r + s = pixel (y + r, x + s)): one filter row,
 //                acc(dy,dx)[j] = X[row 2hp+dy, pair-row j, half dx] . W — one MMA k-step per accumulator on a
 //                2-row halo.
+//   kPairC     : compact RGB layer-1 input, 8 bytes per pixel (R, G, B, 0). Each of the 4 halo rows lands as one plain
+//                row segment (a 1-D bulk copy, pixel p at byte 8p), and the 32 bytes at 16j are pixels 2j .. 2j+3: one
+//                K = 16 row of window j holding the taps of both its columns. A fragments are those overlapping rows
+//                (16-byte row stride, so an 8-row ldmatrix phase reads 128 contiguous bytes: no bank conflicts, no
+//                swizzle); the column parity dx is in the weights ([3 r][2 dx][CO][16], slot s + dx = tap s), so one
+//                A fragment feeds both dx accumulators. Same MMAs as kPairS, a third of its A loads, a quarter of its
+//                halo bytes.
 // Warp roles as in G1: warps 0..7 compute + epilogue (lane = window, quadrant = warp % 4, chunks by warp / 4),
 // warp 8 is the TMA producer.
-constexpr int kPairPlain = 0, kPairS = 1, kPairRS = 2;
+constexpr int kPairPlain = 0, kPairS = 1, kPairRS = 2, kPairC = 3;
+// compact segment: one image row of <= 256 pixels x 8 B, plus zeroed slack for the 16 bytes window 127 reads past it
+constexpr int kPairCSeg = 2048 + 128;
+constexpr int kPairCBuf = 4;
 
 template <int CK, int CO, int PK>
-using PairCfgOf = PairFwdCfg<CK, CO, PK == kPairRS ? 2 : 4>;
+using PairCfgOf = PairFwdCfg<CK, CO, PK == kPairRS ? 2 : 4, PK == kPairC ? kPairCSeg : 136 * 2 * CK * 2,
+                             PK == kPairC ? kPairCBuf : 2>;
 
 template <int CK, int CO, int PK>
-__device__ __forceinline__ void pair_fwd_body(const CUtensorMap& tmA, const CUtensorMap& tmW, const PairFwdArgs& a) {
+__device__ __forceinline__ void pair_fwd_body(const CUtensorMap* tmA, const CUtensorMap& tmW, const PairFwdArgs& a,
+                                              const __nv_bfloat16* __restrict__ xc = nullptr) {
   using Cfg = PairCfgOf<CK, CO, PK>;
   constexpr bool SP = PK == kPairS;
   constexpr int RB = Cfg::ROW_BYTES;
@@ -584,8 +596,14 @@ __device__ __forceinline__ void pair_fwd_body(const CUtensorMap& tmA, const CUte
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
 
+  if constexpr (PK == kPairC) {
+    // the slack past a row segment is never written by a copy but read by the windows past the pooled row's end
+    for (int i = threadIdx.x; i < Cfg::NBUF * Cfg::HALO / 16; i += blockDim.x)
+      reinterpret_cast<uint4*>(sA)[i] = make_uint4(0u, 0u, 0u, 0u);
+    fence_proxy_async();
+  }
   if (warp == 8 && lane == 0) {
-    prefetch_tmap(&tmA);
+    if constexpr (PK != kPairC) prefetch_tmap(tmA);
     prefetch_tmap(&tmW);
     for (int s = 0; s < Cfg::NBUF; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 8); }
     mbar_init(wfull, 1);
@@ -594,7 +612,7 @@ __device__ __forceinline__ void pair_fwd_body(const CUtensorMap& tmA, const CUte
   __syncthreads();
   pdl_trigger();
   if (warp == 8 && elect_one()) {
-    constexpr int NTAPW = PK == kPairRS ? 1 : (SP ? 3 : 9);
+    constexpr int NTAPW = PK == kPairRS ? 1 : (PK == kPairC ? 6 : (SP ? 3 : 9));
     mbar_expect_tx(wfull, NTAPW * Cfg::W_TAP);
     for (int tap = 0; tap < NTAPW; ++tap) tma_load_2d(sW + tap * Cfg::W_TAP, &tmW, 0, tap * CO, wfull);
   }
@@ -610,9 +628,16 @@ __device__ __forceinline__ void pair_fwd_body(const CUtensorMap& tmA, const CUte
         const int b = t / a.Hp, hp = t - b * a.Hp;
         const int q0 = (b * a.H + 2 * hp) * half_w;          // first pair-row of image row 2hp
         mbar_wait(&empty[buf], phase ^ 1);
-        mbar_expect_tx(&full[buf], Cfg::HALO);
         uint8_t* dst = sA + buf * Cfg::HALO;
-        for (int sg = 0; sg < Cfg::NSEG; ++sg) tma_load_2d(dst + sg * Cfg::SEG_BYTES, &tmA, 0, q0 + sg * half_w, &full[buf]);
+        if constexpr (PK == kPairC) {
+          const uint32_t row_bytes = (uint32_t)a.W * 8u;
+          mbar_expect_tx(&full[buf], Cfg::NSEG * row_bytes);
+          for (int sg = 0; sg < Cfg::NSEG; ++sg)
+            bulk_load_1d(dst + sg * Cfg::SEG_BYTES, xc + (size_t)(q0 + sg * half_w) * 8, row_bytes, &full[buf]);
+        } else {
+          mbar_expect_tx(&full[buf], Cfg::HALO);
+          for (int sg = 0; sg < Cfg::NSEG; ++sg) tma_load_2d(dst + sg * Cfg::SEG_BYTES, tmA, 0, q0 + sg * half_w, &full[buf]);
+        }
         if (++buf == Cfg::NBUF) { buf = 0; phase ^= 1; }
       }
     }
@@ -656,6 +681,32 @@ __device__ __forceinline__ void pair_fwd_body(const CUtensorMap& tmA, const CUte
                 mma_bf16(acc[dy * 2 + dx][0][mt], af, bf[0], bf[1]);
                 mma_bf16(acc[dy * 2 + dx][1][mt], af, bf[2], bf[3]);
               }
+        } else if constexpr (PK == kPairC) {
+          uint32_t bf[3][2][4];
+#pragma unroll
+          for (int r = 0; r < 3; ++r)
+#pragma unroll
+            for (int dx = 0; dx < 2; ++dx)
+              ld_b_kmajor<WB>(w_base + (r * 2 + dx) * Cfg::W_TAP, c0 * 8, (c0 + 2) * 8, 0, lane, bf[r][dx]);
+          // halo row R = dy + r serves (dy, r) = (0, R) and (1, R - 1); every accumulator still sums r = 0, 1, 2 in order
+#pragma unroll
+          for (int R = 0; R < 4; ++R)
+#pragma unroll
+            for (int mt = 0; mt < 2; ++mt) {
+              uint32_t af[4];
+              ldsm_x4(a_base + R * Cfg::SEG_BYTES + (uint32_t)((qd * 32 + mt * 16 + (lane & 15)) * 16 + ((lane >> 4) << 4)),
+                      af);
+#pragma unroll
+              for (int dy = 0; dy < 2; ++dy) {
+                const int r = R - dy;
+                if (r < 0 || r > 2) continue;
+#pragma unroll
+                for (int dx = 0; dx < 2; ++dx) {
+                  mma_bf16(acc[dy * 2 + dx][0][mt], af, bf[r][dx][0], bf[r][dx][1]);
+                  mma_bf16(acc[dy * 2 + dx][1][mt], af, bf[r][dx][2], bf[r][dx][3]);
+                }
+              }
+            }
         } else if constexpr (SP) {
 #pragma unroll
           for (int r = 0; r < 3; ++r) {
@@ -748,14 +799,20 @@ template <int CK, int CO, bool SP>
 __global__ void __launch_bounds__(288, PairFwdCfg<CK, CO>::OCC)
 pair_fwd_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmW,
                 const PairFwdArgs a) {
-  pair_fwd_body<CK, CO, SP ? kPairS : kPairPlain>(tmA, tmW, a);
+  pair_fwd_body<CK, CO, SP ? kPairS : kPairPlain>(&tmA, tmW, a);
 }
 
 // the one-channel layer 1 on the rs-packed input (CK = 16, CO = 32)
 __global__ void __launch_bounds__(288, PairCfgOf<16, 32, kPairRS>::OCC)
 pair_fwd_rs_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmW,
                    const PairFwdArgs a) {
-  pair_fwd_body<16, 32, kPairRS>(tmA, tmW, a);
+  pair_fwd_body<16, 32, kPairRS>(&tmA, tmW, a);
+}
+
+// the RGB layer 1 on the compact input (CK = 16, CO = 32): rows are bulk-copied from X, no input tensor map
+__global__ void __launch_bounds__(288, PairCfgOf<16, 32, kPairC>::OCC)
+pair_fwd_compact_kernel(const __grid_constant__ CUtensorMap tmW, const PairFwdArgs a, const __nv_bfloat16* __restrict__ X) {
+  pair_fwd_body<16, 32, kPairC>(nullptr, tmW, a, X);
 }
 
 template <int CK, int CO, int PK = kPairPlain>
@@ -775,6 +832,16 @@ static void launch_pair_fwd(const __nv_bfloat16* X, const __nv_bfloat16* Wt, Pai
   hefl::cuda::note_launch();
 }
 
+static void launch_pair_fwd_compact(const __nv_bfloat16* X, const __nv_bfloat16* Wt, PairFwdArgs a, cudaStream_t st) {
+  using Cfg = PairCfgOf<16, 32, kPairC>;
+  const CUtensorMap tmW = make_map(Wt, 16, 6 * 32, 32, 16, 32);
+  cudaFuncSetAttribute(pair_fwd_compact_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM);
+  int gx = hefl::cuda::device_sm_count() * Cfg::OCC;
+  if (gx > a.num_tiles) gx = a.num_tiles;
+  launch_pdl(pair_fwd_compact_kernel, dim3(gx), dim3(288), Cfg::SMEM, st, tmW, a, X);
+  hefl::cuda::note_launch();
+}
+
 bool conv_fwd_pool_pair_supported(int H, int W, int CK, int CO) {
   return H == W && (W % 2) == 0 && (W - 2) / 2 <= 128 && (CK == 16 || CK == 32) && (CO == 32 || CO == 64);
 }
@@ -782,8 +849,10 @@ bool conv_fwd_pool_pair_supported(int H, int W, int CK, int CO) {
 // Same contract as conv_fwd_pool (plain 9-tap weight layout [9][CO][CK], [3][CO][16] with the s-packed input,
 // [1][CO][16] with the rs-packed one-channel input); see G1b above.
 void conv_fwd_pool_pair(const void* X, const void* Wf, const float* bias, void* out, uint8_t* argmax, int B, int H,
-                        int W, int CK, int CO, int spack, int in_channels, cudaStream_t st) {
+                        int W, int CK, int CO, int spack, int in_channels, int compact, cudaStream_t st) {
   if (!conv_fwd_pool_pair_supported(H, W, CK, CO)) throw std::runtime_error("conv_fwd_pool_pair: unsupported shape");
+  if (compact && !(CK == 16 && CO == 32 && in_channels == 3 && W <= 256))
+    throw std::runtime_error("conv_fwd_pool_pair: the compact input is the RGB first layer (CK=16, CO=32, W <= 256)");
   PairFwdArgs a{};
   a.B = B; a.H = H; a.W = W;
   a.Hp = (H - 2) / 2; a.Wp = (W - 2) / 2;
@@ -796,7 +865,8 @@ void conv_fwd_pool_pair(const void* X, const void* Wf, const float* bias, void* 
   if (spack && !(CK == 16 && CO == 32)) throw std::runtime_error("conv_fwd_pool_pair: s-packed input is CK=16, CO=32 only");
   if (spack && in_channels != 1 && in_channels != 3)
     throw std::runtime_error("conv_fwd_pool_pair: packed input has 1 or 3 channels");
-  if (CK == 16 && CO == 32 && spack && in_channels == 1) launch_pair_fwd<16, 32, kPairRS>(x, w, a, st);
+  if (compact) launch_pair_fwd_compact(x, w, a, st);
+  else if (CK == 16 && CO == 32 && spack && in_channels == 1) launch_pair_fwd<16, 32, kPairRS>(x, w, a, st);
   else if (CK == 16 && CO == 32 && spack) launch_pair_fwd<16, 32, kPairS>(x, w, a, st);
   else if (CK == 16 && CO == 32) launch_pair_fwd<16, 32>(x, w, a, st);
   else if (CK == 32 && CO == 32) launch_pair_fwd<32, 32>(x, w, a, st);

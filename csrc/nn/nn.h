@@ -20,8 +20,10 @@ void adam_step(float* p, float* g, float* m, float* v, void* shadow_bf16, int64_
 void conv_fwd_pool(const void* X, const void* Wf, const float* bias, void* out, uint8_t* argmax, int B, int H,
                    int W, int CK, int CO, int spack, int in_channels, cudaStream_t st);
 bool conv_fwd_pool_pair_supported(int H, int W, int CK, int CO);
+// compact: X is the [B*H*W, 4] RGB layer-1 input (R, G, B, 0; preprocess_u8 compact), Wf the [3 r][2 dx][32][16]
+// weights (conv_weight_relayout compact0); CK = 16, CO = 32, W <= 256
 void conv_fwd_pool_pair(const void* X, const void* Wf, const float* bias, void* out, uint8_t* argmax, int B, int H,
-                        int W, int CK, int CO, int spack, int in_channels, cudaStream_t st);
+                        int W, int CK, int CO, int spack, int in_channels, int compact, cudaStream_t st);
 void conv_set_debug(int mask);
 void conv_dgrad(const void* dY, const void* Wd, void* dX, int B, int H, int W, int CK, int CO, const uint8_t* up_amax,
                 int up_W, cudaStream_t st);
@@ -54,6 +56,9 @@ void wgrad0_gather(const void* X, const void* g, const uint8_t* amax, float* dW,
 bool wgrad0_mma_supported(int W, int Wp, int CK, int Ci, int Co);
 void wgrad0_mma(const void* X, const void* g, const uint8_t* amax, float* dW, float* ws, int B, int H, int W, int Hp,
                 int Wp, int in_channels, cudaStream_t st);
+// the same on the compact [B*H*W, 4] RGB input (preprocess_u8 compact)
+void wgrad0_mma_compact(const void* X, const void* g, const uint8_t* amax, float* dW, float* ws, int B, int H, int W,
+                        int Hp, int Wp, cudaStream_t st);
 // ---- general tensor-core GEMMs for the ResNet convolutions (gemm_tcgen05.cu) ----
 // C[rows_out, N] (bf16) = sum_{t < taps} A[m + shifts[t], K] . B[t*N + n, K]^T. padded != 0: A rows index a zero-padded
 // [Bn][H+2][W+2] grid and only interior pixels are written (to the dense [Bn*H*W, N] output). fp8: A and B hold e4m3
@@ -91,13 +96,15 @@ struct ConvLayerTable {
   int64_t wf_off[kMaxConvLayers], wd_off[kMaxConvLayers];     // offsets (elements) into the bf16 Wf / Wd buffers
   int64_t dw_off[kMaxConvLayers];                             // offsets (elements) into the fp32 dW32 buffer
 };
-// x: uint8 [B,H,W,C] with C = 3 or 1
+// x: uint8 [B,H,W,C] with C = 3 or 1; compact (C = 3 only): X is [B*H*W, 4] (R, G, B, 0) instead of [B*H*W, 16]
 void preprocess_u8(const uint8_t* x, const float* theta, void* X, int B, int H, int W, int C, uint64_t aug_seed,
-                   const int64_t* step, int spack, cudaStream_t st);
+                   const int64_t* step, int spack, int compact, cudaStream_t st);
 void unpool_relu(const void* g, const uint8_t* amax, const void* ypool, void* dY, int B, int H, int W, int Hp,
                  int Wp, int Co, cudaStream_t st);
+// compact0 (with spack0, RGB): layer 1 gets the weights of the compact input, [3 r][2 dx][Co][16], after its s-packed
+// [3][Co][16] ones (both fit in the [9][Co][16] slot)
 void conv_weight_relayout(const void* shadow, const ConvLayerTable& t, void* Wf, void* Wd, int l0, int l1,
-                          int spack0, cudaStream_t st);
+                          int spack0, int compact0, cudaStream_t st);
 void conv_grad_finalize(float* dW32, const ConvLayerTable& t, float* grad, int l0, int l1, cudaStream_t st);
 void fused_update(float* dW32, const ConvLayerTable& t, float* flat, float* grad, float* m, float* v, void* shadow,
                   void* Wf, void* Wd, const int64_t* step, const float* lr_scale, float lr, float decay, float beta1,

@@ -116,9 +116,16 @@ void conv_fwd_pool(const Tensor& X, const Tensor& Wf, const Tensor& bias, Tensor
 // Pair-row forward kernel (conv_tcgen05.cu G1b): same contract as conv_fwd_pool with the plain [9, CO, CK] weights.
 void conv_fwd_pool_pair(const Tensor& X, const Tensor& Wf, const Tensor& bias, Tensor out,
                         const c10::optional<Tensor>& argmax, int64_t B, int64_t H, int64_t W, int64_t CK, int64_t CO,
-                        bool spack, int64_t in_channels) {
+                        bool spack, int64_t in_channels, bool compact) {
   chk_bf16(X, "X"); chk_bf16(Wf, "Wf"); chk_bf16(out, "out");
-  TORCH_CHECK(X.numel() >= B * H * W * CK && Wf.numel() >= packed_taps(spack, in_channels) * CO * CK, "shape mismatch");
+  if (compact) {
+    // [B*H*W, 4] RGB input, weights [3 r][2 dx][32][16]; rows are bulk-copied (16-byte aligned)
+    TORCH_CHECK(in_channels == 3 && CK == 16 && CO == 32 && W <= 256, "the compact input is the RGB first layer (CK=16, CO=32, W <= 256)");
+    TORCH_CHECK(X.numel() >= B * H * W * 4 && Wf.numel() >= 6 * CO * CK, "shape mismatch");
+    TORCH_CHECK(reinterpret_cast<uintptr_t>(X.data_ptr()) % 16 == 0, "the compact input must be 16-byte aligned");
+  } else {
+    TORCH_CHECK(X.numel() >= B * H * W * CK && Wf.numel() >= packed_taps(spack, in_channels) * CO * CK, "shape mismatch");
+  }
   TORCH_CHECK(!spack || (CK == 16 && CO == 32), "packed input is the 1- or 3-channel first layer only");
   TORCH_CHECK(hefl::nn::conv_fwd_pool_pair_supported((int)H, (int)W, (int)CK, (int)CO), "conv_fwd_pool_pair: unsupported shape");
   const int64_t Hp = (H - 2) / 2, Wp = (W - 2) / 2;
@@ -129,7 +136,7 @@ void conv_fwd_pool_pair(const Tensor& X, const Tensor& Wf, const Tensor& bias, T
     am = argmax->data_ptr<uint8_t>();
   }
   hefl::nn::conv_fwd_pool_pair(X.data_ptr(), Wf.data_ptr(), bias.data_ptr<float>(), out.data_ptr(), am, (int)B, (int)H,
-                               (int)W, (int)CK, (int)CO, spack ? 1 : 0, (int)in_channels, cur());
+                               (int)W, (int)CK, (int)CO, spack ? 1 : 0, (int)in_channels, compact ? 1 : 0, cur());
 }
 
 void conv_dgrad(const Tensor& dY, const Tensor& Wd, Tensor dX, int64_t B, int64_t H, int64_t W, int64_t CK,
@@ -159,12 +166,18 @@ void conv_wgrad(const Tensor& X, const Tensor& DY, Tensor dW32, int64_t B, int64
 }
 
 void preprocess_u8(const Tensor& x, const c10::optional<Tensor>& theta, Tensor X, int64_t aug_seed,
-                   const c10::optional<Tensor>& step, bool spack) {
+                   const c10::optional<Tensor>& step, bool spack, bool compact) {
   TORCH_CHECK(x.is_cuda() && x.scalar_type() == at::kByte && x.is_contiguous() && x.dim() == 4 && (x.size(3) == 3 || x.size(3) == 1),
               "x must be uint8 [B,H,W,3] or [B,H,W,1]");
   chk_bf16(X, "X");
   const int64_t B = x.size(0), H = x.size(1), W = x.size(2);
-  TORCH_CHECK(X.numel() == B * H * W * 16, "X must be [B*H*W, 16]");
+  if (compact) {
+    TORCH_CHECK(x.size(3) == 3, "the compact layout is for 3-channel images");
+    TORCH_CHECK(X.numel() == B * H * W * 4 && reinterpret_cast<uintptr_t>(X.data_ptr()) % 8 == 0,
+                "X must be an 8-byte aligned [B*H*W, 4]");
+  } else {
+    TORCH_CHECK(X.numel() == B * H * W * 16, "X must be [B*H*W, 16]");
+  }
   const float* th = nullptr;
   if (theta.has_value()) {
     TORCH_CHECK(theta->is_cuda() && theta->scalar_type() == at::kFloat && theta->numel() == B * 6 && theta->is_contiguous(), "theta must be float32 [B,2,3]");
@@ -176,7 +189,7 @@ void preprocess_u8(const Tensor& x, const c10::optional<Tensor>& theta, Tensor X
     sp = step->data_ptr<int64_t>();
   }
   hefl::nn::preprocess_u8(x.data_ptr<uint8_t>(), th, X.data_ptr(), (int)B, (int)H, (int)W, (int)x.size(3), (uint64_t)aug_seed, sp,
-                          spack ? 1 : 0, cur());
+                          spack ? 1 : 0, compact ? 1 : 0, cur());
 }
 
 void unpool_relu(const Tensor& g, const Tensor& amax, const Tensor& ypool, Tensor dY, int64_t B, int64_t H,
@@ -259,15 +272,25 @@ void bn_backward(const Tensor& dy, const Tensor& x, const Tensor& y, const Tenso
 // Layer-1 weight gradient from the pooled gradient (see wgrad_gather.cu). X: [B*H*W(+slack), 16] bf16,
 // g: [B,Hp,Wp,32] bf16, amax: [B,Hp,Wp,32] u8 (bits 0-1 position, bit 2 active), dW32: [9*16+1, 32] fp32 (+=).
 // spack: X is the packed input of in_channels channels (s-packed for 3, rs-packed for 1) -> masked GEMMs.
+// compact: X is the [B*H*W, 4] RGB input (preprocess_u8 compact) -> masked GEMMs on its overlapping rows.
 void wgrad0_gather(const Tensor& X, const Tensor& g, const Tensor& amax, Tensor dW32, int64_t B, int64_t H, int64_t W, bool spack,
-                   int64_t in_channels) {
+                   int64_t in_channels, bool compact) {
   chk_bf16(X, "X"); chk_bf16(g, "g");
   packed_taps(spack, in_channels);
   const int64_t Hp = (H - 2) / 2, Wp = (W - 2) / 2;
   TORCH_CHECK(hefl::nn::wgrad0_gather_supported((int)W, (int)Wp, 16, 3, 32), "wgrad0_gather: unsupported shape");
-  TORCH_CHECK(X.numel() >= B * H * W * 16 && g.numel() == B * Hp * Wp * 32 && amax.numel() == g.numel(), "shape mismatch");
+  TORCH_CHECK(X.numel() >= B * H * W * (compact ? 4 : 16) && g.numel() == B * Hp * Wp * 32 && amax.numel() == g.numel(),
+              "shape mismatch");
   TORCH_CHECK(amax.scalar_type() == at::kByte && dW32.scalar_type() == at::kFloat && dW32.numel() >= (9 * 16 + 1) * 32, "dtype / size");
   Tensor ws = at::empty({(int64_t)hefl::nn::wgrad0_parts((int)B, (int)Hp) * hefl::nn::kWgrad0Part}, dW32.options());
+  if (compact) {
+    TORCH_CHECK(in_channels == 3 && hefl::nn::wgrad0_mma_supported((int)W, (int)Wp, 16, 3, 32),
+                "wgrad0_gather: the compact input needs the RGB masked-GEMM kernel (HEFL_WGRAD0_MMA on, even W <= 256)");
+    TORCH_CHECK(reinterpret_cast<uintptr_t>(X.data_ptr()) % 16 == 0, "the compact input must be 16-byte aligned");
+    hefl::nn::wgrad0_mma_compact(X.data_ptr(), g.data_ptr(), amax.data_ptr<uint8_t>(), dW32.data_ptr<float>(),
+                                 ws.data_ptr<float>(), (int)B, (int)H, (int)W, (int)Hp, (int)Wp, cur());
+    return;
+  }
   if (spack && hefl::nn::wgrad0_mma_supported((int)W, (int)Wp, 16, 3, 32)) {      // packed input: masked GEMMs on the tensor cores
     hefl::nn::wgrad0_mma(X.data_ptr(), g.data_ptr(), amax.data_ptr<uint8_t>(), dW32.data_ptr<float>(), ws.data_ptr<float>(),
                          (int)B, (int)H, (int)W, (int)Hp, (int)Wp, (int)in_channels, cur());
@@ -432,12 +455,13 @@ hefl::nn::ConvLayerTable table_from(const Tensor& t) {
 // l0/l1: layer range [l0, l1) (l1 = -1: all layers) so the update of the layers whose gradients are final can
 // run on a side stream under the last weight-gradient kernel.
 void conv_weight_relayout(const Tensor& shadow, const Tensor& table, Tensor Wf, Tensor Wd, int64_t l0, int64_t l1,
-                          bool spack0) {
+                          bool spack0, bool compact0) {
   chk_bf16(shadow, "shadow"); chk_bf16(Wf, "Wf"); chk_bf16(Wd, "Wd");
   const auto t = table_from(table);
   if (l1 < 0) l1 = t.n;
   TORCH_CHECK(0 <= l0 && l1 <= t.n, "layer range");
-  hefl::nn::conv_weight_relayout(shadow.data_ptr(), t, Wf.data_ptr(), Wd.data_ptr(), (int)l0, (int)l1, spack0 ? 1 : 0, cur());
+  hefl::nn::conv_weight_relayout(shadow.data_ptr(), t, Wf.data_ptr(), Wd.data_ptr(), (int)l0, (int)l1, spack0 ? 1 : 0,
+                                 compact0 ? 1 : 0, cur());
 }
 
 void conv_grad_finalize(Tensor dW32, const Tensor& table, Tensor grad, int64_t l0, int64_t l1) {
@@ -454,17 +478,17 @@ TORCH_LIBRARY_FRAGMENT(hefl, m) {
   m.def("adam_step_(Tensor(a!) p, Tensor(b!) g, Tensor(c!) m, Tensor(d!) v, Tensor? shadow, Tensor step, Tensor? lr_scale, float lr, float decay, float beta1, float beta2, float eps, Tensor? anchor=None, float mu=0.0) -> ()", &adam_step_);
   m.def("gather_h2d_(Tensor(a!) dst, Tensor src, Tensor indices) -> ()", &gather_h2d_);
   m.def("conv_fwd_pool(Tensor X, Tensor Wf, Tensor bias, Tensor(a!) out, Tensor(b!)? argmax, int B, int H, int W, int CK, int CO, bool spack=False, int in_channels=3) -> ()", &conv_fwd_pool);
-  m.def("conv_fwd_pool_pair(Tensor X, Tensor Wf, Tensor bias, Tensor(a!) out, Tensor(b!)? argmax, int B, int H, int W, int CK, int CO, bool spack=False, int in_channels=3) -> ()", &conv_fwd_pool_pair);
+  m.def("conv_fwd_pool_pair(Tensor X, Tensor Wf, Tensor bias, Tensor(a!) out, Tensor(b!)? argmax, int B, int H, int W, int CK, int CO, bool spack=False, int in_channels=3, bool compact=False) -> ()", &conv_fwd_pool_pair);
   m.def("conv_dgrad(Tensor dY, Tensor Wd, Tensor(a!) dX, int B, int H, int W, int CK, int CO, Tensor? up_amax=None, int up_W=0) -> ()", &conv_dgrad);
   m.def("conv_wgrad(Tensor X, Tensor DY, Tensor(a!) dW32, int B, int H, int W, int CK, int Co) -> ()", &conv_wgrad);
-  m.def("preprocess_u8(Tensor x, Tensor? theta, Tensor(a!) X, int aug_seed, Tensor? step, bool spack=False) -> ()", &preprocess_u8);
+  m.def("preprocess_u8(Tensor x, Tensor? theta, Tensor(a!) X, int aug_seed, Tensor? step, bool spack=False, bool compact=False) -> ()", &preprocess_u8);
   m.def("unpool_relu(Tensor g, Tensor amax, Tensor ypool, Tensor(a!) dY, int B, int H, int W, int Co) -> ()", &unpool_relu);
   m.def("head_forward_backward(Tensor feat, Tensor flat, Tensor(a!) grad, int[] offs, Tensor y, Tensor(b!) dfeat, Tensor(c!) h1_buf, Tensor(d!) dh1_buf, Tensor(e!) out, Tensor(f!)? step, int B, int F, int H1, int H2, int C, bool train) -> ()", &head_forward_backward);
   m.def("fused_update(Tensor(a!) dW32, Tensor table, Tensor(b!) flat, Tensor(c!) grad, Tensor(d!) m, Tensor(e!) v, Tensor(f!) shadow, Tensor(g!) Wf, Tensor(h!) Wd, Tensor step, Tensor? lr_scale, float lr, float decay, float beta1, float beta2, float eps, int dense_off, int n_trainable, Tensor? anchor=None, float mu=0.0) -> ()", &fused_update);
   m.def("conv_set_debug(int mask) -> ()", &conv_set_debug);
   m.def("set_head_cluster(int on) -> ()", [](int64_t on) { g_head_cluster = (int)on; });
   m.def("set_pdl(int on) -> ()", [](int64_t on) { hefl::nn::set_pdl((int)on); });
-  m.def("wgrad0_gather(Tensor X, Tensor g, Tensor amax, Tensor(a!) dW32, int B, int H, int W, bool spack=False, int in_channels=3) -> ()", &wgrad0_gather);
+  m.def("wgrad0_gather(Tensor X, Tensor g, Tensor amax, Tensor(a!) dW32, int B, int H, int W, bool spack=False, int in_channels=3, bool compact=False) -> ()", &wgrad0_gather);
   m.def("fp8_quantize(Tensor x, Tensor(a!) q, Tensor scale, Tensor(b!) amax) -> ()", &fp8_quantize);
   m.def("gemm_taps(Tensor A, Tensor B, Tensor(a!) out, int N, int K, int[] shifts, int padded, int Bn, int H, int W, Tensor? scale_a, Tensor? scale_b) -> ()", &gemm_taps);
   m.def("wgrad_taps(Tensor DY, Tensor X, Tensor(a!) dW, int taps, int Wp) -> ()", &wgrad_taps);
@@ -479,6 +503,6 @@ TORCH_LIBRARY_FRAGMENT(hefl, m) {
   m.def("avgpool_forward(Tensor x, Tensor(a!) out, int B, int HW, int C) -> ()", &avgpool_forward);
   m.def("avgpool_backward(Tensor dout, Tensor(a!) dx, int B, int HW, int C) -> ()", &avgpool_backward);
   m.def("umma_shift_probe(Tensor A, Tensor Bm, int CK, int shift_rows) -> Tensor", &umma_shift_probe);
-  m.def("conv_weight_relayout(Tensor shadow, Tensor table, Tensor(a!) Wf, Tensor(b!) Wd, int l0=0, int l1=-1, bool spack0=False) -> ()", &conv_weight_relayout);
+  m.def("conv_weight_relayout(Tensor shadow, Tensor table, Tensor(a!) Wf, Tensor(b!) Wd, int l0=0, int l1=-1, bool spack0=False, bool compact0=False) -> ()", &conv_weight_relayout);
   m.def("conv_grad_finalize(Tensor(a!) dW32, Tensor table, Tensor(b!) grad, int l0=0, int l1=-1) -> ()", &conv_grad_finalize);
 }

@@ -88,10 +88,11 @@ __device__ __forceinline__ bool preprocess_theta(const float* __restrict__ theta
 
 // uint8 NHWC (3 channels) -> bf16 [P,16] (channels 3..15 zero), with 1/255 rescale and an optional per-sample affine warp (Keras shear/zoom/flip,
 // FLPyfhelin.py:80-86) sampled bilinearly with border clamp (torch.grid_sample semantics,
-// align_corners=False).
+// align_corners=False). With `compact` the output is [P,4] instead: R, G, B, 0 — one 8-byte store per pixel, the
+// same values as channels 0-2 of the other layouts.
 __global__ void preprocess_u8_kernel(const uint8_t* __restrict__ x, const float* __restrict__ theta,
                                      __nv_bfloat16* __restrict__ X, int B, int H, int W, uint64_t aug_seed,
-                                     const int64_t* __restrict__ step, int spack) {
+                                     const int64_t* __restrict__ step, int spack, int compact) {
   pdl_prologue();
   const int b = blockIdx.y;
   float tl[6];
@@ -100,7 +101,7 @@ __global__ void preprocess_u8_kernel(const uint8_t* __restrict__ x, const float*
   // 0-2 = this pixel, 3-5 = pixel w+1, 6-8 = pixel w+2, so the three horizontal filter taps become part of the
   // GEMM K dimension) a warp stores 30 pixels and lanes 30/31 only feed their values to the shuffles.
   const int lane = threadIdx.x & 31;
-  const int PW = spack ? 30 : 32;
+  const int PW = spack && !compact ? 30 : 32;
   const int chunks = (W + PW - 1) / PW;
   const int tasks = H * chunks;
   const int wpb = blockDim.x >> 5;
@@ -133,6 +134,10 @@ __global__ void preprocess_u8_kernel(const uint8_t* __restrict__ x, const float*
     uint32_t p01 = (uint32_t)__bfloat16_as_ushort(__float2bfloat16(c[0])) |
                    ((uint32_t)__bfloat16_as_ushort(__float2bfloat16(c[1])) << 16);
     uint32_t p2 = __bfloat16_as_ushort(__float2bfloat16(c[2]));
+    if (compact) {
+      if (w < W) *reinterpret_cast<uint2*>(X + ((int64_t)(b * H + h) * W + w) * 4) = make_uint2(p01, p2);
+      continue;
+    }
     if (w >= W) { p01 = 0u; p2 = 0u; }                       // past the row end: zero neighbours
     const uint32_t n1_01 = __shfl_down_sync(0xffffffffu, p01, 1), n1_2 = __shfl_down_sync(0xffffffffu, p2, 1);
     const uint32_t n2_01 = __shfl_down_sync(0xffffffffu, p01, 2), n2_2 = __shfl_down_sync(0xffffffffu, p2, 2);
@@ -217,13 +222,18 @@ __global__ void preprocess_u8_gray_kernel(const uint8_t* __restrict__ x, const f
 }
 
 void preprocess_u8(const uint8_t* x, const float* theta, void* X, int B, int H, int W, int C, uint64_t aug_seed,
-                   const int64_t* step, int spack, cudaStream_t st) {
-  const int tasks = H * ((W + (spack ? 29 : 31)) / (spack ? 30 : 32));
+                   const int64_t* step, int spack, int compact, cudaStream_t st) {
+  const int pw = spack && !compact ? 30 : 32;
+  const int tasks = H * ((W + pw - 1) / pw);
   int bx = (tasks + 7) / 8;
   if (bx > 64) bx = 64;
   dim3 grid(bx, B);
-  launch_pdl(C == 1 ? preprocess_u8_gray_kernel : preprocess_u8_kernel, dim3(grid), dim3(256), 0, st, x, theta,
-             reinterpret_cast<__nv_bfloat16*>(X), B, H, W, aug_seed, step, spack);
+  if (C == 1)
+    launch_pdl(preprocess_u8_gray_kernel, dim3(grid), dim3(256), 0, st, x, theta, reinterpret_cast<__nv_bfloat16*>(X),
+               B, H, W, aug_seed, step, spack);
+  else
+    launch_pdl(preprocess_u8_kernel, dim3(grid), dim3(256), 0, st, x, theta, reinterpret_cast<__nv_bfloat16*>(X), B,
+               H, W, aug_seed, step, spack, compact);
   hefl::cuda::note_launch();
 }
 
@@ -296,11 +306,23 @@ void unpool_relu(const void* g, const uint8_t* amax, const void* ypool, void* dY
 // operand, channel-padded) and Wd [tap][Ci][Co] (dgrad B operand).
 __global__ void conv_weight_relayout_kernel(const __nv_bfloat16* __restrict__ shadow, const ConvLayerTable t,
                                             __nv_bfloat16* __restrict__ Wf, __nv_bfloat16* __restrict__ Wd, int l0,
-                                            int spack0) {
+                                            int spack0, int compact0) {
   pdl_wait();   // parameter writer: no early trigger (see launch.cuh)
   const int l = blockIdx.y + l0;
   const int Ci = t.Ci[l], CK = t.CK[l], Co = t.Co[l];
   const __nv_bfloat16* w = shadow + t.w_off[l];
+  if (l == 0 && compact0) {
+    // compact RGB layer 1 ([P,4] input, pixels 2j..2j+3 x (R, G, B, 0) form one K = 16 row): Wf [3 r][2 dx][Co][16]
+    // after the s-packed [3][Co][CK] (written below too: the 16-channel kernels may be selected at any time), k =
+    // 4 * slot + ci with slot = s + dx, so column parity dx is a choice of weights, not of input address
+    const int nf = 6 * Co * CK;
+    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < nf; i += gridDim.x * blockDim.x) {
+      const int k = i % CK, co = (i / CK) % Co, rd = i / (CK * Co);
+      const int r = rd >> 1, sx = (k >> 2) - (rd & 1), ci = k & 3;
+      Wf[t.wf_off[l] + 3 * Co * CK + i] =
+          sx >= 0 && sx < 3 && ci < Ci ? w[(co * Ci + ci) * 9 + r * 3 + sx] : __float2bfloat16(0.f);
+    }
+  }
   if (l == 0 && spack0 && Ci == 1) {
     // rs-packed one-channel layer 1: Wf [1][Co][CK], k = 3r + s (the input carries the whole 3x3 neighbourhood)
     const int nf = Co * CK;
@@ -335,12 +357,12 @@ __global__ void conv_weight_relayout_kernel(const __nv_bfloat16* __restrict__ sh
 }
 
 void conv_weight_relayout(const void* shadow, const ConvLayerTable& t, void* Wf, void* Wd, int l0, int l1,
-                          int spack0, cudaStream_t st) {
+                          int spack0, int compact0, cudaStream_t st) {
   if (l1 <= l0) return;
   dim3 grid(32, l1 - l0);
   launch_pdl(conv_weight_relayout_kernel, dim3(grid), dim3(256), 0, st, reinterpret_cast<const __nv_bfloat16*>(shadow), t,
                                                     reinterpret_cast<__nv_bfloat16*>(Wf),
-                                                    reinterpret_cast<__nv_bfloat16*>(Wd), l0, spack0);
+                                                    reinterpret_cast<__nv_bfloat16*>(Wd), l0, spack0, compact0);
   hefl::cuda::note_launch();
 }
 

@@ -32,6 +32,13 @@
 // (2i + dy, 2j + dx) already are all nine taps, so each code's GEMM has M = 16 (9 rows used) and a pooled row needs
 // input rows 2i and 2i+1 only (wgrad0_mma_rs_kernel); the partial rows tap * 3 + 0 carry the result.
 //
+// With the compact RGB input ([P, 4] = R, G, B, 0; wgrad0_mma_compact_kernel) an input row is one plain 1-D bulk copy
+// of W x 8 bytes into a 2 KB ring slot, and the 32 bytes at 16j (pixels 2j .. 2j+3 x 4 channels) are the A rows of
+// window j: M = 16 = 4 pixel slots x 4 channels, read with ldmatrix.trans at a 16-byte row stride (8 rows = 128
+// contiguous bytes, conflict-free without a swizzle). Slot s + dx holds tap s, so the two column parities keep separate
+// accumulators (96 registers) and are folded when the warp tiles are parked: tile row 4s + ci of dx = 1 is added to row
+// 4(s - 1) + ci of dx = 0.
+//
 // (Why mma.sync and not tcgen05 here: the B operand is produced by the CUDA cores, M x N is 48 x 32 and the
 // kernel is bound by the 116 MB it reads; the legacy tensor path needs no TMEM / descriptor round trip for that.)
 // Reference semantics: Keras Conv2D/MaxPooling2D backward of the first block (FLPyfhelin.py:120-121).
@@ -55,36 +62,43 @@ using namespace hefl::tc;
 constexpr int kT = 256;                 // 8 warps
 constexpr int kPx = 128;                // pooled pixels per strip tile (Wp <= 128)
 constexpr int kSlot = 8192;             // one input row: W <= 256 pixels x 32 B
+constexpr int kSlotC = 2048 + 128;      // compact: W <= 256 pixels x 8 B + zeroed slack (window 127 reads 16 B past)
 constexpr int kRing = 6;
 constexpr int kGst = kPx * 64;          // staged g of a strip      [px][32] bf16
 constexpr int kCst = kPx * 32;          // staged codes of a strip  [px][32] u8
 constexpr int kGs = kPx * 64;           // one masked tile
-constexpr int kBarOff = kRing * kSlot + 2 * kGst + 2 * kCst + 4 * kGs;
+constexpr int bar_off(int slot) { return kRing * slot + 2 * kGst + 2 * kCst + 4 * kGs; }
+constexpr int kBarOff = bar_off(kSlot);
 constexpr int kSmem = kBarOff + 64;     // 104 KB -> 2 CTAs / SM
+constexpr int kSmemC = bar_off(kSlotC) + 64 + 8 * kT * 4;   // 77 KB (+ bias sums); registers keep it at 2 CTAs / SM
 constexpr int kPartStride = 40;         // floats per row of a parked accumulator tile (bank spread)
 constexpr int kPart = 48 * kPartStride + 32;   // one warp's tile + its bias sums
-static_assert(8 * kPart * 4 <= kBarOff, "parked tiles must fit in the operand buffers");
+static_assert(8 * kPart * 4 <= bar_off(kSlotC), "parked tiles must fit in the operand buffers");
 
 // FR = filter rows that are separate GEMMs: 3 on the s-packed input (M = 3 x 16, a strip reads input rows 2i .. 2i+3),
 // 1 on the rs-packed one-channel input (channel 3r + s = pixel (h + r, w + s): M = 16 with 9 rows used, a strip reads
-// rows 2i and 2i+1 only, so consecutive strips share none).
-template <int FR>
-__device__ __forceinline__ void wgrad0_mma_body(const CUtensorMap& tmX, const __nv_bfloat16* __restrict__ g,
+// rows 2i and 2i+1 only, so consecutive strips share none). CPT: the compact RGB input (FR = 3; A = overlapping
+// 32-byte rows of plain [pixel][4] rows, dx in separate accumulators).
+template <int FR, bool CPT = false>
+__device__ __forceinline__ void wgrad0_mma_body(const CUtensorMap* tmX, const __nv_bfloat16* __restrict__ xc,
+                                                const __nv_bfloat16* __restrict__ g,
                                                 const uint8_t* __restrict__ amax, float* __restrict__ ws, int B, int H,
                                                 int W, int Hp, int Wp) {
   constexpr int NR = FR + 1;            // input rows under one pooled row
+  constexpr int SLOT = CPT ? kSlotC : kSlot;
+  constexpr int NDX = CPT ? 2 : 1;      // accumulator sets: column parities kept apart on the compact input
   extern __shared__ __align__(1024) uint8_t sm[];
   uint8_t* ring = sm;
-  uint8_t* gst = ring + kRing * kSlot;
+  uint8_t* gst = ring + kRing * SLOT;
   uint8_t* cst = gst + 2 * kGst;
   uint8_t* Gs = cst + 2 * kCst;
-  uint64_t* full = reinterpret_cast<uint64_t*>(sm + kBarOff);      // [2]: everything strip s needs, by strip parity
+  uint64_t* full = reinterpret_cast<uint64_t*>(sm + bar_off(SLOT));   // [2]: everything strip s needs, by strip parity
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
 
   // stale / never-written shared memory is multiplied by zero masks: it has to be finite
-  for (int i = tid; i < (kRing * kSlot) / 16; i += kT) reinterpret_cast<uint4*>(ring)[i] = make_uint4(0u, 0u, 0u, 0u);
+  for (int i = tid; i < (kRing * SLOT) / 16; i += kT) reinterpret_cast<uint4*>(ring)[i] = make_uint4(0u, 0u, 0u, 0u);
   if (tid == 0) {
-    prefetch_tmap(&tmX);
+    if constexpr (!CPT) prefetch_tmap(tmX);
     mbar_init(&full[0], 1);
     mbar_init(&full[1], 1);
     fence_barrier_init();
@@ -95,17 +109,31 @@ __device__ __forceinline__ void wgrad0_mma_body(const CUtensorMap& tmX, const __
 
   const long long S = (long long)B * Hp;
   const int s0 = (int)(S * blockIdx.x / gridDim.x), s1 = (int)(S * (blockIdx.x + 1) / gridDim.x);
-  const uint32_t row_bytes = (uint32_t)W * 32u, g_bytes = (uint32_t)Wp * 64u, c_bytes = (uint32_t)Wp * 32u;
+  const uint32_t row_bytes = (uint32_t)W * (CPT ? 8u : 32u), g_bytes = (uint32_t)Wp * 64u, c_bytes = (uint32_t)Wp * 32u;
   const int pairs = W >> 1;
+  // input row `row` (of the B*H rows) into ring slot `sl`
+  auto load_row = [&](int sl, int row, uint64_t* bar) {
+    if constexpr (CPT) bulk_load_1d(ring + sl * SLOT, xc + (size_t)row * W * 4, row_bytes, bar);
+    else tma_load_2d(ring + sl * SLOT, tmX, 0, row * pairs, bar);
+  };
 
-  float acc[FR][4][4];
+  float acc[FR][NDX][4][4];
 #pragma unroll
   for (int r = 0; r < FR; ++r)
 #pragma unroll
-    for (int n = 0; n < 4; ++n) acc[r][n][0] = acc[r][n][1] = acc[r][n][2] = acc[r][n][3] = 0.f;
+    for (int d = 0; d < NDX; ++d)
+#pragma unroll
+      for (int n = 0; n < 4; ++n) acc[r][d][n][0] = acc[r][d][n][1] = acc[r][d][n][2] = acc[r][d][n][3] = 0.f;
   float bsum[8];
 #pragma unroll
   for (int e = 0; e < 8; ++e) bsum[e] = 0.f;
+  // compact: the bias sums wait in shared memory ([e][thread]) between mask passes, so that the 96 accumulators fit
+  // in 128 registers without spills (the same additions in the same order)
+  float* bs = reinterpret_cast<float*>(sm + bar_off(SLOT) + 64) + tid;
+  if constexpr (CPT) {
+#pragma unroll
+    for (int e = 0; e < 8; ++e) bs[e * kT] = 0.f;
+  }
 
   // lane-constant pieces of the ldmatrix addresses
   const int mq = lane >> 3, li = lane & 7;
@@ -113,8 +141,9 @@ __device__ __forceinline__ void wgrad0_mma_body(const CUtensorMap& tmX, const __
   // A (slot = [pixel pair j][dx][16 ch], 16-byte chunk index XOR (j >> 1) & 3): matrices (k-half 0, m-half 0),
   // (0, 1), (1, 0), (1, 1) = a0..a3 of m16n8k16
   const int ja = j0 + (mq >> 1) * 8 + li;
-  const uint32_t a_off0 = ja * 64 + (((0 + (mq & 1)) ^ ((ja >> 1) & 3)) << 4);      // dx = 0
-  const uint32_t a_off1 = ja * 64 + (((2 + (mq & 1)) ^ ((ja >> 1) & 3)) << 4);      // dx = 1
+  // compact: window ja's 32-byte row at 16 ja, the same for both dx
+  const uint32_t a_off0 = CPT ? ja * 16 + ((mq & 1) << 4) : ja * 64 + (((0 + (mq & 1)) ^ ((ja >> 1) & 3)) << 4);
+  const uint32_t a_off1 = CPT ? a_off0 : ja * 64 + (((2 + (mq & 1)) ^ ((ja >> 1) & 3)) << 4);
   // B: matrices (k-half 0, n-tile nb), (1, nb), (0, nb + 1), (1, nb + 1)
   const int pb = j0 + (mq & 1) * 8 + li;
   const uint32_t b_off0 = pb * 64 + ((((mq >> 1) + 0) ^ ((pb >> 1) & 3)) << 4);
@@ -132,7 +161,7 @@ __device__ __forceinline__ void wgrad0_mma_body(const CUtensorMap& tmX, const __
       if (!pref) {                                           // first strip of the CTA or of an image: all of it, now
         mbar_expect_tx(&full[par], NR * row_bytes + g_bytes + c_bytes);
 #pragma unroll
-        for (int r = 0; r < NR; ++r) tma_load_2d(ring + r * kSlot, &tmX, 0, (b * H + 2 * i + r) * pairs, &full[par]);
+        for (int r = 0; r < NR; ++r) load_row(r, b * H + 2 * i + r, &full[par]);
         bulk_load_1d(gst + par * kGst, g + (size_t)s * Wp * 32, g_bytes, &full[par]);
         bulk_load_1d(cst + par * kCst, amax + (size_t)s * Wp * 32, c_bytes, &full[par]);
       }
@@ -142,14 +171,18 @@ __device__ __forceinline__ void wgrad0_mma_body(const CUtensorMap& tmX, const __
         sl4 = sl4 >= kRing ? sl4 - kRing : sl4;
         sl5 = sl5 >= kRing ? sl5 - kRing : sl5;
         mbar_expect_tx(&full[q], 2 * row_bytes + g_bytes + c_bytes);
-        tma_load_2d(ring + sl4 * kSlot, &tmX, 0, (b * H + 2 * i + NR) * pairs, &full[q]);
-        tma_load_2d(ring + sl5 * kSlot, &tmX, 0, (b * H + 2 * i + NR + 1) * pairs, &full[q]);
+        load_row(sl4, b * H + 2 * i + NR, &full[q]);
+        load_row(sl5, b * H + 2 * i + NR + 1, &full[q]);
         bulk_load_1d(gst + q * kGst, g + (size_t)(s + 1) * Wp * 32, g_bytes, &full[q]);
         bulk_load_1d(cst + q * kCst, amax + (size_t)(s + 1) * Wp * 32, c_bytes, &full[q]);
       }
     }
     mbar_wait(&full[par], ((s - s0) >> 1) & 1);
 
+    if constexpr (CPT) {
+#pragma unroll
+      for (int e = 0; e < 8; ++e) bsum[e] = bs[e * kT];
+    }
     // masks: item = (pooled pixel, 8 channels)
 #pragma unroll
     for (int it = 0; it < 2; ++it) {
@@ -184,6 +217,10 @@ __device__ __forceinline__ void wgrad0_mma_body(const CUtensorMap& tmX, const __
         bsum[6] += __uint_as_float(w3 << 16); bsum[7] += __uint_as_float(w3 & 0xFFFF0000u);
       }
     }
+    if constexpr (CPT) {
+#pragma unroll
+      for (int e = 0; e < 8; ++e) bs[e * kT] = bsum[e];
+    }
     __syncthreads();
 
     if (j0 < Wp) {                                           // warp-uniform
@@ -197,12 +234,13 @@ __device__ __forceinline__ void wgrad0_mma_body(const CUtensorMap& tmX, const __
         for (int r = 0; r < FR; ++r) {
           int slot = head + dy + r;
           slot = slot >= kRing ? slot - kRing : slot;
+          const int d = CPT ? (c & 1) : 0;
           uint32_t a[4];
-          ldsm_x4_t(ring_u + slot * kSlot + ((c & 1) ? a_off1 : a_off0), a);
-          mma_bf16(acc[r][0], a, bq[0][0], bq[0][1]);
-          mma_bf16(acc[r][1], a, bq[0][2], bq[0][3]);
-          mma_bf16(acc[r][2], a, bq[1][0], bq[1][1]);
-          mma_bf16(acc[r][3], a, bq[1][2], bq[1][3]);
+          ldsm_x4_t(ring_u + slot * SLOT + ((c & 1) ? a_off1 : a_off0), a);
+          mma_bf16(acc[r][d][0], a, bq[0][0], bq[0][1]);
+          mma_bf16(acc[r][d][1], a, bq[0][2], bq[0][3]);
+          mma_bf16(acc[r][d][2], a, bq[1][0], bq[1][1]);
+          mma_bf16(acc[r][d][3], a, bq[1][2], bq[1][3]);
         }
       }
     }
@@ -221,9 +259,31 @@ __device__ __forceinline__ void wgrad0_mma_body(const CUtensorMap& tmX, const __
 #pragma unroll
       for (int n = 0; n < 4; ++n) {
         const int col = n * 8 + 2 * tq;
-        *reinterpret_cast<float2*>(mine + (r * 16 + gq) * kPartStride + col) = make_float2(acc[r][n][0], acc[r][n][1]);
-        *reinterpret_cast<float2*>(mine + (r * 16 + gq + 8) * kPartStride + col) = make_float2(acc[r][n][2], acc[r][n][3]);
+        *reinterpret_cast<float2*>(mine + (r * 16 + gq) * kPartStride + col) = make_float2(acc[r][0][n][0], acc[r][0][n][1]);
+        *reinterpret_cast<float2*>(mine + (r * 16 + gq + 8) * kPartStride + col) =
+            make_float2(acc[r][0][n][2], acc[r][0][n][3]);
       }
+    if constexpr (CPT) {
+      // dx = 1: tile row 4 (s + 1) + ci is tap s; each lane adds to rows only it owns in the dx = 1 tile (rows 0..3,
+      // slot 0, are no tap of dx = 1)
+      __syncwarp();
+#pragma unroll
+      for (int r = 0; r < FR; ++r)
+#pragma unroll
+        for (int n = 0; n < 4; ++n) {
+          const int col = n * 8 + 2 * tq;
+          if (gq >= 4) {
+            float2* p = reinterpret_cast<float2*>(mine + (r * 16 + gq - 4) * kPartStride + col);
+            *p = make_float2(p->x + acc[r][1][n][0], p->y + acc[r][1][n][1]);
+          }
+          float2* p = reinterpret_cast<float2*>(mine + (r * 16 + gq + 4) * kPartStride + col);
+          *p = make_float2(p->x + acc[r][1][n][2], p->y + acc[r][1][n][3]);
+        }
+    }
+    if constexpr (CPT) {
+#pragma unroll
+      for (int e = 0; e < 8; ++e) bsum[e] = bs[e * kT];
+    }
 #pragma unroll
     for (int e = 0; e < 8; ++e) {                            // lanes with the same (lane & 3) hold the same 8 channels
       float v = bsum[e];
@@ -239,7 +299,11 @@ __device__ __forceinline__ void wgrad0_mma_body(const CUtensorMap& tmX, const __
     // partial row = tap * 3 + ci (as in wgrad0_reduce_kernel), 27 = bias
     float v = 0.f;
     if (FR == 3) {
-      const int src = row < 27 ? ((row / 9) * 16 + row % 9) * kPartStride + co : 48 * kPartStride + co;
+      // tile row of (r, s, ci): r * 16 + s * 3 + ci on the s-packed input, r * 16 + 4 s + ci on the compact one
+      int src;
+      if constexpr (CPT) src = row < 27 ? ((row / 9) * 16 + ((row / 3) % 3) * 4 + row % 3) * kPartStride + co
+                                        : 48 * kPartStride + co;
+      else src = row < 27 ? ((row / 9) * 16 + row % 9) * kPartStride + co : 48 * kPartStride + co;
 #pragma unroll
       for (int w = 0; w < 8; ++w) v += part[w * kPart + src];
     } else if (row >= 27 || row % 3 == 0) {               // rs: tile row 3r + s holds tap 3r + s of channel 0
@@ -254,13 +318,19 @@ __device__ __forceinline__ void wgrad0_mma_body(const CUtensorMap& tmX, const __
 __global__ void __launch_bounds__(kT, 2)
 wgrad0_mma_kernel(const __grid_constant__ CUtensorMap tmX, const __nv_bfloat16* __restrict__ g,
                   const uint8_t* __restrict__ amax, float* __restrict__ ws, int B, int H, int W, int Hp, int Wp) {
-  wgrad0_mma_body<3>(tmX, g, amax, ws, B, H, W, Hp, Wp);
+  wgrad0_mma_body<3>(&tmX, nullptr, g, amax, ws, B, H, W, Hp, Wp);
 }
 
 __global__ void __launch_bounds__(kT, 2)
 wgrad0_mma_rs_kernel(const __grid_constant__ CUtensorMap tmX, const __nv_bfloat16* __restrict__ g,
                      const uint8_t* __restrict__ amax, float* __restrict__ ws, int B, int H, int W, int Hp, int Wp) {
-  wgrad0_mma_body<1>(tmX, g, amax, ws, B, H, W, Hp, Wp);
+  wgrad0_mma_body<1>(&tmX, nullptr, g, amax, ws, B, H, W, Hp, Wp);
+}
+
+__global__ void __launch_bounds__(kT, 2)
+wgrad0_mma_compact_kernel(const __nv_bfloat16* __restrict__ X, const __nv_bfloat16* __restrict__ g,
+                          const uint8_t* __restrict__ amax, float* __restrict__ ws, int B, int H, int W, int Hp, int Wp) {
+  wgrad0_mma_body<3, true>(nullptr, X, g, amax, ws, B, H, W, Hp, Wp);
 }
 
 }  // namespace
@@ -306,6 +376,21 @@ void wgrad0_mma(const void* X, const void* g, const uint8_t* amax, float* dW, fl
                                      {32, (uint32_t)(W / 2)}, CU_TENSOR_MAP_SWIZZLE_64B);
   const int grid = wgrad0_parts(B, Hp);
   launch_pdl(in_channels == 1 ? wgrad0_mma_rs_kernel : wgrad0_mma_kernel, dim3(grid), dim3(kT), kSmem, st, tmX,
+             reinterpret_cast<const __nv_bfloat16*>(g), amax, ws, B, H, W, Hp, Wp);
+  hefl::cuda::note_launch();
+  wgrad0_reduce(ws, grid, dW, st);
+}
+
+void wgrad0_mma_compact(const void* X, const void* g, const uint8_t* amax, float* dW, float* ws, int B, int H, int W,
+                        int Hp, int Wp, cudaStream_t st) {
+  static bool attrs_set = false;
+  if (!attrs_set) {
+    cudaFuncSetAttribute(wgrad0_mma_compact_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemC);
+    cudaFuncSetAttribute(wgrad0_mma_compact_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, 100);
+    attrs_set = true;
+  }
+  const int grid = wgrad0_parts(B, Hp);
+  launch_pdl(wgrad0_mma_compact_kernel, dim3(grid), dim3(kT), kSmemC, st, reinterpret_cast<const __nv_bfloat16*>(X),
              reinterpret_cast<const __nv_bfloat16*>(g), amax, ws, B, H, W, Hp, Wp);
   hefl::cuda::note_launch();
   wgrad0_reduce(ws, grid, dW, st);

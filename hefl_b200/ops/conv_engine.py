@@ -2,9 +2,10 @@
 
 Replaces Keras' ``model.fit`` compute path (FLPyfhelin.py:118-136, :193) for the medical CNN:
 
-  input     preprocess_u8 (uint8 -> bf16 NHWC [P,16], 1/255, Philox affine augmentation; layer-1 input
-            carries pixels w, w+1, w+2 in its channels for RGB, the whole 3x3 neighbourhood for grayscale)
-            into one of two X0 slots — the trainer stages batch i+1 on a side stream while step i runs
+  input     preprocess_u8 (uint8 -> bf16 NHWC, 1/255, Philox affine augmentation; RGB: [P,4] = R, G, B, 0 by
+            default (``compact0``), else [P,16] with pixels w, w+1, w+2 in its channels; grayscale: [P,16] with the
+            whole 3x3 neighbourhood) into one of two X0 slots — the trainer stages batch i+1 on a side stream while
+            step i runs
   forward   6 x conv_fwd_pool  (TMA-fed tensor-core tap GEMMs, bias + ReLU + 2x2 max-pool + 3-bit
                                 arg-max/active code fused in the epilogue; only pooled tensors
                                 reach HBM; layer 1 on the pair-row variant: the whole pooling window
@@ -93,13 +94,17 @@ class MedCNNEngine:
         # layer-1 weight gradient by gather from the pooled gradient (csrc/nn/wgrad_gather.cu)
         self.gather_wgrad0 = (os.environ.get("HEFL_GATHER_WGRAD0", "1") != "0" and self.Co[0] == 32
                               and self.CK[0] == 16 and self.H[0] <= 256)
+        self._wgrad0_mma = not os.environ.get("HEFL_WGRAD0_MMA", "1").startswith("0")     # as wgrad0_mma.cu reads it
         bf = dict(dtype=torch.bfloat16, device=device)
         self.P = [B * self.H[l] * self.H[l] for l in range(self.n + 1)]
         # activations / gradients (all NHWC bf16 viewed as [pixels, channels])
         # layer-1 input with 8 pixels of slack: its wgrad reads 4-pixel windows (overlapping TMA rows)
         # two copies: batch i+1 is pre-processed into the other slot while step i trains (fl/trainer.py)
+        # Sized for the 16-channel layouts, which the switches below may select at any time; the compact RGB layout
+        # (``compact0``) uses the first quarter, so only the bytes it touches cost bandwidth.
         self._x0_bufs = [torch.zeros(self.P[0] + 8, 16, **bf) for _ in range(2)]
         self.X0 = [b[: self.P[0]] for b in self._x0_bufs]
+        self._x0c = [b.view(-1)[: self.P[0] * 4].view(self.P[0], 4) for b in self._x0_bufs]
         self._x0_base = self._x0_bufs[0]
         self.X = [self.X0[0]]
         self.amax, self.dY, self.gX = [], [], [None]
@@ -158,10 +163,25 @@ class MedCNNEngine:
         self.step_ref: Optional[torch.Tensor] = None     # device step counter (set by the trainer)
         self.after_restore()
 
+    @property
+    def compact0(self) -> bool:
+        """Layer-1 input as [P, 4] = R, G, B, 0 (8 bytes per pixel instead of 32) — the one place that picks it.
+        Only the RGB defaults read it: the s-packed layer 1 on the pair-row forward and the masked-GEMM weight gradient
+        (both have compact variants, conv_tcgen05.cu kPairC and wgrad0_mma.cu). Any switch that selects a layer-1
+        kernel needing 16 channels (HEFL_SPACK0=0, HEFL_FWD_PAIR=0, HEFL_GATHER_WGRAD0=0, HEFL_WGRAD0_MMA=0, odd
+        image sizes), or the same attributes changed after construction, gives the 16-channel layout back."""
+        h = self.H[0]
+        return (self.spack0 and self.Ci[0] == 3 and self.fwd_pair >= 1 and self.gather_wgrad0 and self._wgrad0_mma
+                and h % 2 == 0 and h <= 256)
+
+    def x0(self, slot: int) -> torch.Tensor:
+        """Layer-1 input buffer of ``slot`` in the current layout."""
+        return self._x0c[slot] if self.compact0 else self._x0_bufs[slot]
+
     # ------------------------------------------------------------------ weights
     def after_update(self) -> None:
         """Called after Adam wrote the bf16 shadow: rebuild the tensor-core weight layouts."""
-        self.ops.conv_weight_relayout(self.shadow, self.table, self.Wf, self.Wd, 0, -1, self.spack0)
+        self.ops.conv_weight_relayout(self.shadow, self.table, self.Wf, self.Wd, 0, -1, self.spack0, self.compact0)
 
     def after_restore(self) -> None:
         self.shadow.copy_(self.pack.trainable())
@@ -169,6 +189,10 @@ class MedCNNEngine:
 
     def _wf(self, l):
         return self.Wf[self.wf_off[l]: self.wf_off[l + 1]]
+
+    def _wf0c(self):
+        """Layer-1 weights of the compact input: [3 r][2 dx][Co][16], after the s-packed [3][Co][16] (conv_weight_relayout)."""
+        return self.Wf[self.wf_off[0] + 3 * self.Co[0] * 16: self.wf_off[1]]
 
     def _wd(self, l):
         return self.Wd[self.wd_off[l]: self.wd_off[l + 1]]
@@ -200,16 +224,19 @@ class MedCNNEngine:
         if train and augment:
             seed = (self.aug_seed + 0x9E3779B97F4A7C15 * (self.prep_count + 1)) & 0x7FFFFFFFFFFFFFFF or 1
             self.prep_count += 1
-        self.ops.preprocess_u8(x_u8, None, self.X0[slot], seed, None, self.spack0)     # channels from x_u8
+        compact = self.compact0
+        self.ops.preprocess_u8(x_u8, None, self._x0c[slot] if compact else self.X0[slot], seed, None, self.spack0,
+                               compact)     # channels from x_u8
 
     def forward_convs(self, slot: int, train: bool) -> torch.Tensor:
         x = self.X0[slot]
         for l in range(self.n):
             h = self.H[l]
             if l < self.fwd_pair and h % 2 == 0 and (h - 2) // 2 <= 128 and self.CK[l] <= 32 and self.Co[l] <= 64:
-                self.ops.conv_fwd_pool_pair(x if l else self._x0_bufs[slot], self._wf(l), self.bias[l], self.X[l + 1],
-                                            self.amax[l] if train else None, self.B, h, h, self.CK[l], self.Co[l],
-                                            self.spack0 and l == 0, self.Ci[0])
+                compact = l == 0 and self.compact0
+                self.ops.conv_fwd_pool_pair(x if l else self.x0(slot), self._wf0c() if compact else self._wf(l),
+                                            self.bias[l], self.X[l + 1], self.amax[l] if train else None, self.B, h, h,
+                                            self.CK[l], self.Co[l], self.spack0 and l == 0, self.Ci[0], compact)
                 x = self.X[l + 1]
                 continue
             self.ops.conv_fwd_pool(x, self._wf(l), self.bias[l], self.X[l + 1],
@@ -272,8 +299,8 @@ class MedCNNEngine:
                         opt.apply(self.p0, self.pack.n_trainable)
                         self.ops.conv_weight_relayout(self.shadow, self.table, self.Wf, self.Wd, 1, self.n)
                 # 1- or 3-channel layer: weight gradient gathered straight from the pooled gradient
-                self.ops.wgrad0_gather(self._x0_bufs[slot], g, self.amax[0], self._dw(0), self.B, h, h, self.spack0,
-                                       self.Ci[0])
+                self.ops.wgrad0_gather(self.x0(slot), g, self.amax[0], self._dw(0), self.B, h, h, self.spack0,
+                                       self.Ci[0], self.compact0)
                 break
             xin = self.X0[slot] if l == 0 else self.X[l]
             if self.dY[l] is None:
@@ -309,7 +336,7 @@ class MedCNNEngine:
         elif split:
             self.ops.conv_grad_finalize(self.dW32, self.table, self.pack.grad, 0, 1)
             opt.apply(0, self.p0)
-            self.ops.conv_weight_relayout(self.shadow, self.table, self.Wf, self.Wd, 0, 1, self.spack0)
+            self.ops.conv_weight_relayout(self.shadow, self.table, self.Wf, self.Wd, 0, 1, self.spack0, self.compact0)
         else:
             opt.bump()
             self.ops.conv_grad_finalize(self.dW32, self.table, self.pack.grad)
@@ -324,7 +351,7 @@ class MedCNNEngine:
                               step, lr_scale, cfg.lr, cfg.lr_decay, 0.9, 0.999, 1e-7, self.dense_off,
                               self.pack.n_trainable, anchor, mu)
         if self.spack0:
-            self.ops.conv_weight_relayout(self.shadow, self.table, self.Wf, self.Wd, 0, 1, True)
+            self.ops.conv_weight_relayout(self.shadow, self.table, self.Wf, self.Wd, 0, 1, True, self.compact0)
 
     def eval_step(self, x_u8: torch.Tensor, y: torch.Tensor, out: torch.Tensor) -> None:
         self.preprocess(x_u8, 0, False, False)

@@ -295,7 +295,9 @@ void pairwise_mask(uint64_t* data, int64_t numel, int L, int logn, const MaskArg
 }
 
 // Local K-way modular sum of K buffers living on ONE device (loopback transport on a single
-// GPU, and the aggregation step of the file-based compat path).
+// GPU, and the aggregation step of the file-based compat path). The accumulator is reduced after
+// every 7 addends: a reduced accumulator (< q) plus 7 residues stays <= 8 (q - 1) < 2^64 for q <= 2^61,
+// while plus 8 residues it can exceed 2^64 under a 61-bit prime.
 __global__ void local_sum_modq_kernel(const uint64_t* const* __restrict__ srcs, int K,
                                       uint64_t* __restrict__ out, int64_t numel, int logn, int L,
                                       const uint64_t* __restrict__ consts) {
@@ -310,7 +312,7 @@ __global__ void local_sum_modq_kernel(const uint64_t* const* __restrict__ srcs, 
       const ulonglong2 v = *reinterpret_cast<const ulonglong2*>(srcs[k] + e);
       acc.x += v.x;
       acc.y += v.y;
-      if ((k & 7) == 7) { acc.x = mod_sum(acc.x, q, rh); acc.y = mod_sum(acc.y, q, rh); }
+      if (k % 7 == 6) { acc.x = mod_sum(acc.x, q, rh); acc.y = mod_sum(acc.y, q, rh); }
     }
     acc.x = mod_sum(acc.x, q, rh);
     acc.y = mod_sum(acc.y, q, rh);

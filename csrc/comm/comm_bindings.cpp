@@ -155,7 +155,7 @@ void local_sum_modq(at::TensorList srcs, Tensor out, int64_t L, int64_t logn, co
     uint64_t acc = 0;
     for (int k = 0; k < K; ++k) {
       acc += sp[k][e];
-      if ((k & 7) == 7) acc = hefl::barrett_reduce_64(acc, m);
+      if (k % 7 == 6) acc = hefl::barrett_reduce_64(acc, m);   // as the kernel: < q plus 7 addends < 2^64
     }
     o[e] = hefl::barrett_reduce_64(acc, m);
   }

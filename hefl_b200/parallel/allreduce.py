@@ -79,7 +79,9 @@ class FusedTransport(Transport):
 
     def pick_algo(self, nbytes: int) -> str:
         if self.algo != "auto":
-            return self.algo
+            # one_shot has every rank load every peer's whole ciphertext, so a key holder turns a forced one_shot
+            # into two_shot (where it owns no chunk); multimem honours the key holder and is kept
+            return "two_shot" if self.algo == "one_shot" and self.no_owner >= 0 else self.algo
         if self.world == 1:
             return "two_shot"
         if nbytes <= 256 * 1024 and self.no_owner < 0:
@@ -115,7 +117,7 @@ class FusedTransport(Transport):
                                 self.sym.mc_ptr + off if self.sym.mc_ptr else 0, out, self.status,
                                 self.ctx.consts_cpu, numel, data.shape[-2], self.ctx.logn,
                                 self.rank, self.world, ALGOS[algo], blocks, self.threads,
-                                self.timeout_ms, self.no_owner if algo != "one_shot" else -1, self.stats)
+                                self.timeout_ms, self.no_owner, self.stats)
         src = self.out if algo == "one_shot" else base
         return src[e0:e0 + numel].view(data.shape)
 

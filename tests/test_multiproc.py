@@ -1,5 +1,6 @@
 """Multi-process tests. CPU (gloo, world 2) checks the host-side transport logic here;
-the GPU variants run the fused NVLink kernel across real devices on an H100."""
+the GPU variants run the fused NVLink kernel across real devices on an H100 and skip on a one-GPU machine.
+test_gpu_allreduce_ranks.py runs the same kernel with 1-8 logical ranks in one process on one GPU."""
 import json
 import os
 import subprocess

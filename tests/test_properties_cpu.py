@@ -68,6 +68,20 @@ def test_local_sum_matches_bigint(K, L, seed):
         assert [int(v) for v in out[:, l].reshape(-1)] == exp
 
 
+def test_local_sum_of_many_maximal_addends_under_61_bit_primes():
+    """q - 1 from every source under primes just below 2^61: 8 of them sum to just below 2^64, so a reduced
+    accumulator may take only 7 more before the next reduction."""
+    logn, n, L = 10, 1024, 3
+    primes = ops.gen_primes(61, logn, L, [])
+    _, consts = ops.build_tables(primes, logn)
+    top = torch.stack([torch.full((2, n), int(q) - 1, dtype=torch.int64) for q in primes], dim=1).contiguous()
+    for K in (1, 7, 8, 9, 15, 16, 17, 24, 25, 64):
+        out = torch.empty_like(top)
+        ops.local_sum_modq([top] * K, out, L, logn, consts)
+        for l, q in enumerate(int(v) for v in primes):
+            assert torch.equal(out[:, l], torch.full((2, n), K * (q - 1) % q, dtype=torch.int64)), (K, l)
+
+
 def test_serialization_golden_bytes():
     """Byte-level fixture of the HEFL stream header (format version 1)."""
     ctx = CKKSContext(4096, prime_bits=(36, 36, 37), scale_bits=40)

@@ -12,8 +12,6 @@ The decode reference is exact CRT centring with Python integers followed by a pl
 of m is m(zeta^(5^j)) with zeta = exp(i*pi/N), i.e. 2N * ifft(pad(m, 2N))[5^j mod 2N]. The CPU tests tie it to
 `oracle.ckks_slots_of` and to the host twin; the GPU tests compare the fused decode kernel with both."""
 import contextlib
-import re
-import warnings
 
 import numpy as np
 import pytest
@@ -23,40 +21,13 @@ from hefl_b200 import _ext
 from hefl_b200.he import oracle
 from hefl_b200.he.bfv import BFVFracContext, BFVRelinKey
 from hefl_b200.he.context import CKKSContext, CtBatch
+from kernel_trace import kernels_run, ran
 
 ops = _ext.ops()
 gpu = pytest.mark.gpu
 
 
 # ---------------------------------------------------------------------------------------------- helpers
-def kernels_run(fn, attempts=3):
-    """Runs fn() under torch.profiler and returns (its result, the names of the CUDA kernels it launched).
-
-    Now and then the profiler hands back a trace with no device activity at all although fn launched native
-    kernels (the launch counter moved). Such a trace says nothing about which kernel ran, so fn, which must be
-    repeatable, runs again under a fresh profiler, up to `attempts` times. A trace with any kernel in it is final."""
-    from torch.profiler import ProfilerActivity, profile
-
-    for _ in range(attempts):
-        torch.cuda.synchronize()
-        launches = int(ops.launch_count())
-        with profile(activities=[ProfilerActivity.CPU, ProfilerActivity.CUDA]) as prof:
-            out = fn()
-            torch.cuda.synchronize()
-        names = {e.name for e in prof.events() if e.device_type == torch.autograd.DeviceType.CUDA}
-        if names or int(ops.launch_count()) == launches:
-            break
-        warnings.warn("torch.profiler returned no device activity for launched kernels; running again")
-    return out, names
-
-
-def ran(names, kernel):
-    """True if a launched kernel's demangled name contains `kernel` (e.g. "ntt2_kernel<12, true, 3u>") as a whole
-    identifier."""
-    pat = re.compile(r"(?<![\w])" + re.escape(kernel))
-    return any(pat.search(n) for n in names)
-
-
 @pytest.fixture
 def cta_budget():
     """`with cta_budget(ntt, enc, dec):` sets the persistent kernels' per-role CTA budgets and restores the whole chip

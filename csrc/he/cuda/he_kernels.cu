@@ -545,7 +545,7 @@ void coeff_encode(const float* vals, int64_t C, int64_t nvals_total, int n, doub
 // Fused public-key encryption (K6): sample -> NTT -> multiply-add with pk, one CTA per
 // (ciphertext, limb). TWO_BUF keeps NTT(u) in a second shared buffer so each output word is
 // written exactly once; for N = 16384 one buffer is used and the partial products make a
-// round trip through L2.
+// round trip through L2. acc: ct = (ct + Enc(m)) mod q, the old word read where it is stored.
 // ------------------------------------------------------------------------------------------
 
 template <bool TWO_BUF>
@@ -553,7 +553,7 @@ __global__ void __launch_bounds__(1024)
 encrypt_kernel(const int64_t* __restrict__ msg, const uint64_t* __restrict__ pk,
                uint64_t* __restrict__ ct, int L, int logn, const uint64_t* __restrict__ tables,
                const uint64_t* __restrict__ consts, const uint64_t* __restrict__ msg_scale,
-               uint64_t seed, uint32_t ct_offset) {
+               uint64_t seed, uint32_t ct_offset, bool acc) {
   extern __shared__ uint64_t smem[];
   const int n = 1 << logn;
   const int64_t c = blockIdx.x / L;
@@ -577,8 +577,8 @@ encrypt_kernel(const int64_t* __restrict__ msg, const uint64_t* __restrict__ pk,
   if (!TWO_BUF) {
     for (int i = threadIdx.x; i < n; i += blockDim.x) {
       const uint64_t uh = reduce_4q(bufU[pad_idx(i)], T.q);
-      c0[i] = mul_mod(uh, pk0[i], m);
-      c1[i] = mul_mod(uh, pk1[i], m);
+      c0[i] = mad_mod(uh, pk0[i], acc ? c0[i] : 0, m);
+      c1[i] = mad_mod(uh, pk1[i], acc ? c1[i] : 0, m);
     }
     __syncthreads();
   }
@@ -593,7 +593,7 @@ encrypt_kernel(const int64_t* __restrict__ msg, const uint64_t* __restrict__ pk,
     const uint64_t a = reduce_4q(bufA[pad_idx(i)], T.q);
     if (TWO_BUF) {
       const uint64_t uh = reduce_4q(bufU[pad_idx(i)], T.q);
-      c0[i] = mad_mod(uh, pk0[i], a, m);
+      c0[i] = mad_mod(uh, pk0[i], acc ? add_mod(a, c0[i], T.q) : a, m);
     } else {
       c0[i] = add_mod(c0[i], a, T.q);
     }
@@ -608,7 +608,7 @@ encrypt_kernel(const int64_t* __restrict__ msg, const uint64_t* __restrict__ pk,
     const uint64_t b = reduce_4q(bufA[pad_idx(i)], T.q);
     if (TWO_BUF) {
       const uint64_t uh = reduce_4q(bufU[pad_idx(i)], T.q);
-      c1[i] = mad_mod(uh, pk1[i], b, m);
+      c1[i] = mad_mod(uh, pk1[i], acc ? add_mod(b, c1[i], T.q) : b, m);
     } else {
       c1[i] = add_mod(c1[i], b, T.q);
     }
@@ -640,7 +640,7 @@ __global__ void enc_sample_kernel(const int64_t* __restrict__ msg, uint64_t* __r
 __global__ void enc_combine_kernel(const uint64_t* __restrict__ u, const uint64_t* __restrict__ a,
                                    const uint64_t* __restrict__ b, const uint64_t* __restrict__ pk,
                                    uint64_t* __restrict__ ct, int L, int n,
-                                   const uint64_t* __restrict__ consts) {
+                                   const uint64_t* __restrict__ consts, bool acc) {
   const int64_t c = blockIdx.y / L;
   const int l = blockIdx.y % L;
   const uint64_t* cc = consts + (size_t)l * 8;
@@ -652,14 +652,14 @@ __global__ void enc_combine_kernel(const uint64_t* __restrict__ u, const uint64_
   const uint64_t* pk1 = pk + (size_t)(1 * L + l) * n;
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
     const uint64_t uh = u[row + i];
-    c0[i] = mad_mod(uh, pk0[i], a[row + i], m);
-    c1[i] = mad_mod(uh, pk1[i], b[row + i], m);
+    c0[i] = mad_mod(uh, pk0[i], acc ? add_mod(a[row + i], c0[i], m.q) : a[row + i], m);
+    c1[i] = mad_mod(uh, pk1[i], acc ? add_mod(b[row + i], c1[i], m.q) : b[row + i], m);
   }
 }
 
 void encrypt(const int64_t* msg, const uint64_t* pk, uint64_t* ct, int64_t C, int L, int logn,
              const uint64_t* tables, const uint64_t* consts, const uint64_t* msg_scale,
-             uint64_t seed, uint32_t ct_offset, cudaStream_t st) {
+             uint64_t seed, uint32_t ct_offset, bool accumulate, cudaStream_t st) {
   if (C == 0) return;
   const int n = 1 << logn;
   if (logn <= 14) {
@@ -668,10 +668,12 @@ void encrypt(const int64_t* msg, const uint64_t* pk, uint64_t* ct, int64_t C, in
     const size_t smem = ntt_smem_bytes(logn) * (two ? 2 : 1);
     if (two) {
       set_smem(encrypt_kernel<true>, smem);
-      encrypt_kernel<true><<<(unsigned)(C * L), threads, smem, st>>>(msg, pk, ct, L, logn, tables, consts, msg_scale, seed, ct_offset);
+      encrypt_kernel<true><<<(unsigned)(C * L), threads, smem, st>>>(msg, pk, ct, L, logn, tables, consts, msg_scale, seed,
+                                                                     ct_offset, accumulate);
     } else {
       set_smem(encrypt_kernel<false>, smem);
-      encrypt_kernel<false><<<(unsigned)(C * L), threads, smem, st>>>(msg, pk, ct, L, logn, tables, consts, msg_scale, seed, ct_offset);
+      encrypt_kernel<false><<<(unsigned)(C * L), threads, smem, st>>>(msg, pk, ct, L, logn, tables, consts, msg_scale, seed,
+                                                                      ct_offset, accumulate);
     }
     note_launch();
     return;
@@ -686,7 +688,7 @@ void encrypt(const int64_t* msg, const uint64_t* pk, uint64_t* ct, int64_t C, in
   enc_sample_kernel<<<grid, 256, 0, st>>>(msg, u, a, b, L, n, consts, msg_scale, seed, ct_offset);
   note_launch();
   ntt(u, 3 * C * L, L, logn, tables, consts, false, st);  // rows keep (row % L) == limb
-  enc_combine_kernel<<<grid, 256, 0, st>>>(u, a, b, pk, ct, L, n, consts);
+  enc_combine_kernel<<<grid, 256, 0, st>>>(u, a, b, pk, ct, L, n, consts, accumulate);
   note_launch();
   cudaFreeAsync(u, st);
 }

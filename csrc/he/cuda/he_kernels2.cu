@@ -239,6 +239,7 @@ struct EncArgs {
   int L;
   int64_t C;
   uint64_t* scratch;        // N = 16384 only: [grid][N] words for u_hat, private to the launch
+  bool acc;                 // ct = (ct + Enc(m)) mod q: the epilogue reads the old word where it stores the new one
 };
 
 __device__ __forceinline__ uint32_t pack_e(int e0, int e1) { return ((uint32_t)e0 & 0xFFu) | (((uint32_t)e1 & 0xFFu) << 8); }
@@ -253,7 +254,7 @@ __device__ __forceinline__ int unpack_e1(uint32_t p) { return (int)(int8_t)((p >
 template <int LOGN, bool USCR>
 __device__ __forceinline__ void enc_epilogue(uint32_t bufA, uint32_t bufU, const uint64_t* uscr, const Limb& T,
                                              const uint64_t* pkx_limb, uint64_t* ct, int64_t c_first, int64_t C,
-                                             int which, int L, int limb) {
+                                             int which, int L, int limb, bool acc) {
   constexpr int NP = num_passes(LOGN);
   constexpr int N = 1 << LOGN;
   using GG = Geo<LOGN, NP - 1>;
@@ -290,6 +291,13 @@ __device__ __forceinline__ void enc_epilogue(uint32_t bufA, uint32_t bufU, const
         uint64_t s = t + lazy_reduce(x[4 * v + k], T);     // < 4q
         s = s >= T.two_q ? s - T.two_q : s;
         r[k] = s >= T.q ? s - T.q : s;
+      }
+      if (acc && c < C) {
+        uint64_t old[4];
+        asm volatile("ld.global.v2.u64 {%0, %1}, [%2];" : "=l"(old[0]), "=l"(old[1]) : "l"(o + 4 * v) : "memory");
+        asm volatile("ld.global.v2.u64 {%0, %1}, [%2];" : "=l"(old[2]), "=l"(old[3]) : "l"(o + 4 * v + 2) : "memory");
+#pragma unroll
+        for (int k = 0; k < 4; ++k) r[k] = add_mod(r[k], old[k], T.q);
       }
       if (c < C) stg256(o + 4 * v, r[0], r[1], r[2], r[3]);
     }
@@ -392,7 +400,7 @@ encrypt2_kernel(const __grid_constant__ CUtensorMap tmap, EncArgs a) {
     compute_sync();
     if constexpr (NP >= 3) fwd_pass_smem<LOGN, 1>(bufA, T);
     if constexpr (NP >= 4) fwd_pass_smem<LOGN, 2>(bufA, T);
-    enc_epilogue<LOGN, USCR>(bufA, bufU, uscr, T, pk0, a.ct, c_first, a.C, 0, a.L, W.limb);
+    enc_epilogue<LOGN, USCR>(bufA, bufU, uscr, T, pk0, a.ct, c_first, a.C, 0, a.L, W.limb, a.acc);
     // ---- phase 3: c1 = u_hat * pk1 + NTT(e1) ----
 #pragma unroll
     for (int j = 0; j < PT; ++j) {
@@ -409,7 +417,7 @@ encrypt2_kernel(const __grid_constant__ CUtensorMap tmap, EncArgs a) {
     compute_sync();
     if constexpr (NP >= 3) fwd_pass_smem<LOGN, 1>(bufA, T);
     if constexpr (NP >= 4) fwd_pass_smem<LOGN, 2>(bufA, T);
-    enc_epilogue<LOGN, USCR>(bufA, bufU, uscr, T, pk1, a.ct, c_first, a.C, 1, a.L, W.limb);
+    enc_epilogue<LOGN, USCR>(bufA, bufU, uscr, T, pk1, a.ct, c_first, a.C, 1, a.L, W.limb, a.acc);
   }
   cluster_sync_all();
 }
@@ -663,7 +671,7 @@ int64_t encrypt2_scratch_words(int logn) { return logn >= 14 ? (int64_t)grid_cta
 
 bool encrypt2(const int64_t* msg, const uint64_t* pkx, uint64_t* ct, int64_t C, int L, int logn, const uint64_t* tw2,
               const uint64_t* consts, const uint64_t* msg_scale, uint64_t seed, uint32_t ct_offset, int qbits,
-              uint64_t* scratch, cudaStream_t st) {
+              uint64_t* scratch, bool accumulate, cudaStream_t st) {
   if (C == 0) return true;
   if (!ntt2_supported(logn, L, qbits)) return false;
   if (logn >= 14 && scratch == nullptr) return false;
@@ -675,7 +683,7 @@ bool encrypt2(const int64_t* msg, const uint64_t* pkx, uint64_t* ct, int64_t C, 
     const int64_t workers = (grid_ctas(1) / 2 / L) * 2;
     if (units < 2 * workers) return false;
   }
-  const EncArgs a{msg, pkx, ct, tw2, consts, msg_scale, seed, ct_offset, L, C, scratch};
+  const EncArgs a{msg, pkx, ct, tw2, consts, msg_scale, seed, ct_offset, L, C, scratch, accumulate};
   switch (logn) {
     case 10: launch_encrypt2<10>(a, st); break;
     case 11: launch_encrypt2<11>(a, st); break;

@@ -365,12 +365,13 @@ void ckks_decode_server_step_(const Tensor& res, const Tensor& consts_cpu, int64
 
 void encrypt_out(const c10::optional<Tensor>& msg, const Tensor& pk, int64_t C, int64_t L, int64_t logn,
                  const Tensor& tables, const Tensor& consts, const c10::optional<Tensor>& msg_scale,
-                 int64_t seed, int64_t ct_offset, Tensor ct) {
+                 int64_t seed, int64_t ct_offset, Tensor ct, bool accumulate) {
   same_device(pk, tables);
   same_device(pk, ct);
   const int64_t n = 1ll << logn;
   TORCH_CHECK(pk.numel() == 2 * L * n, "pk must be [2,L,N]");
   TORCH_CHECK(ct.numel() >= C * 2 * L * n, "output buffer too small");
+  TORCH_CHECK(!accumulate || ct.is_contiguous(), "accumulate reads the output buffer: it must be contiguous");
   const int64_t* mp = nullptr;
   if (msg.has_value()) {
     same_device(*msg, pk);
@@ -387,22 +388,22 @@ void encrypt_out(const c10::optional<Tensor>& msg, const Tensor& pk, int64_t C, 
         if (const int64_t words = hefl::cuda::encrypt2_scratch_words((int)logn)) scratch = at::empty({words}, pk.options());
         if (hefl::cuda::encrypt2(mp, u64(pkx), u64(ct), C, (int)L, (int)logn, u64(te.tw2), u64(consts),
                                  u64o(msg_scale), (uint64_t)seed, (uint32_t)ct_offset, te.qbits,
-                                 scratch.defined() ? u64(scratch) : nullptr, cur_stream()))
+                                 scratch.defined() ? u64(scratch) : nullptr, accumulate, cur_stream()))
           return;
       }
     }
     hefl::cuda::encrypt(mp, u64(pk), u64(ct), C, (int)L, (int)logn, u64(tables), u64(consts),
-                        u64o(msg_scale), (uint64_t)seed, (uint32_t)ct_offset, cur_stream());
+                        u64o(msg_scale), (uint64_t)seed, (uint32_t)ct_offset, accumulate, cur_stream());
   } else
     hefl::host::encrypt(mp, u64(pk), u64(ct), C, (int)L, (int)logn, u64(tables), u64(consts),
-                        u64o(msg_scale), (uint64_t)seed, (uint32_t)ct_offset);
+                        u64o(msg_scale), (uint64_t)seed, (uint32_t)ct_offset, accumulate);
 }
 
 Tensor encrypt(const c10::optional<Tensor>& msg, const Tensor& pk, int64_t C, int64_t L, int64_t logn,
                const Tensor& tables, const Tensor& consts, const c10::optional<Tensor>& msg_scale,
                int64_t seed, int64_t ct_offset) {
   Tensor ct = at::empty({C, 2, L, 1ll << logn}, pk.options());
-  encrypt_out(msg, pk, C, L, logn, tables, consts, msg_scale, seed, ct_offset, ct);
+  encrypt_out(msg, pk, C, L, logn, tables, consts, msg_scale, seed, ct_offset, ct, false);
   return ct;
 }
 
@@ -597,7 +598,7 @@ TORCH_LIBRARY_FRAGMENT(hefl, m) {
   m.def("ckks_decode_residues(Tensor res, Tensor consts_cpu, int q0_inv_q1, int logn, float inv_scale, Tensor rot, Tensor ksi, int nvals) -> Tensor", &ckks_decode_residues);
   m.def("ckks_decode_server_step_(Tensor res, Tensor consts_cpu, int q0_inv_q1, int logn, float inv_scale, Tensor rot, Tensor ksi, int nvals, int g0, int n_trainable, Tensor x_t, Tensor(a!) x_new, Tensor(b!) m, Tensor(c!) v, int opt, float lr, float beta1, float beta2, float tau, Tensor(d!)? avg_out=None) -> ()", &ckks_decode_server_step_);
   m.def("encrypt(Tensor? msg, Tensor pk, int C, int L, int logn, Tensor tables, Tensor consts, Tensor? msg_scale, int seed, int ct_offset) -> Tensor", &encrypt);
-  m.def("encrypt_out(Tensor? msg, Tensor pk, int C, int L, int logn, Tensor tables, Tensor consts, Tensor? msg_scale, int seed, int ct_offset, Tensor(a!) out) -> ()", &encrypt_out);
+  m.def("encrypt_out(Tensor? msg, Tensor pk, int C, int L, int logn, Tensor tables, Tensor consts, Tensor? msg_scale, int seed, int ct_offset, Tensor(a!) out, bool accumulate=False) -> ()", &encrypt_out);
   m.def("decrypt(Tensor ct, Tensor sk, int k, int logn, Tensor tables, Tensor consts) -> Tensor", &decrypt);
   m.def("keygen_secret(int L, int logn, Tensor tables, Tensor consts, int seed) -> Tensor", &keygen_secret);
   m.def("keygen_public(Tensor sk, int L, int logn, Tensor tables, Tensor consts, int seed, int idx) -> Tensor", &keygen_public);

@@ -379,7 +379,7 @@ void coeff_encode(const float* vals, int64_t C, int64_t nvals_total, int n, doub
 
 void encrypt(const int64_t* msg, const uint64_t* pk, uint64_t* ct, int64_t C, int L, int logn,
              const uint64_t* tables, const uint64_t* consts, const uint64_t* msg_scale,
-             uint64_t seed, uint32_t ct_offset) {
+             uint64_t seed, uint32_t ct_offset, bool accumulate) {
   const int64_t n = 1ll << logn;
 #pragma omp parallel for schedule(static) collapse(2)
   for (int64_t c = 0; c < C; ++c) {
@@ -404,8 +404,8 @@ void encrypt(const int64_t* msg, const uint64_t* pk, uint64_t* ct, int64_t C, in
       const uint64_t* pk0 = pk + (int64_t)(0 * L + l) * n;
       const uint64_t* pk1 = pk + (int64_t)(1 * L + l) * n;
       for (int64_t i = 0; i < n; ++i) {
-        c0[i] = mad_mod(u[i], pk0[i], a[i], m);
-        c1[i] = mad_mod(u[i], pk1[i], b[i], m);
+        c0[i] = mad_mod(u[i], pk0[i], accumulate ? add_mod(a[i], c0[i], m.q) : a[i], m);
+        c1[i] = mad_mod(u[i], pk1[i], accumulate ? add_mod(b[i], c1[i], m.q) : b[i], m);
       }
     }
   }

@@ -51,7 +51,7 @@ void coeff_encode(const float* vals, int64_t C, int64_t nvals_total, int n, doub
                   int64_t* msg);
 void encrypt(const int64_t* msg, const uint64_t* pk, uint64_t* ct, int64_t C, int L, int logn,
              const uint64_t* tables, const uint64_t* consts, const uint64_t* msg_scale,
-             uint64_t seed, uint32_t ct_offset);
+             uint64_t seed, uint32_t ct_offset, bool accumulate);
 void decrypt(const uint64_t* ct, const uint64_t* sk, uint64_t* out, int64_t C, int Lct, int k,
              int logn, const uint64_t* tables, const uint64_t* consts);
 void crt_center(const uint64_t* res, int64_t C, int k, int n, const uint64_t* consts, double* out);

@@ -37,9 +37,10 @@ void ckks_decode_server_step(const uint64_t* res, int64_t C, int k, int logn, ui
                              int64_t nvals, const ServerStep& sv, int opt, double* scratch, cudaStream_t st);
 void coeff_encode(const float* vals, int64_t C, int64_t nvals_total, int n, double scale,
                   int64_t* msg, cudaStream_t st);
+// accumulate: ct = (ct + Enc(m)) mod q word by word (the rank's clients summed without a buffer per client)
 void encrypt(const int64_t* msg, const uint64_t* pk, uint64_t* ct, int64_t C, int L, int logn,
              const uint64_t* tables, const uint64_t* consts, const uint64_t* msg_scale,
-             uint64_t seed, uint32_t ct_offset, cudaStream_t st);
+             uint64_t seed, uint32_t ct_offset, bool accumulate, cudaStream_t st);
 void decrypt(const uint64_t* ct, const uint64_t* sk, uint64_t* out, int64_t C, int Lct, int k,
              int logn, const uint64_t* tables, const uint64_t* consts, cudaStream_t st);
 void crt_center(const uint64_t* res, int64_t C, int k, int n, uint64_t q0, uint64_t q1,
@@ -77,7 +78,7 @@ bool ntt2(uint64_t* data, int64_t rows, int L, int logn, const uint64_t* tw2, co
 int64_t encrypt2_scratch_words(int logn);
 bool encrypt2(const int64_t* msg, const uint64_t* pkx, uint64_t* ct, int64_t C, int L, int logn, const uint64_t* tw2,
               const uint64_t* consts, const uint64_t* msg_scale, uint64_t seed, uint32_t ct_offset, int qbits,
-              uint64_t* scratch, cudaStream_t st);
+              uint64_t* scratch, bool accumulate, cudaStream_t st);
 bool decrypt2(const uint64_t* ct, const uint64_t* skx, uint64_t* out, int64_t C, int Lct, int k, int logn,
               const uint64_t* tw2, const uint64_t* consts, int Ltab, int qbits, cudaStream_t st);
 

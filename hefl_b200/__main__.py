@@ -1,5 +1,5 @@
-"""Command-line launcher of the product path: multi-round encrypted federated training, one client per
-process (one process per GPU under ``torchrun``; a single process on CPU or one GPU is a 1-client federation).
+"""Command-line launcher of the product path: multi-round encrypted federated training, one client (or
+``--clients-per-rank`` clients) per process (one process per GPU under ``torchrun``; a single process on CPU or one GPU is a 1-client federation).
 
     # 8 clients on one box, 3 rounds of the reference's medical-CNN recipe (10 local epochs each)
     torchrun --nproc-per-node 8 -m hefl_b200 --rounds 3 --log-jsonl run.jsonl --checkpoint ckpt.pt
@@ -10,6 +10,8 @@ process (one process per GPU under ``torchrun``; a single process on CPU or one 
     torchrun --nproc-per-node 8 -m hefl_b200 --dirichlet-alpha 0.3 --fedavg-weighting samples --fedprox-mu 0.01
     # ... with a server optimizer: FedAdam (eta 0.1, beta1 0.9, beta2 0.99, tau 1e-3) fused into the CKKS decode
     torchrun --nproc-per-node 8 -m hefl_b200 --dirichlet-alpha 0.3 --server-opt fedadam --server-lr 0.1
+    # 8 clients on one GPU, half of them sampled per round (DESIGN.md §9)
+    python -m hefl_b200 --clients-per-rank 8 --client-fraction 0.5 --dirichlet-alpha 0.3 --fedavg-weighting samples
 
 Every ``FLConfig`` field is a flag (``--local-epochs 10``) or an environment variable
 (``HEFL_LOCAL_EPOCHS=10``); the reference hard-codes all of them (FLPyfhelin.py:31-36, notebook N:24-32).
@@ -80,15 +82,21 @@ def main(argv=None) -> int:
             dist.init_process_group("nccl", device_id=device)
         else:
             dist.init_process_group("gloo")
-    cfg.clients = world
+    from .fl.runner import check_client_options
+
+    check_client_options(cfg)
+    M = cfg.clients_per_rank
+    cfg.clients = world * M
     dataset = None
     if ns.data_dir:
         from .fl.data import ImageFolderDataset
 
-        dataset = ImageFolderDataset(ns.data_dir, cfg.image_size, cfg.in_channels, index=rank, num_clients=world,
-                                     shuffle_seed=cfg.seed, stream=ns.stream_decode,
-                                     dirichlet_alpha=cfg.dirichlet_alpha, min_train=cfg.batch_size)
-        cfg.num_classes = max(cfg.num_classes, dataset.classes)
+        # one shard per client of this rank, in client-id order
+        dataset = [ImageFolderDataset(ns.data_dir, cfg.image_size, cfg.in_channels, index=cid, num_clients=cfg.clients,
+                                      shuffle_seed=cfg.seed, stream=ns.stream_decode,
+                                      dirichlet_alpha=cfg.dirichlet_alpha, min_train=cfg.batch_size)
+                   for cid in range(rank * M, rank * M + M)]
+        cfg.num_classes = max(cfg.num_classes, dataset[0].classes)
     run = FederatedRunner(cfg, rank=rank, world=world, device=device, dataset=dataset)
     if ns.checkpoint and os.path.exists(ns.checkpoint):
         run.load_checkpoint(ns.checkpoint)
@@ -99,8 +107,12 @@ def main(argv=None) -> int:
         rec["stage_ms_max"] = StageTimes.max_over_ranks(rec["stage_ms"], device, None)
         run.log.write(rec)
         if rank == 0:
-            print(json.dumps({"round": rec["round"], "loss": rec["loss"], "accuracy": rec["accuracy"],
-                              "stage_ms_max": rec["stage_ms_max"], "clients": world, "transport": rec["transport"]}))
+            line = {"round": rec["round"], "loss": rec["loss"], "accuracy": rec["accuracy"],
+                    "stage_ms_max": rec["stage_ms_max"], "clients": cfg.clients, "transport": rec["transport"]}
+            if "selected" in rec:                    # several clients per rank or client sampling
+                line["selected"] = rec["selected"]
+                line["rank0_clients"] = rec["clients"]
+            print(json.dumps(line))
         if ns.checkpoint:
             run.save_checkpoint(ns.checkpoint)       # rank 0: global model; every rank: its own optimiser / RNG state
         if world > 1:

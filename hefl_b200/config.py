@@ -70,6 +70,10 @@ class FLConfig:
     debug_precision: bool = False             # also all-reduce the PLAINTEXT updates and record the CKKS error of the
                                               # round (debug only: it defeats the privacy the ciphertext path provides)
     debug_poison: bool = False                # overwrite ciphertext / scratch buffers with a poison pattern between rounds
+    # many clients per rank (DESIGN.md §9): the federation has world x clients_per_rank clients; rank r hosts ids
+    # r*M .. r*M+M-1, each with its own shard, optimiser state and randomness, encrypted into the rank's ciphertext
+    clients_per_rank: int = 1
+    client_fraction: float = 1.0              # C: each round trains max(1, round(C*K)) clients, drawn from (seed, round)
     # non-IID clients (DESIGN.md §7)
     dirichlet_alpha: float = 0.0              # 0: equal IID shards; > 0: Dirichlet(alpha) label-skew shards of one pool
     fedavg_weighting: str = "uniform"         # uniform (1/K) | samples (n_k / N, McMahan et al.'s FedAvg)

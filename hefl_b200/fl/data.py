@@ -238,6 +238,19 @@ class BatchFeeder:
         self._ready = [torch.cuda.Event() if self.cuda else None for _ in range(2)]
         self._consumed = [torch.cuda.Event() if self.cuda else None for _ in range(2)]
         self.bytes_per_step = int(np.prod(shp)) + batch_size * 8
+        self.drop_last = drop_last
+
+    def retarget(self, ds, indices, gen: torch.Generator) -> None:
+        """Serve another client of the rank: its dataset, index set and shuffle generator, through the same
+        pinned staging buffers, device slots and copy stream (pinned memory is slow to allocate and finite)."""
+        shape = tuple(ds.image_shape) if getattr(ds, "images", None) is None else tuple(ds.images.shape[1:])
+        if shape != tuple(self._dev_x[0].shape[1:]) or (getattr(ds, "images", None) is None) != self.streaming:
+            raise ValueError(f"retarget: every client of a rank needs images of one shape, got {shape}")
+        self.ds = ds
+        self.indices = torch.tensor(list(indices), dtype=torch.int64)
+        n = len(self.indices)
+        self.steps = n // self.bs if self.drop_last else (n + self.bs - 1) // self.bs
+        self.gen = gen
 
     def _order(self) -> torch.Tensor:
         if self.shuffle:

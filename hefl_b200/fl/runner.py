@@ -1,4 +1,5 @@
-"""Federated round loop: one client per rank (one process per GPU), encrypted FedAvg.
+"""Federated round loop: one client per rank (one process per GPU), or several (``clients_per_rank``, DESIGN.md §9),
+encrypted FedAvg.
 
 One round = what the reference's notebook cell 3 does once (N:233-272):
 ``train_clients`` (FLPyfhelin.py:179-198) -> ``export_encrypted_clients_weights`` (:242) ->
@@ -41,6 +42,24 @@ from .trainer import LocalTrainer
 FEDAVG_WEIGHTINGS = ("uniform", "samples")
 
 
+def check_client_options(cfg: FLConfig) -> None:
+    """Reject out-of-range client placement / sampling settings (they arrive from flags and environment variables)."""
+    if not (isinstance(cfg.clients_per_rank, int) and cfg.clients_per_rank >= 1):
+        raise ValueError(f"clients_per_rank must be an integer >= 1, got {cfg.clients_per_rank!r}")
+    if not 0 < cfg.client_fraction <= 1:
+        raise ValueError(f"client_fraction must be in (0, 1], got {cfg.client_fraction}")
+
+
+def select_clients(cfg: FLConfig, num_clients: int, rnd: int) -> List[int]:
+    """The ids that train in round ``rnd``: all of them, or max(1, round(C*K)) drawn without replacement from a
+    generator seeded by (seed, round), so every rank computes the same set without communicating."""
+    if cfg.client_fraction >= 1:
+        return list(range(num_clients))
+    count = max(1, round(cfg.client_fraction * num_clients))
+    g = torch.Generator().manual_seed((cfg.seed * 1_000_003 + rnd) & 0x7FFFFFFFFFFFFFFF)
+    return sorted(torch.randperm(num_clients, generator=g)[:count].tolist())
+
+
 def check_noniid_options(cfg: FLConfig) -> None:
     """Reject out-of-range non-IID settings (they arrive from flags and environment variables)."""
     if not cfg.dirichlet_alpha >= 0:
@@ -56,6 +75,7 @@ class FederatedRunner:
                  device: Optional[torch.device] = None, samples_per_client: Optional[int] = None, dataset=None):
         check_noniid_options(cfg)
         check_server_options(cfg)
+        check_client_options(cfg)
         self.cfg = cfg
         self.rank, self.world, self.group = rank, world, group
         self.device = device or torch.device(cfg.device if torch.cuda.is_available() or cfg.device == "cpu" else "cpu")
@@ -84,37 +104,74 @@ class FederatedRunner:
                                         **({"algo": cfg.allreduce_algo, "timeout_s": cfg.timeout_s,
                                             "no_owner": self.key_holder} if kind == "fused" else {}))
         self._pair_seeds = self._agree_pair_seeds() if (cfg.pairwise_masks and world > 1) else None
+        # clients: rank r hosts ids r*M .. r*M+M-1 of a federation of K = world*M; everything a client draws is keyed
+        # by its id, so a client trains the same wherever it is placed (DESIGN.md §9)
+        M = int(cfg.clients_per_rank)
+        self.clients_per_rank, self.num_clients = M, world * M
+        self.client_ids = list(range(rank * M, rank * M + M))
+        self.multi = M > 1 or cfg.client_fraction < 1      # the per-client round; M = 1, C = 1 is the 1-client rank
+        datasets = list(dataset) if isinstance(dataset, (list, tuple)) else [dataset] if dataset is not None else None
+        if datasets is not None and len(datasets) != M:
+            raise ValueError(f"dataset: {len(datasets)} datasets for {M} clients per rank (one per client, in id order)")
         # data: IID contiguous shard of a synthetic set (FLPyfhelin.py:75-78), 90/10 split (:85)
         # or, with ``dataset`` (e.g. ImageFolderDataset of this client's shard), real images: 10 % validate
-        if dataset is not None:
-            self.dataset = dataset
-            per = len(dataset)
-            nval = int(per * 0.1)
-        elif cfg.dirichlet_alpha > 0:
-            # label-skew shard: this client's Dirichlet part of one pooled set of world x per samples (the pool
-            # and the partition are the same on every rank); 10 % of the part validates
+        pool = parts = None
+        if datasets is None and cfg.dirichlet_alpha > 0:
+            # label-skew shard: this client's Dirichlet part of one pooled set of K x per samples (the pool and the
+            # partition are the same on every rank); 10 % of the part validates
             per = samples_per_client or (cfg.steps_per_epoch * cfg.batch_size + cfg.val_steps * cfg.batch_size)
-            pool = SyntheticImageDataset(world * per, cfg.image_size, cfg.in_channels, cfg.num_classes,
+            pool = SyntheticImageDataset(self.num_clients * per, cfg.image_size, cfg.in_channels, cfg.num_classes,
                                          seed=cfg.seed, pin=False)
-            part = dirichlet_partition(pool.labels, world, cfg.dirichlet_alpha, cfg.seed, cfg.batch_size)[rank]
-            self.dataset = pool.subset(part)
-            del pool
-            per = len(self.dataset)
-            nval = int(per * 0.1)
-        else:
-            per = samples_per_client or (cfg.steps_per_epoch * cfg.batch_size + cfg.val_steps * cfg.batch_size)
-            self.dataset = SyntheticImageDataset(per, cfg.image_size, cfg.in_channels, cfg.num_classes,
-                                                 seed=cfg.seed + 17 * rank)
-            nval = cfg.val_steps * cfg.batch_size
-        self.n_train = per - nval                # n_k of sample-weighted FedAvg
-        self.label_counts = torch.bincount(self.dataset.labels[nval:per].long(),
-                                           minlength=int(getattr(self.dataset, "classes", cfg.num_classes))).tolist()
+            parts = dirichlet_partition(pool.labels, self.num_clients, cfg.dirichlet_alpha, cfg.seed, cfg.batch_size)
+        self.clients: List[Dict] = []
+        for i, cid in enumerate(self.client_ids):
+            if datasets is not None:
+                ds = datasets[i]
+                per = len(ds)
+                nval = int(per * 0.1)
+            elif pool is not None:
+                ds = pool.subset(parts[cid])
+                per = len(ds)
+                nval = int(per * 0.1)
+            else:
+                per = samples_per_client or (cfg.steps_per_epoch * cfg.batch_size + cfg.val_steps * cfg.batch_size)
+                ds = SyntheticImageDataset(per, cfg.image_size, cfg.in_channels, cfg.num_classes, seed=cfg.seed + 17 * cid)
+                nval = cfg.val_steps * cfg.batch_size
+            counts = torch.bincount(ds.labels[nval:per].long(),
+                                    minlength=int(getattr(ds, "classes", cfg.num_classes))).tolist()
+            self.clients.append({"id": cid, "dataset": ds, "nval": nval, "per": per, "n_train": per - nval,
+                                 "label_counts": counts})
+        del pool
+        c0 = self.clients[0]
+        self.dataset, self.n_train, self.label_counts = c0["dataset"], c0["n_train"], c0["label_counts"]   # n_k
+        per, nval = c0["per"], c0["nval"]
         self.train_feed = BatchFeeder(self.dataset, range(nval, per), cfg.batch_size, self.device,
-                                      shuffle=True, seed=cfg.seed + rank)
-        self.val_feed = BatchFeeder(self.dataset, range(0, nval), cfg.batch_size, self.device,
-                                    shuffle=True, seed=cfg.seed + rank) if nval else None
+                                      shuffle=True, seed=cfg.seed + c0["id"])
+        vc = next((c for c in self.clients if c["nval"]), None)
+        self.val_feed = BatchFeeder(vc["dataset"], range(0, vc["nval"]), cfg.batch_size, self.device,
+                                    shuffle=True, seed=cfg.seed + vc["id"]) if vc is not None else None
+        if self.multi:
+            # per-client state that persists across rounds, swapped into the trainer around each client's fit: Adam
+            # m / v, step and LR scale in [M, n] device tensors (the captured graphs keep the trainer's buffers),
+            # the engine's augmentation position, the feeders' shuffle generators and the torch RNG state
+            n = self.pack.n_trainable
+            tr = self.trainer
+            self._c_m = torch.zeros(M, n, dtype=torch.float32, device=self.device)
+            self._c_v = torch.zeros(M, n, dtype=torch.float32, device=self.device)
+            self._c_step = torch.zeros(M, 1, dtype=torch.int64, device=self.device)
+            self._c_lr = torch.ones(M, 1, dtype=torch.float32, device=self.device)
+            self._c_prep = [tr.engine.prep_count if tr.engine is not None else 0] * M
+            self._c_gen = [(torch.Generator().manual_seed(cfg.seed + c["id"]),
+                            torch.Generator().manual_seed(cfg.seed + c["id"])) for c in self.clients]
+            self._c_rng: Optional[List] = None          # filled at the first round, after the graphs are captured
+        self._selected: List[int] = list(range(self.num_clients))
+        self._enc_buf: Optional[torch.Tensor] = None   # the rank's ciphertext buffer while clients accumulate into it
+        self._plain_sum: Optional[torch.Tensor] = None
+        self._enc_count = 0                  # ciphertexts accumulated into the rank's buffer this round
+        self._last_client: Optional[int] = None
         self.round = 0
-        self.participating = True        # set False to sit a round out (needs cfg.allow_dropouts on every rank)
+        self.participating = True        # set False to sit a round out (needs cfg.allow_dropouts on every rank); with
+                                         # several clients per rank also a list of M flags, one per client
         self._active = None              # contributors of the current round when dropouts are allowed
         self._n_total = None             # N = sum of n_k over the round's contributors (sample-weighted FedAvg)
         self.timer = DeviceTimer(self.device)
@@ -148,11 +205,13 @@ class FederatedRunner:
         self.pk = pk
         self.sk = sk if self.has_sk else None
 
-    def _encrypt_seed(self) -> int:
+    def _encrypt_seed(self, client: Optional[int] = None) -> int:
         """Fresh randomness for every encryption call. Re-running a round (resume, retry) must never reuse
-        (u, e0, e1) on different weights, and a seed derived from public values lets anybody strip the mask."""
+        (u, e0, e1) on different weights, and a seed derived from public values lets anybody strip the mask.
+        ``client``: the id whose update is encrypted (the rank's id when it hosts one client)."""
         if self.cfg.deterministic_crypto:
-            return (self.cfg.seed * 1_000_003 + self.round * 1009 + self.rank) & 0x7FFFFFFFFFFFFFFF
+            cid = self.rank if client is None else client
+            return (self.cfg.seed * 1_000_003 + self.round * 1009 + cid) & 0x7FFFFFFFFFFFFFFF
         return secrets.randbits(63)
 
     def _agree_pair_seeds(self):
@@ -188,10 +247,91 @@ class FederatedRunner:
                                     self.ctx.logn, self.ctx.consts_cpu)
 
     # ------------------------------------------------------------------ stages
-    def local_train(self, early_stopping: Optional[int] = None):
-        with self.timer.stage("train"):
-            return self.trainer.fit(self.train_feed, self.val_feed, self.cfg.local_epochs,
-                                    early_stopping=early_stopping)
+    def local_train(self, early_stopping: Optional[int] = None, order: Optional[List[int]] = None):
+        """Train this rank's client(s) of the round from the current global model. With several clients per rank
+        (or client sampling) this trains the round's selected clients one after another -- ``order``: their local
+        slots, default ascending -- and encrypt-accumulates every update but the last into the rank's ciphertext
+        buffer; ``encrypt_update`` / ``fedavg_pipelined`` add the last. Returns the epoch history, or with several
+        clients a dict local slot -> history."""
+        if not self.multi:
+            with self.timer.stage("train"):
+                return self.trainer.fit(self.train_feed, self.val_feed, self.cfg.local_epochs,
+                                        early_stopping=early_stopping)
+        self._selected = select_clients(self.cfg, self.num_clients, self.round)
+        chosen = set(self._selected)
+        local = [i for i, cid in enumerate(self.client_ids) if cid in chosen]
+        order = local if order is None else [i for i in order if i in local]
+        self._agree_on_participants()
+        self.global_flat.copy_(self.pack.flat)
+        if self._c_rng is None:
+            # every client starts from the RNG state a one-client rank holds when its first step runs: after capture
+            self.trainer.prepare()
+            self._c_rng = [self._rng_state()] * self.clients_per_rank
+        self._enc_buf = self.transport.buffer(self.ct_numel)
+        self._enc_count = 0
+        weighted = self._n_total is not None
+        self._plain_sum = (torch.zeros(self.pack.numel, dtype=torch.float64, device=self.device)
+                           if self.cfg.debug_precision else None)
+        hists: Dict[int, list] = {}
+        for j, i in enumerate(order):
+            with self.timer.stage("train"):
+                if j:
+                    self.pack.load_flat(self.global_flat)
+                    if self.trainer.engine is not None:
+                        self.trainer.engine.after_restore()
+                val = self._swap_in(i)
+                hists[i] = self.trainer.fit(self.train_feed, val, self.cfg.local_epochs, early_stopping=early_stopping)
+                self._swap_out(i)
+            if self._plain_sum is not None and self._client_takes_part(i):
+                self._plain_sum.add_(self.pack.flat.double(), alpha=self.clients[i]["n_train"] if weighted else 1)
+            if j + 1 < len(order):
+                with self.timer.stage("encrypt"):
+                    self._accumulate(i, self._enc_buf)
+        self._last_client = order[-1] if order else None
+        return hists
+
+    # ------------------------------------------------------------------ per-client state
+    def _rng_state(self):
+        return (torch.get_rng_state(), torch.cuda.get_rng_state(self.device) if self.device.type == "cuda" else None)
+
+    def _set_rng_state(self, st) -> None:
+        torch.set_rng_state(st[0])
+        if st[1] is not None:
+            torch.cuda.set_rng_state(st[1], self.device)
+
+    def _swap_in(self, i: int) -> Optional[BatchFeeder]:
+        """Install client slot ``i``'s state in the trainer and point the feeders at its shard; returns its
+        validation feeder (None when it has no validation samples)."""
+        tr, c = self.trainer, self.clients[i]
+        tr.m.copy_(self._c_m[i]); tr.v.copy_(self._c_v[i]); tr.step_t.copy_(self._c_step[i]); tr.lr_scale.copy_(self._c_lr[i])
+        if tr.engine is not None:
+            tr.engine.prep_count = self._c_prep[i]
+        self._set_rng_state(self._c_rng[i])
+        self.train_feed.retarget(c["dataset"], range(c["nval"], c["per"]), self._c_gen[i][0])
+        if not c["nval"]:
+            return None
+        self.val_feed.retarget(c["dataset"], range(0, c["nval"]), self._c_gen[i][1])
+        return self.val_feed
+
+    def _swap_out(self, i: int) -> None:
+        tr = self.trainer
+        self._c_m[i].copy_(tr.m); self._c_v[i].copy_(tr.v); self._c_step[i].copy_(tr.step_t); self._c_lr[i].copy_(tr.lr_scale)
+        if tr.engine is not None:
+            self._c_prep[i] = tr.engine.prep_count
+        self._c_rng[i] = self._rng_state()
+
+    def _client_takes_part(self, i: int) -> bool:
+        p = self.participating
+        return bool(p[i] if isinstance(p, (list, tuple)) else p) or not self.cfg.allow_dropouts
+
+    def _accumulate(self, i: int, buf: torch.Tensor) -> None:
+        """Encrypt client slot ``i``'s trained model (in ``pack.flat``) with its own seed and FedAvg weight and add
+        it into ``buf`` mod q; the first ciphertext of the round overwrites the buffer."""
+        if not self._client_takes_part(i):
+            return
+        self.ctx.encrypt(self.pack.flat, self.pk, seed=self._encrypt_seed(self.client_ids[i]), packing=self.cfg.packing,
+                         out=buf, weight=self.fedavg_weight(i), accumulate=self._enc_count > 0)
+        self._enc_count += 1
 
     def _contributors(self) -> float:
         """K of this round: the world size, or — with ``allow_dropouts`` — the number of ranks that take part
@@ -203,10 +343,27 @@ class FederatedRunner:
 
     def _agree_on_participants(self) -> None:
         """One all-reduce of [participating, n_k] (float64): the participant count K when dropouts are allowed
-        and the round's total of training samples N for sample-weighted FedAvg."""
+        and the round's total of training samples N for sample-weighted FedAvg. With several clients per rank
+        each rank adds its selected clients that take part, and K is always the count of those over all ranks."""
         self._active = None
         self._n_total = None
         weighted = self.cfg.fedavg_weighting == "samples"
+        if self.multi:
+            chosen = set(self._selected)
+            mine = [i for i, cid in enumerate(self.client_ids) if cid in chosen and self._client_takes_part(i)]
+            t = [float(len(mine)), float(sum(self.clients[i]["n_train"] for i in mine))]
+            reduce = (self.cfg.allow_dropouts or weighted) and self.world > 1 \
+                and not isinstance(self.transport, LoopbackTransport)
+            if reduce:
+                tt = torch.tensor(t, dtype=torch.float64, device=self.device)
+                dist.all_reduce(tt, op=dist.ReduceOp.SUM, group=self.group)
+                t = tt.tolist()
+            if reduce or self.world == 1:
+                self._active = int(round(t[0]))
+                self._n_total = t[1] if weighted else None
+            else:                           # no collective needed: every rank knows the selection
+                self._active = len(self._selected)
+            return
         if not (self.cfg.allow_dropouts or weighted) or isinstance(self.transport, LoopbackTransport):
             return
         t = torch.tensor([1.0 if self._takes_part() else 0.0, float(self._my_samples())], dtype=torch.float64,
@@ -220,16 +377,16 @@ class FederatedRunner:
             self._n_total = t[1]
 
     def _takes_part(self) -> bool:
-        return self.participating or not self.cfg.allow_dropouts
+        return self._client_takes_part(0)
 
-    def _my_samples(self) -> int:
-        """n_k: this client's training samples, 0 when it sits the round out."""
-        return self.n_train if self._takes_part() else 0
+    def _my_samples(self, i: int = 0) -> int:
+        """n_k: client slot ``i``'s training samples, 0 when it sits the round out."""
+        return self.clients[i]["n_train"] if self._client_takes_part(i) else 0
 
-    def fedavg_weight(self) -> float:
-        """w_k = K·n_k / N, folded into the encode scale (1.0 for uniform FedAvg). Σ w_k = K, so the aggregate has
-        the magnitude bound of uniform FedAvg; equal shards give exactly 1.0."""
-        n = self._my_samples()
+    def fedavg_weight(self, i: int = 0) -> float:
+        """w_k = K·n_k / N of client slot ``i``, folded into the encode scale (1.0 for uniform FedAvg). Σ w_k = K, so
+        the aggregate has the magnitude bound of uniform FedAvg; equal shards give exactly 1.0."""
+        n = self._my_samples(i)
         if not self._n_total or n == 0:
             return 1.0
         return self._contributors() * n / self._n_total
@@ -238,11 +395,29 @@ class FederatedRunner:
         return self.pack.flat if self._takes_part() else torch.zeros_like(self.pack.flat)
 
     def encrypt_update(self) -> CtBatch:
+        if self.multi:
+            return self._encrypt_rank()
         self._agree_on_participants()
         with self.timer.stage("encrypt"):
             buf = self.transport.buffer(self.ct_numel)
             ct = self.ctx.encrypt(self._my_update(), self.pk, seed=self._encrypt_seed(), packing=self.cfg.packing,
                                   out=buf, weight=self.fedavg_weight())
+            self._mask(ct.data)
+            return ct
+
+    def _encrypt_rank(self) -> CtBatch:
+        """The rank's ciphertext of the round: the last trained client accumulated into the buffer its co-located
+        clients were encrypted into (an encryption of zeros when none of them takes part), masked once."""
+        with self.timer.stage("encrypt"):
+            buf = self._enc_buf if self._enc_buf is not None else self.transport.buffer(self.ct_numel)
+            if self._last_client is not None:
+                self._accumulate(self._last_client, buf)
+            if self._enc_count == 0:
+                self.ctx.encrypt(torch.zeros_like(self.pack.flat), self.pk, seed=self._encrypt_seed(self.num_clients + self.rank),
+                                 packing=self.cfg.packing, out=buf)
+            self._last_client, self._enc_buf = None, None
+            ct = CtBatch(buf[: self.ct_numel].view(self.n_ct, 2, self.ctx.L, self.ctx.n), self.ctx.scale,
+                         self.pack.numel, self.cfg.packing)
             self._mask(ct.data)
             return ct
 
@@ -283,14 +458,26 @@ class FederatedRunner:
         vpc = ctx.values_per_ct(self.cfg.packing)
         n_ct = self.n_ct
         per_ct = 2 * ctx.L * ctx.n
-        self._agree_on_participants()
-        flat = self._my_update()
-        out = torch.empty_like(flat)
+        acc, buf = False, None
+        if self.multi:
+            # the rank's other clients are already in the buffer; the last one is encrypted chunk by chunk into it
+            buf, last = self._enc_buf, self._last_client
+            self._last_client, self._enc_buf = None, None
+            flat = self.pack.flat if last is not None and self._client_takes_part(last) else None
+            if flat is not None:
+                weight, seed, acc = self.fedavg_weight(last), self._encrypt_seed(self.client_ids[last]), self._enc_count > 0
+            elif self._enc_count == 0:
+                flat = torch.zeros_like(self.pack.flat)
+                weight, seed = 1.0, self._encrypt_seed(self.num_clients + self.rank)
+        else:
+            self._agree_on_participants()
+            flat = self._my_update()
+            weight = self.fedavg_weight()
+            seed = self._encrypt_seed()
+        out = torch.empty_like(self.pack.flat)
         k = self._contributors()
         if k == 0:
             return
-        weight = self.fedavg_weight()
-        seed = self._encrypt_seed()
         if self.server_opt is not None:
             self.server_opt.ensure_state()               # on the current stream, before the three streams fork
         # the three streams live as long as the runner: the caching allocator keeps one pool per stream, so
@@ -301,7 +488,8 @@ class FederatedRunner:
         cur = torch.cuda.current_stream(dev)
         for st in (s_enc, s_comm, s_dec):
             st.wait_stream(cur)
-        buf = self.transport.buffer(self.ct_numel)
+        if buf is None:
+            buf = self.transport.buffer(self.ct_numel)
         # The three stages only overlap if they fit on the chip together: encrypt / decrypt are persistent
         # one-CTA-per-SM kernels and the all-reduce is a copy engine that saturates NVLink from a few SMs, so the
         # SMs are partitioned for the duration of the pipeline (HEFL_PIPE_SPLIT overrides the default split).
@@ -332,14 +520,17 @@ class FederatedRunner:
             chunks = [(c0, min(n_ct, c0 + chunk_cts)) for c0 in range(0, n_ct, chunk_cts)]
             t_origin = mark(cur) if timeline is not None else None
             for ci, (c0, c1) in enumerate(chunks):
-                vals = flat[c0 * vpc: min(flat.numel(), c1 * vpc)]
+                nv = min(self.pack.numel, c1 * vpc) - c0 * vpc
                 view = buf[c0 * per_ct: c1 * per_ct]
                 rec = {"chunk": ci}
                 with torch.cuda.stream(s_enc):
                     if timeline is not None:
                         rec["enc0"] = mark(s_enc)
-                    ct = ctx.encrypt(vals, self.pk, seed=seed, packing=self.cfg.packing, out=view, ct_offset=c0,
-                                     weight=weight)
+                    if flat is not None:
+                        ct = ctx.encrypt(flat[c0 * vpc: c0 * vpc + nv], self.pk, seed=seed, packing=self.cfg.packing,
+                                         out=view, ct_offset=c0, weight=weight, accumulate=acc)
+                    else:                        # every client of the rank is already in the buffer
+                        ct = CtBatch(view.view(c1 - c0, 2, ctx.L, ctx.n), ctx.scale, nv, self.cfg.packing)
                     self._mask(ct.data, chunk=ci)
                     ev_enc.append(mark(s_enc))
                 with torch.cuda.stream(s_comm):
@@ -394,14 +585,18 @@ class FederatedRunner:
         hist = self.local_train()
         plain_mean = None
         self._avg_out = None
-        if self.cfg.debug_precision and not isinstance(self.transport, LoopbackTransport):
+        if self.cfg.debug_precision and (not isinstance(self.transport, LoopbackTransport)
+                                         or (self.multi and self.world == 1)):
             # plaintext FedAvg oracle (SURVEY.md §5.5 "CKKS precision: max abs error vs plaintext FedAvg")
             # the oracle averages what the encrypted path averages: sitting-out clients contribute zeros and
             # K is the agreed participant count; with sample weighting it is sum(n_k x_k) / N
-            self._agree_on_participants()
-            plain_mean = self._my_update().detach().clone().double()
-            if self._n_total is not None:
-                plain_mean *= self._my_samples()
+            if self.multi:                   # the rank's clients' (weighted) updates, summed as local_train trained them
+                plain_mean = self._plain_sum
+            else:
+                self._agree_on_participants()
+                plain_mean = self._my_update().detach().clone().double()
+                if self._n_total is not None:
+                    plain_mean *= self._my_samples()
             if self.world > 1:
                 dist.all_reduce(plain_mean, op=dist.ReduceOp.SUM, group=self.group)
             kk = self._n_total if self._n_total is not None else self._contributors()
@@ -427,10 +622,13 @@ class FederatedRunner:
         if check:
             self.guard_finite()
         rec = {"round": self.round, "rank": self.rank, "stage_ms": times,
-               "loss": hist[-1].loss if hist else None, "accuracy": hist[-1].accuracy if hist else None,
+               "loss": hist[-1].loss if hist and not self.multi else None,
+               "accuracy": hist[-1].accuracy if hist and not self.multi else None,
                "transport": self.transport.name, "n_ct": self.n_ct, "ct_bytes": self.ct_numel * 8,
                "n_train": self.n_train, "fedavg_weight": self.fedavg_weight(), "label_counts": self.label_counts,
                "server_opt": self.cfg.server_opt}
+        if self.multi:
+            rec.update(self._client_records(hist))
         if plain_mean is not None:
             avg = self._avg_out if self._avg_out is not None else self.pack.flat
             err = float((avg.double() - plain_mean).abs().max())
@@ -439,6 +637,27 @@ class FederatedRunner:
         self.history.append(rec)
         self.round += 1
         return rec
+
+    def _client_records(self, hists: Dict[int, list]) -> Dict:
+        """Round-record fields of a rank with several clients: loss / accuracy as the sample-weighted mean over its
+        trained clients, n_train / fedavg_weight / label_counts summed over those that took part, and per client."""
+        clients, n_sum, w_sum = [], 0, 0.0
+        counts = [0] * len(self.label_counts)
+        for i in sorted(hists):
+            c, h = self.clients[i], hists[i]
+            w = self.fedavg_weight(i) if self._client_takes_part(i) else 0.0
+            clients.append({"id": c["id"], "n_train": c["n_train"], "fedavg_weight": w,
+                            "loss": h[-1].loss if h else None, "accuracy": h[-1].accuracy if h else None,
+                            "label_counts": c["label_counts"]})
+            if self._client_takes_part(i):
+                n_sum, w_sum = n_sum + c["n_train"], w_sum + w
+                counts = [a + b for a, b in zip(counts, c["label_counts"])]
+        scored = [(c["n_train"], c) for c in clients if c["loss"] is not None]
+        tot = sum(n for n, _ in scored)
+        return {"loss": sum(n * c["loss"] for n, c in scored) / tot if tot else None,
+                "accuracy": sum(n * c["accuracy"] for n, c in scored) / tot if tot else None,
+                "n_train": n_sum, "fedavg_weight": w_sum, "label_counts": counts,
+                "selected": list(self._selected), "clients": clients}
 
     POISON = 0x7FF8DEADBEEF7FF8          # > every q_l: a stale word can never pass for a residue
 
@@ -487,8 +706,40 @@ class FederatedRunner:
             torch.save({"round": self.round, "flat": self.pack.flat.detach().cpu(), "config": self.cfg.to_json()}, path)
         torch.save({"round": self.round, "opt": self.trainer.state_dict(), "rng": torch.get_rng_state(),
                     "cuda_rng": torch.cuda.get_rng_state(self.device) if self.device.type == "cuda" else None,
-                    "server": self.server_opt.state_dict() if self.server_opt is not None else None},
+                    "server": self.server_opt.state_dict() if self.server_opt is not None else None,
+                    "clients": self._clients_state() if self.multi else None},
                    f"{path}.rank{self.rank}")
+
+    def _clients_state(self) -> Dict:
+        """Every client's persistent state (several clients per rank): optimiser, augmentation position, shuffle
+        generators and RNG."""
+        rng = self._c_rng
+        return {"ids": torch.tensor(self.client_ids), "m": self._c_m.cpu(), "v": self._c_v.cpu(),
+                "step": self._c_step.cpu(), "lr_scale": self._c_lr.cpu(), "prep_count": torch.tensor(self._c_prep),
+                "gen": [[g.get_state() for g in pair] for pair in self._c_gen],
+                "rng": [r[0] for r in rng] if rng is not None else None,
+                "cuda_rng": [r[1] for r in rng] if rng is not None and rng[0][1] is not None else None}
+
+    def _load_clients_state(self, st: Optional[Dict]) -> None:
+        M = self.clients_per_rank
+        if st is None or st["ids"].tolist() != self.client_ids:          # no state of these clients: start fresh
+            self._c_m.zero_(); self._c_v.zero_(); self._c_step.zero_(); self._c_lr.fill_(1.0)
+            self._c_prep = [0] * M
+            self._c_gen = [(torch.Generator().manual_seed(self.cfg.seed + cid),
+                            torch.Generator().manual_seed(self.cfg.seed + cid)) for cid in self.client_ids]
+            self._c_rng = None
+            return
+        self._c_m.copy_(st["m"]); self._c_v.copy_(st["v"]); self._c_step.copy_(st["step"]); self._c_lr.copy_(st["lr_scale"])
+        self._c_prep = [int(x) for x in st["prep_count"]]
+        for pair, states in zip(self._c_gen, st["gen"]):
+            for g, gs in zip(pair, states):
+                g.set_state(gs)
+        if st["rng"] is None:
+            self._c_rng = None
+        else:
+            cuda = st["cuda_rng"] if self.device.type == "cuda" else None
+            self._c_rng = [(st["rng"][i], cuda[i] if cuda is not None else None) for i in range(M)]
+            self.trainer.prepare()         # the states were taken after capture: capture now, not inside a fit
 
     def load_checkpoint(self, path: str) -> None:
         ck = torch.load(path, map_location="cpu", weights_only=True)      # tensors and plain containers only
@@ -501,6 +752,8 @@ class FederatedRunner:
             torch.set_rng_state(st["rng"])
             if st.get("cuda_rng") is not None and self.device.type == "cuda":
                 torch.cuda.set_rng_state(st["cuda_rng"], self.device)
+            if self.multi:
+                self._load_clients_state(st.get("clients"))
             if self.server_opt is not None:          # the server state sits in the key holder's own file
                 if st.get("server") is not None:
                     self.server_opt.load_state_dict(st["server"])
@@ -508,6 +761,8 @@ class FederatedRunner:
                     self.server_opt.reset()
         else:                                       # no state of this rank (e.g. a different world size): start it fresh
             self.trainer.reset_optimizer()
+            if self.multi:
+                self._load_clients_state(None)
             if self.server_opt is not None:
                 self.server_opt.reset()
         if self.trainer.engine is not None:

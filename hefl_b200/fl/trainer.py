@@ -235,6 +235,12 @@ class LocalTrainer:
         torch.cuda.synchronize(self.device)
 
     # ------------------------------------------------------------------ public API
+    def prepare(self) -> None:
+        """Capture the CUDA graphs now rather than at the first step (a rank with several clients captures once,
+        before any client's state is installed). No-op without graphs or when they exist."""
+        if self.use_graph and (not self._graphs if self.engine is not None else self._graph_train is None):
+            self._capture()
+
     def train_step(self, x_u8: torch.Tensor, y: torch.Tensor) -> torch.Tensor:
         """One optimisation step on a uint8 NHWC batch. Returns a device tensor [loss, ncorrect]."""
         if self.use_graph:

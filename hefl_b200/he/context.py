@@ -206,10 +206,15 @@ class CKKSContext:
         raise ValueError(f"unknown packing {packing}")
 
     def encrypt(self, vals: torch.Tensor, pk: torch.Tensor, seed: int, packing: str = "slots",
-                out: Optional[torch.Tensor] = None, ct_offset: int = 0, weight: float = 1.0) -> CtBatch:
+                out: Optional[torch.Tensor] = None, ct_offset: int = 0, weight: float = 1.0,
+                accumulate: bool = False) -> CtBatch:
         """encode + public-key encrypt; ``out`` may be a view of a symmetric-memory buffer. ``weight`` multiplies
         the values inside the encode (scale Δ·weight) at no cost: the ciphertext carries weight·vals at scale Δ
-        (sample-weighted FedAvg). ``weight=1.0`` encodes exactly as without it."""
+        (sample-weighted FedAvg). ``weight=1.0`` encodes exactly as without it. ``accumulate=True`` adds the new
+        ciphertexts into ``out`` mod q (out = out + Enc(vals)) in the encryption's own store, so the clients of one
+        rank sum their updates without a buffer per client."""
+        if accumulate and out is None:
+            raise ValueError("accumulate=True adds into an existing ciphertext buffer: pass it as out=")
         nvals = vals.numel()
         msg = self.encode(vals, packing, scale=self.scale * float(weight))
         C = msg.shape[0]
@@ -219,7 +224,7 @@ class CKKSContext:
         else:
             data = out
             self.ops.encrypt_out(msg, pk, C, self.L, self.logn, self.tables, self.consts, None,
-                                 int(seed), int(ct_offset), data)
+                                 int(seed), int(ct_offset), data, bool(accumulate))
             data = data.view(-1)[: C * 2 * self.L * self.n].view(C, 2, self.L, self.n)
         return CtBatch(data, self.scale, nvals, packing)
 

@@ -110,7 +110,7 @@ def rounds(local_epochs, counts):
         torch.cuda.synchronize()
         row = {"clients_per_rank": M, "round_ms": (time.perf_counter() - t0) * 1e3,
                "stage_ms": rec["stage_ms"], "loss": rec["loss"]}
-        if run.multi:
+        if M > 1:
             def switch():
                 for i in range(M):
                     run.pack.load_flat(run.global_flat)

@@ -1,5 +1,5 @@
-"""Federated round loop: one client per rank (one process per GPU), or several (``clients_per_rank``, DESIGN.md §9),
-encrypted FedAvg.
+"""Federated round loop of encrypted FedAvg: M >= 1 clients per rank (``clients_per_rank``, one process per GPU,
+DESIGN.md §9); a one-client rank is the M = 1 case of the same round.
 
 One round = what the reference's notebook cell 3 does once (N:233-272):
 ``train_clients`` (FLPyfhelin.py:179-198) -> ``export_encrypted_clients_weights`` (:242) ->
@@ -109,7 +109,6 @@ class FederatedRunner:
         M = int(cfg.clients_per_rank)
         self.clients_per_rank, self.num_clients = M, world * M
         self.client_ids = list(range(rank * M, rank * M + M))
-        self.multi = M > 1 or cfg.client_fraction < 1      # the per-client round; M = 1, C = 1 is the 1-client rank
         datasets = list(dataset) if isinstance(dataset, (list, tuple)) else [dataset] if dataset is not None else None
         if datasets is not None and len(datasets) != M:
             raise ValueError(f"dataset: {len(datasets)} datasets for {M} clients per rank (one per client, in id order)")
@@ -150,29 +149,24 @@ class FederatedRunner:
         vc = next((c for c in self.clients if c["nval"]), None)
         self.val_feed = BatchFeeder(vc["dataset"], range(0, vc["nval"]), cfg.batch_size, self.device,
                                     shuffle=True, seed=cfg.seed + vc["id"]) if vc is not None else None
-        if self.multi:
+        if M > 1:
             # per-client state that persists across rounds, swapped into the trainer around each client's fit: Adam
             # m / v, step and LR scale in [M, n] device tensors (the captured graphs keep the trainer's buffers),
-            # the engine's augmentation position, the feeders' shuffle generators and the torch RNG state
+            # the engine's augmentation position, the feeders' shuffle generators and the torch RNG state. A
+            # one-client rank keeps its client's state where it lives: in the trainer, the feeders and the RNG.
             n = self.pack.n_trainable
-            tr = self.trainer
-            self._c_m = torch.zeros(M, n, dtype=torch.float32, device=self.device)
-            self._c_v = torch.zeros(M, n, dtype=torch.float32, device=self.device)
-            self._c_step = torch.zeros(M, 1, dtype=torch.int64, device=self.device)
-            self._c_lr = torch.ones(M, 1, dtype=torch.float32, device=self.device)
-            self._c_prep = [tr.engine.prep_count if tr.engine is not None else 0] * M
-            self._c_gen = [(torch.Generator().manual_seed(cfg.seed + c["id"]),
-                            torch.Generator().manual_seed(cfg.seed + c["id"])) for c in self.clients]
-            self._c_rng: Optional[List] = None          # filled at the first round, after the graphs are captured
+            self._c_m = torch.empty(M, n, dtype=torch.float32, device=self.device)
+            self._c_v = torch.empty(M, n, dtype=torch.float32, device=self.device)
+            self._c_step = torch.empty(M, 1, dtype=torch.int64, device=self.device)
+            self._c_lr = torch.empty(M, 1, dtype=torch.float32, device=self.device)
+            self._load_clients_state(None)              # every client starts fresh
         self._selected: List[int] = list(range(self.num_clients))
-        self._enc_buf: Optional[torch.Tensor] = None   # the rank's ciphertext buffer while clients accumulate into it
         self._plain_sum: Optional[torch.Tensor] = None
-        self._enc_count = 0                  # ciphertexts accumulated into the rank's buffer this round
-        self._last_client: Optional[int] = None
+        self._clear_pending()
         self.round = 0
         self.participating = True        # set False to sit a round out (needs cfg.allow_dropouts on every rank); with
                                          # several clients per rank also a list of M flags, one per client
-        self._active = None              # contributors of the current round when dropouts are allowed
+        self._active = None              # K: the round's contributing clients, once the ranks agreed on it
         self._n_total = None             # N = sum of n_k over the round's contributors (sample-weighted FedAvg)
         self.timer = DeviceTimer(self.device)
         self.log = JsonlLogger(cfg.log_jsonl, rank)
@@ -248,28 +242,24 @@ class FederatedRunner:
 
     # ------------------------------------------------------------------ stages
     def local_train(self, early_stopping: Optional[int] = None, order: Optional[List[int]] = None):
-        """Train this rank's client(s) of the round from the current global model. With several clients per rank
-        (or client sampling) this trains the round's selected clients one after another -- ``order``: their local
-        slots, default ascending -- and encrypt-accumulates every update but the last into the rank's ciphertext
-        buffer; ``encrypt_update`` / ``fedavg_pipelined`` add the last. Returns the epoch history, or with several
-        clients a dict local slot -> history."""
-        if not self.multi:
-            with self.timer.stage("train"):
-                return self.trainer.fit(self.train_feed, self.val_feed, self.cfg.local_epochs,
-                                        early_stopping=early_stopping)
+        """Train this rank's clients selected for the round, one after another from the current global model
+        (``order``: their local slots, default ascending). Every update but the last is encrypt-accumulated into the
+        rank's ciphertext buffer; the last stays installed in ``pack.flat`` for ``encrypt_update`` /
+        ``fedavg_pipelined`` to add. Returns a dict local slot -> epoch history."""
         self._selected = select_clients(self.cfg, self.num_clients, self.round)
         chosen = set(self._selected)
         local = [i for i, cid in enumerate(self.client_ids) if cid in chosen]
         order = local if order is None else [i for i in order if i in local]
-        self._agree_on_participants()
-        self.global_flat.copy_(self.pack.flat)
-        if self._c_rng is None:
-            # every client starts from the RNG state a one-client rank holds when its first step runs: after capture
-            self.trainer.prepare()
-            self._c_rng = [self._rng_state()] * self.clients_per_rank
+        swap = self.clients_per_rank > 1
+        if swap:
+            self.global_flat.copy_(self.pack.flat)
+            if self._c_rng is None:
+                # every client starts from the RNG state a one-client rank holds when its first step runs: after capture
+                self.trainer.prepare()
+                self._c_rng = [self._rng_state()] * self.clients_per_rank
+        self._clear_pending()
         self._enc_buf = self.transport.buffer(self.ct_numel)
-        self._enc_count = 0
-        weighted = self._n_total is not None
+        weighted = self.cfg.fedavg_weighting == "samples"
         self._plain_sum = (torch.zeros(self.pack.numel, dtype=torch.float64, device=self.device)
                            if self.cfg.debug_precision else None)
         hists: Dict[int, list] = {}
@@ -279,9 +269,10 @@ class FederatedRunner:
                     self.pack.load_flat(self.global_flat)
                     if self.trainer.engine is not None:
                         self.trainer.engine.after_restore()
-                val = self._swap_in(i)
+                val = self._swap_in(i) if swap else self.val_feed
                 hists[i] = self.trainer.fit(self.train_feed, val, self.cfg.local_epochs, early_stopping=early_stopping)
-                self._swap_out(i)
+                if swap:
+                    self._swap_out(i)
             if self._plain_sum is not None and self._client_takes_part(i):
                 self._plain_sum.add_(self.pack.flat.double(), alpha=self.clients[i]["n_train"] if weighted else 1)
             if j + 1 < len(order):
@@ -327,6 +318,7 @@ class FederatedRunner:
     def _accumulate(self, i: int, buf: torch.Tensor) -> None:
         """Encrypt client slot ``i``'s trained model (in ``pack.flat``) with its own seed and FedAvg weight and add
         it into ``buf`` mod q; the first ciphertext of the round overwrites the buffer."""
+        self._agree_on_participants()
         if not self._client_takes_part(i):
             return
         self.ctx.encrypt(self.pack.flat, self.pk, seed=self._encrypt_seed(self.client_ids[i]), packing=self.cfg.packing,
@@ -334,52 +326,38 @@ class FederatedRunner:
         self._enc_count += 1
 
     def _contributors(self) -> float:
-        """K of this round: the world size, or — with ``allow_dropouts`` — the number of ranks that take part
-        (participation mask, SURVEY.md §5.3). A client that sits out still joins the collective with an
-        encryption of zeros, so the fused kernel and its barriers are unchanged."""
+        """K of this round: the number of selected clients that take part (participation mask, SURVEY.md §5.3). A
+        rank none of whose clients takes part still joins the collective with an encryption of zeros, so the fused
+        kernel and its barriers are unchanged."""
         if self._active is not None:
             return float(self._active)
         return float(self.transport.contributors())
 
     def _agree_on_participants(self) -> None:
-        """One all-reduce of [participating, n_k] (float64): the participant count K when dropouts are allowed
-        and the round's total of training samples N for sample-weighted FedAvg. With several clients per rank
-        each rank adds its selected clients that take part, and K is always the count of those over all ranks."""
-        self._active = None
-        self._n_total = None
+        """K and N of the round, once, before its first encryption: each rank counts its selected clients that take
+        part and sums their n_k, and one all-reduce of [count, n_k sum] (float64) over the ranks gives K and the
+        total N for sample-weighted FedAvg. Without dropouts or sample weighting no collective runs (every rank knows
+        the selection, so K is its size), nor in an in-process loopback federation of several ranks."""
+        if self._agreed:
+            return
+        self._agreed = True
         weighted = self.cfg.fedavg_weighting == "samples"
-        if self.multi:
-            chosen = set(self._selected)
-            mine = [i for i, cid in enumerate(self.client_ids) if cid in chosen and self._client_takes_part(i)]
-            t = [float(len(mine)), float(sum(self.clients[i]["n_train"] for i in mine))]
-            reduce = (self.cfg.allow_dropouts or weighted) and self.world > 1 \
-                and not isinstance(self.transport, LoopbackTransport)
-            if reduce:
-                tt = torch.tensor(t, dtype=torch.float64, device=self.device)
-                dist.all_reduce(tt, op=dist.ReduceOp.SUM, group=self.group)
-                t = tt.tolist()
-            if reduce or self.world == 1:
-                self._active = int(round(t[0]))
-                self._n_total = t[1] if weighted else None
-            else:                           # no collective needed: every rank knows the selection
-                self._active = len(self._selected)
-            return
-        if not (self.cfg.allow_dropouts or weighted) or isinstance(self.transport, LoopbackTransport):
-            return
-        t = torch.tensor([1.0 if self._takes_part() else 0.0, float(self._my_samples())], dtype=torch.float64,
-                         device=self.device)
-        if self.world > 1:
-            dist.all_reduce(t, op=dist.ReduceOp.SUM, group=self.group)
-        t = t.tolist()
-        if self.cfg.allow_dropouts:
+        chosen = set(self._selected)
+        mine = [i for i, cid in enumerate(self.client_ids) if cid in chosen and self._client_takes_part(i)]
+        t = [float(len(mine)), float(sum(self.clients[i]["n_train"] for i in mine))]
+        reduce = (self.cfg.allow_dropouts or weighted) and self.world > 1 \
+            and not isinstance(self.transport, LoopbackTransport)
+        if reduce:
+            tt = torch.tensor(t, dtype=torch.float64, device=self.device)
+            dist.all_reduce(tt, op=dist.ReduceOp.SUM, group=self.group)
+            t = tt.tolist()
+        if reduce or self.world == 1:
             self._active = int(round(t[0]))
-        if weighted:
-            self._n_total = t[1]
+            self._n_total = t[1] if weighted else None
+        else:
+            self._active, self._n_total = len(self._selected), None
 
-    def _takes_part(self) -> bool:
-        return self._client_takes_part(0)
-
-    def _my_samples(self, i: int = 0) -> int:
+    def _my_samples(self, i: int) -> int:
         """n_k: client slot ``i``'s training samples, 0 when it sits the round out."""
         return self.clients[i]["n_train"] if self._client_takes_part(i) else 0
 
@@ -391,31 +369,36 @@ class FederatedRunner:
             return 1.0
         return self._contributors() * n / self._n_total
 
-    def _my_update(self) -> torch.Tensor:
-        return self.pack.flat if self._takes_part() else torch.zeros_like(self.pack.flat)
+    def _clear_pending(self) -> None:
+        """Start the rank's next ciphertext. A one-client rank's installed model is always its client's update, so it
+        stays pending (a caller may load weights and encrypt without ``local_train``); with several clients
+        ``local_train`` names the slot whose model is installed."""
+        self._enc_buf, self._enc_count, self._agreed = None, 0, False
+        self._last_client = 0 if self.clients_per_rank == 1 else None
+
+    def _rank_update(self):
+        """Agree on K and N if this round has not yet, and return what completes the rank's ciphertext: (buffer,
+        values, weight, seed, accumulate). The values are the installed model of the last trained client, zeros
+        under the rank's own seed when none of its clients takes part, or None when the buffer already holds every
+        contribution."""
+        self._agree_on_participants()
+        buf = self._enc_buf if self._enc_buf is not None else self.transport.buffer(self.ct_numel)
+        last, acc = self._last_client, self._enc_count > 0
+        self._clear_pending()
+        if last is not None and self._client_takes_part(last):
+            return buf, self.pack.flat, self.fedavg_weight(last), self._encrypt_seed(self.client_ids[last]), acc
+        if acc:
+            return buf, None, 1.0, 0, True
+        return buf, torch.zeros_like(self.pack.flat), 1.0, self._encrypt_seed(self.num_clients + self.rank), False
 
     def encrypt_update(self) -> CtBatch:
-        if self.multi:
-            return self._encrypt_rank()
-        self._agree_on_participants()
+        """The rank's ciphertext of the round: the last trained client added into the buffer its co-located clients
+        were accumulated into (an encryption of zeros when none of them takes part), masked once."""
+        buf, flat, weight, seed, acc = self._rank_update()
         with self.timer.stage("encrypt"):
-            buf = self.transport.buffer(self.ct_numel)
-            ct = self.ctx.encrypt(self._my_update(), self.pk, seed=self._encrypt_seed(), packing=self.cfg.packing,
-                                  out=buf, weight=self.fedavg_weight())
-            self._mask(ct.data)
-            return ct
-
-    def _encrypt_rank(self) -> CtBatch:
-        """The rank's ciphertext of the round: the last trained client accumulated into the buffer its co-located
-        clients were encrypted into (an encryption of zeros when none of them takes part), masked once."""
-        with self.timer.stage("encrypt"):
-            buf = self._enc_buf if self._enc_buf is not None else self.transport.buffer(self.ct_numel)
-            if self._last_client is not None:
-                self._accumulate(self._last_client, buf)
-            if self._enc_count == 0:
-                self.ctx.encrypt(torch.zeros_like(self.pack.flat), self.pk, seed=self._encrypt_seed(self.num_clients + self.rank),
-                                 packing=self.cfg.packing, out=buf)
-            self._last_client, self._enc_buf = None, None
+            if flat is not None:
+                self.ctx.encrypt(flat, self.pk, seed=seed, packing=self.cfg.packing, out=buf, weight=weight,
+                                 accumulate=acc)
             ct = CtBatch(buf[: self.ct_numel].view(self.n_ct, 2, self.ctx.L, self.ctx.n), self.ctx.scale,
                          self.pack.numel, self.cfg.packing)
             self._mask(ct.data)
@@ -458,22 +441,8 @@ class FederatedRunner:
         vpc = ctx.values_per_ct(self.cfg.packing)
         n_ct = self.n_ct
         per_ct = 2 * ctx.L * ctx.n
-        acc, buf = False, None
-        if self.multi:
-            # the rank's other clients are already in the buffer; the last one is encrypted chunk by chunk into it
-            buf, last = self._enc_buf, self._last_client
-            self._last_client, self._enc_buf = None, None
-            flat = self.pack.flat if last is not None and self._client_takes_part(last) else None
-            if flat is not None:
-                weight, seed, acc = self.fedavg_weight(last), self._encrypt_seed(self.client_ids[last]), self._enc_count > 0
-            elif self._enc_count == 0:
-                flat = torch.zeros_like(self.pack.flat)
-                weight, seed = 1.0, self._encrypt_seed(self.num_clients + self.rank)
-        else:
-            self._agree_on_participants()
-            flat = self._my_update()
-            weight = self.fedavg_weight()
-            seed = self._encrypt_seed()
+        # the rank's other clients are already in the buffer; the last one is encrypted chunk by chunk into it
+        buf, flat, weight, seed, acc = self._rank_update()
         out = torch.empty_like(self.pack.flat)
         k = self._contributors()
         if k == 0:
@@ -488,8 +457,6 @@ class FederatedRunner:
         cur = torch.cuda.current_stream(dev)
         for st in (s_enc, s_comm, s_dec):
             st.wait_stream(cur)
-        if buf is None:
-            buf = self.transport.buffer(self.ct_numel)
         # The three stages only overlap if they fit on the chip together: encrypt / decrypt are persistent
         # one-CTA-per-SM kernels and the all-reduce is a copy engine that saturates NVLink from a few SMs, so the
         # SMs are partitioned for the duration of the pipeline (HEFL_PIPE_SPLIT overrides the default split).
@@ -582,28 +549,13 @@ class FederatedRunner:
     # ------------------------------------------------------------------ round
     def run_round(self, check: bool = False, pipelined: Optional[bool] = None) -> Dict:
         self.global_flat.copy_(self.pack.flat)       # x_t of the server step
-        hist = self.local_train()
-        plain_mean = None
-        self._avg_out = None
-        if self.cfg.debug_precision and (not isinstance(self.transport, LoopbackTransport)
-                                         or (self.multi and self.world == 1)):
-            # plaintext FedAvg oracle (SURVEY.md §5.5 "CKKS precision: max abs error vs plaintext FedAvg")
-            # the oracle averages what the encrypted path averages: sitting-out clients contribute zeros and
-            # K is the agreed participant count; with sample weighting it is sum(n_k x_k) / N
-            if self.multi:                   # the rank's clients' (weighted) updates, summed as local_train trained them
-                plain_mean = self._plain_sum
-            else:
-                self._agree_on_participants()
-                plain_mean = self._my_update().detach().clone().double()
-                if self._n_total is not None:
-                    plain_mean *= self._my_samples()
-            if self.world > 1:
-                dist.all_reduce(plain_mean, op=dist.ReduceOp.SUM, group=self.group)
-            kk = self._n_total if self._n_total is not None else self._contributors()
-            plain_mean = plain_mean / kk if kk > 0 else None
-            if plain_mean is not None and self.cfg.server_opt != "fedavg":
-                # the error is the decoded average's, not the stepped model's: the decode also writes it here
-                self._avg_out = torch.empty_like(self.pack.flat)
+        hists = self.local_train()
+        # plaintext FedAvg oracle (SURVEY.md §5.5 "CKKS precision: max abs error vs plaintext FedAvg"): the ranks'
+        # sums of their clients' (n_k-weighted) updates as local_train trained them, over the agreed K or N. An
+        # in-process loopback federation of several ranks has no process group to sum them over.
+        oracle = self.cfg.debug_precision and (self.world == 1 or not isinstance(self.transport, LoopbackTransport))
+        # with a server step the error is the decoded average's, not the stepped model's: the decode also writes it here
+        self._avg_out = torch.empty_like(self.pack.flat) if oracle and self.cfg.server_opt != "fedavg" else None
         if pipelined is None:
             pipelined = self.device.type == "cuda" and self.n_ct > 512 and self.transport.name in ("fused", "nccl", "gloo")
         if pipelined:
@@ -621,26 +573,31 @@ class FederatedRunner:
             self.transport.check_status()
         if check:
             self.guard_finite()
+        hist = hists.get(0)
         rec = {"round": self.round, "rank": self.rank, "stage_ms": times,
-               "loss": hist[-1].loss if hist and not self.multi else None,
-               "accuracy": hist[-1].accuracy if hist and not self.multi else None,
+               "loss": hist[-1].loss if hist else None, "accuracy": hist[-1].accuracy if hist else None,
                "transport": self.transport.name, "n_ct": self.n_ct, "ct_bytes": self.ct_numel * 8,
                "n_train": self.n_train, "fedavg_weight": self.fedavg_weight(), "label_counts": self.label_counts,
                "server_opt": self.cfg.server_opt}
-        if self.multi:
-            rec.update(self._client_records(hist))
-        if plain_mean is not None:
-            avg = self._avg_out if self._avg_out is not None else self.pack.flat
-            err = float((avg.double() - plain_mean).abs().max())
-            rec["ckks_max_abs_err"] = err
-            rec["ckks_precision_bits"] = float(-math.log2(err)) if err > 0 else float("inf")
+        if self.clients_per_rank > 1 or self.cfg.client_fraction < 1:
+            rec.update(self._client_records(hists))
+        if oracle:
+            if self.world > 1:
+                dist.all_reduce(self._plain_sum, op=dist.ReduceOp.SUM, group=self.group)
+            kk = self._n_total if self._n_total is not None else self._contributors()
+            if kk > 0:
+                avg = self._avg_out if self._avg_out is not None else self.pack.flat
+                err = float((avg.double() - self._plain_sum / kk).abs().max())
+                rec["ckks_max_abs_err"] = err
+                rec["ckks_precision_bits"] = float(-math.log2(err)) if err > 0 else float("inf")
         self.history.append(rec)
         self.round += 1
         return rec
 
     def _client_records(self, hists: Dict[int, list]) -> Dict:
-        """Round-record fields of a rank with several clients: loss / accuracy as the sample-weighted mean over its
-        trained clients, n_train / fedavg_weight / label_counts summed over those that took part, and per client."""
+        """Round-record fields of a rank with several clients or client sampling: loss / accuracy as the sample-weighted
+        mean over its trained clients, n_train / fedavg_weight / label_counts summed over those that took part, the
+        round's selection, and per client."""
         clients, n_sum, w_sum = [], 0, 0.0
         counts = [0] * len(self.label_counts)
         for i in sorted(hists):
@@ -700,14 +657,16 @@ class FederatedRunner:
 
     # ------------------------------------------------------------------ checkpoint / resume
     def save_checkpoint(self, path: str) -> None:
-        """Round index + global model (rank 0 -> ``path``) and, PER RANK, optimiser moments, LR state and RNG
-        (``path.rank{r}``) so that a resumed multi-round run equals an uninterrupted one (SURVEY.md §5.4)."""
+        """Round index + global model (rank 0 -> ``path``) and, PER RANK, optimiser moments, LR state, RNG, the
+        feeders' shuffle generators and, with several clients per rank, every client's state (``path.rank{r}``) so
+        that a resumed multi-round run equals an uninterrupted one (SURVEY.md §5.4)."""
         if self.rank == 0:
             torch.save({"round": self.round, "flat": self.pack.flat.detach().cpu(), "config": self.cfg.to_json()}, path)
         torch.save({"round": self.round, "opt": self.trainer.state_dict(), "rng": torch.get_rng_state(),
                     "cuda_rng": torch.cuda.get_rng_state(self.device) if self.device.type == "cuda" else None,
+                    "feeds": [f.gen.get_state() if f is not None else None for f in (self.train_feed, self.val_feed)],
                     "server": self.server_opt.state_dict() if self.server_opt is not None else None,
-                    "clients": self._clients_state() if self.multi else None},
+                    "clients": self._clients_state() if self.clients_per_rank > 1 else None},
                    f"{path}.rank{self.rank}")
 
     def _clients_state(self) -> Dict:
@@ -749,10 +708,15 @@ class FederatedRunner:
         if os.path.exists(mine):
             st = torch.load(mine, map_location="cpu", weights_only=True)
             self.trainer.load_state_dict(st["opt"])
+            if int(st["opt"]["step"]) > 0:
+                self.trainer.prepare()     # the RNG state was taken after capture: capture now, not inside a fit
             torch.set_rng_state(st["rng"])
             if st.get("cuda_rng") is not None and self.device.type == "cuda":
                 torch.cuda.set_rng_state(st["cuda_rng"], self.device)
-            if self.multi:
+            for f, gs in zip((self.train_feed, self.val_feed), st.get("feeds") or ()):
+                if f is not None and gs is not None:
+                    f.gen.set_state(gs)
+            if self.clients_per_rank > 1:
                 self._load_clients_state(st.get("clients"))
             if self.server_opt is not None:          # the server state sits in the key holder's own file
                 if st.get("server") is not None:
@@ -761,7 +725,7 @@ class FederatedRunner:
                     self.server_opt.reset()
         else:                                       # no state of this rank (e.g. a different world size): start it fresh
             self.trainer.reset_optimizer()
-            if self.multi:
+            if self.clients_per_rank > 1:
                 self._load_clients_state(None)
             if self.server_opt is not None:
                 self.server_opt.reset()

@@ -1,22 +1,26 @@
 """Which CUDA kernels a piece of work launched, as torch.profiler reports them (shared by the GPU test modules)."""
 import re
+import time
 import warnings
 
 import torch
 
 
-def kernels_run(fn, attempts=3):
+def kernels_run(fn, attempts=5):
     """Runs fn() under torch.profiler and returns (its result, the names of the CUDA kernels it launched).
 
     Now and then the profiler hands back a trace with no device activity at all although fn launched native
     kernels (the launch counter moved). Such a trace says nothing about which kernel ran, so fn, which must be
-    repeatable, runs again under a fresh profiler, up to `attempts` times. A trace with any kernel in it is final."""
+    repeatable, runs again under a fresh profiler, up to `attempts` times. Empty traces can come several in a row and
+    then stop, so each retry waits a little longer before it starts. A trace with any kernel in it is final."""
     from torch.profiler import ProfilerActivity, profile
 
     from hefl_b200 import _ext
 
     ops = _ext.ops()
-    for _ in range(attempts):
+    for attempt in range(attempts):
+        if attempt:
+            time.sleep(0.25 * attempt)
         torch.cuda.synchronize()
         launches = int(ops.launch_count())
         with profile(activities=[ProfilerActivity.CPU, ProfilerActivity.CUDA]) as prof:

@@ -162,15 +162,31 @@ def test_round_record_is_the_sample_weighted_mean_of_the_clients():
     assert rec["label_counts"] == [sum(c["label_counts"][k] for c in cl) for k in range(10)]
 
 
-def test_debug_precision_oracle_sums_the_clients():
-    run = FederatedRunner(_cfg(clients_per_rank=3, debug_precision=True, fedavg_weighting="samples",
+def _debug_precision_error(per_rank):
+    run = FederatedRunner(_cfg(clients_per_rank=per_rank, debug_precision=True, fedavg_weighting="samples",
                                dirichlet_alpha=0.5), device=CPU)
-    rec = run.run_round(check=True)
-    assert rec["ckks_max_abs_err"] < 1e-6
+    return run.run_round(check=True)["ckks_max_abs_err"]
 
 
-def test_resumed_run_equals_uninterrupted_run(tmp_path):
-    kw = dict(clients_per_rank=3, client_fraction=0.67)
+def test_debug_precision_oracle_sums_the_clients():
+    assert _debug_precision_error(3) < 1e-6
+
+
+def test_debug_precision_oracle_of_a_single_one_client_process():
+    assert _debug_precision_error(1) < 1e-6
+
+
+def test_one_client_rank_encrypts_its_installed_model_without_training():
+    run = FederatedRunner(_cfg(), device=CPU)
+    run.run_round(check=True)
+    ct = run.encrypt_update()
+    assert float((run.ctx.decrypt(ct, run.sk) - run.pack.flat).abs().max()) < 1e-6
+
+
+def _resume_at_round_2(tmp_path, per_rank, fraction):
+    """The uninterrupted runner after three rounds and one saved after two, resumed and run for the third; their
+    global models must be equal."""
+    kw = dict(clients_per_rank=per_rank, client_fraction=fraction)
     a = FederatedRunner(_cfg(**kw), device=CPU)
     for _ in range(3):
         a.run_round(check=True)
@@ -184,7 +200,17 @@ def test_resumed_run_equals_uninterrupted_run(tmp_path):
     assert c.round == 2
     c.run_round(check=True)
     assert torch.equal(a.pack.flat, c.pack.flat)
+    return a, c
+
+
+def test_resumed_run_equals_uninterrupted_run(tmp_path):
+    a, c = _resume_at_round_2(tmp_path, 3, 0.67)
     assert torch.equal(a._c_m, c._c_m) and torch.equal(a._c_step, c._c_step)
+
+
+def test_resumed_one_client_run_with_sampling_equals_uninterrupted_run(tmp_path):
+    a, c = _resume_at_round_2(tmp_path, 1, 0.5)
+    assert torch.equal(a.trainer.m, c.trainer.m) and torch.equal(a.trainer.step_t, c.trainer.step_t)
 
 
 def test_dataset_list_must_have_one_dataset_per_client():

@@ -206,7 +206,7 @@ def test_simulated_server_step_matches_its_float64_oracle(name, lr):
 def _runner(**kw):
     cfg = _cfg(clients=1, transport="gloo", deterministic_crypto=True, server_opt="fedadam", server_lr=0.1, **kw)
     r = FederatedRunner(cfg, device=torch.device("cpu"))
-    # the data order is not part of the checkpoint: fixed here, so that only the server state can differ
+    # the data order is fixed here, so that only the server state can differ
     r.train_feed.shuffle = False
     if r.val_feed is not None:
         r.val_feed.shuffle = False

@@ -516,9 +516,9 @@ void conv_dgrad(const void* dY, const void* Wd, void* dX, int B, int H, int W, i
 // With e = dx + s, column 2j+e is pair-row j + (e >> 1), half e & 1: a row shift of the A descriptor plus a
 // K byte offset of (e & 1) * CK * 2 inside the pair-row — both are things G1 already does (row-shifted starts,
 // 32-byte K steps inside a swizzle atom). Four accumulators (2 rows x 2 column parities), M = 128 windows.
-// The epilogue thread of window j then holds all four values of its window: max/arg-max in registers, no
-// shuffles, every lane stores a full 16-byte pooled pixel chunk. Restricted to CK <= 32 (one swizzle atom per
-// pair-row) and CO <= 64 (4 accumulators in registers).
+// The four accumulators share one fragment layout, so max/arg-max are element-wise on the fragments (no shuffles, no
+// transpose); the pooled row is staged in shared memory and leaves the CTA as two TMA stores (values, codes).
+// Restricted to CK <= 32 (one swizzle atom per pair-row) and CO <= 64 (4 accumulators in registers).
 // ------------------------------------------------------------------------------------------
 template <int CK, int CO, int NSEG_ = 4, int SEG_BYTES_ = 136 * 2 * CK * 2, int NBUF_ = 2>
 struct PairFwdCfg {
@@ -531,21 +531,30 @@ struct PairFwdCfg {
   static constexpr int W_TAP = CO * W_ROW;
   static constexpr int W_BYTES = 9 * W_TAP;
   static constexpr int BAR_BYTES = 384;
-  static constexpr int SCR_BYTES = 8 * 1024;
+  // pooled output tile of one pooled row, staged for the TMA store: [128 windows][CO] bf16, then [128][CO] codes,
+  // each laid out as its tensor map's swizzle (span = one row) so the fragment writes are free of bank conflicts;
+  // two of them, so one is filled while the store of the other still reads it
+  static constexpr int OUT_V = 128 * CO * 2;
+  static constexpr int OUT_BYTES = OUT_V + 128 * CO;
   static constexpr int NBUF = NBUF_;
-  static constexpr int SMEM = W_BYTES + NBUF * HALO + SCR_BYTES + BAR_BYTES + 1024;
+  static constexpr int SMEM = W_BYTES + NBUF * HALO + 2 * OUT_BYTES + BAR_BYTES + 1024;
   static constexpr int NACC = 4;
   static constexpr int NG = 2;                            // 8-channel chunks per warp and pass
   static constexpr int OCC = blocks_fit(SMEM, 2) ? 2 : 1;
   static_assert(CK == 16 || CK == 32, "pair-row forward: one swizzle atom per pair-row");
   static_assert(CO == 32 || CO == 64, "pair-row forward: CO is 32 or 64");
   static_assert(SMEM <= kSmemMax, "shared memory");
+  static_assert((W_BYTES + NBUF * HALO) % 1024 == 0 && OUT_V % 1024 == 0 && OUT_BYTES % 1024 == 0,
+                "output tiles start on the 1024-byte swizzle repeat");
 };
 
 struct PairFwdArgs {
   int B, H, W;          // input grid (W even)
   int Hp, Wp;           // pooled grid
   int num_tiles;        // B * Hp (one pooled row per tile; Wp <= 128)
+#ifdef HEFL_CONV_DEBUG
+  int dbg;              // as TapGemmArgs::dbg: 1 = skip TMA data, 2 = skip MMAs, 4 = skip epilogue
+#endif
   const float* bias;
   __nv_bfloat16* out;   // [B,Hp,Wp,CO]
   uint8_t* argmax;      // may be null
@@ -566,7 +575,7 @@ struct PairFwdArgs {
 //                swizzle); the column parity dx is in the weights ([3 r][2 dx][CO][16], slot s + dx = tap s), so one
 //                A fragment feeds both dx accumulators. Same MMAs as kPairS, a third of its A loads, a quarter of its
 //                halo bytes.
-// Warp roles as in G1: warps 0..7 compute + epilogue (lane = window, quadrant = warp % 4, chunks by warp / 4),
+// Warp roles as in G1: warps 0..7 compute + epilogue (windows 32 * (warp % 4) .., chunks by warp / 4),
 // warp 8 is the TMA producer.
 constexpr int kPairPlain = 0, kPairS = 1, kPairRS = 2, kPairC = 3;
 // compact segment: one image row of <= 256 pixels x 8 B, plus zeroed slack for the 16 bytes window 127 reads past it
@@ -578,7 +587,8 @@ using PairCfgOf = PairFwdCfg<CK, CO, PK == kPairRS ? 2 : 4, PK == kPairC ? kPair
                              PK == kPairC ? kPairCBuf : 2>;
 
 template <int CK, int CO, int PK>
-__device__ __forceinline__ void pair_fwd_body(const CUtensorMap* tmA, const CUtensorMap& tmW, const PairFwdArgs& a,
+__device__ __forceinline__ void pair_fwd_body(const CUtensorMap* tmA, const CUtensorMap& tmW, const CUtensorMap& tmO,
+                                              const CUtensorMap& tmC, const PairFwdArgs& a,
                                               const __nv_bfloat16* __restrict__ xc = nullptr) {
   using Cfg = PairCfgOf<CK, CO, PK>;
   constexpr bool SP = PK == kPairS;
@@ -588,11 +598,13 @@ __device__ __forceinline__ void pair_fwd_body(const CUtensorMap* tmA, const CUte
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* sW = smem;
   uint8_t* sA = smem + Cfg::W_BYTES;
-  float* scr_all = reinterpret_cast<float*>(sA + Cfg::NBUF * Cfg::HALO);
-  uint64_t* bars = reinterpret_cast<uint64_t*>(reinterpret_cast<uint8_t*>(scr_all) + Cfg::SCR_BYTES);
+  uint8_t* sOut = sA + Cfg::NBUF * Cfg::HALO;           // [2][OUT_BYTES]
+  uint64_t* bars = reinterpret_cast<uint64_t*>(sOut + 2 * Cfg::OUT_BYTES);
   uint64_t* full = bars;
   uint64_t* empty = bars + Cfg::NBUF;
   uint64_t* wfull = bars + 2 * Cfg::NBUF;
+  float* sBias = reinterpret_cast<float*>(bars + 16);      // [CO], in the barrier block
+  static_assert(16 * 8 + CO * 4 <= Cfg::BAR_BYTES, "bias slot");
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
 
@@ -605,6 +617,8 @@ __device__ __forceinline__ void pair_fwd_body(const CUtensorMap* tmA, const CUte
   if (warp == 8 && lane == 0) {
     if constexpr (PK != kPairC) prefetch_tmap(tmA);
     prefetch_tmap(&tmW);
+    prefetch_tmap(&tmO);
+    if (a.argmax) prefetch_tmap(&tmC);
     for (int s = 0; s < Cfg::NBUF; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 8); }
     mbar_init(wfull, 1);
     fence_barrier_init();
@@ -629,6 +643,11 @@ __device__ __forceinline__ void pair_fwd_body(const CUtensorMap* tmA, const CUte
         const int q0 = (b * a.H + 2 * hp) * half_w;          // first pair-row of image row 2hp
         mbar_wait(&empty[buf], phase ^ 1);
         uint8_t* dst = sA + buf * Cfg::HALO;
+#ifdef HEFL_CONV_DEBUG
+        if (a.dbg & 1) {
+          mbar_arrive(&full[buf]);
+        } else
+#endif
         if constexpr (PK == kPairC) {
           const uint32_t row_bytes = (uint32_t)a.W * 8u;
           mbar_expect_tx(&full[buf], Cfg::NSEG * row_bytes);
@@ -645,16 +664,19 @@ __device__ __forceinline__ void pair_fwd_body(const CUtensorMap* tmA, const CUte
     // ===== compute + epilogue warps 0..7; accumulator (dy, dx) = acc[dy * 2 + dx] =====
     const int qd = warp & 3;
     const int grp = warp >> 2;
-    const int j = qd * 32 + lane;                          // window index in the pooled row
-    float* scr = scr_all + warp * 256;
     const uint32_t w_base = smem_u32(sW);
+    // the bias (written by the previous kernel, so read after pdl_wait) from shared memory: a per-chunk global
+    // address would stay live across the MMAs
+    if (threadIdx.x < CO) sBias[threadIdx.x] = a.bias[threadIdx.x];
+    named_barrier_sync(1, 256);
     mbar_wait(wfull, 0);
-    int buf = 0;
+    int buf = 0, ob = 0;
     uint32_t phase = 0;
     for (int t = blockIdx.x; t < a.num_tiles; t += gridDim.x) {
       mbar_wait(&full[buf], phase);
       const uint32_t a_base = smem_u32(sA + buf * Cfg::HALO);
-      const size_t row_out = (size_t)t * a.Wp;             // t = b * Hp + hp
+      const uint32_t sv = smem_u32(sOut + ob * Cfg::OUT_BYTES);   // [128 windows][CO] bf16, swizzle span CO * 2 B
+      const uint32_t sc = sv + Cfg::OUT_V;                         // [128 windows][CO] codes, swizzle span CO B
 #pragma unroll 1
       for (int g = 0; g < CO / 16 / Cfg::NG; ++g) {
         const int c0 = grp + 2 * g * Cfg::NG;              // chunks c0 and c0 + 2
@@ -667,6 +689,9 @@ __device__ __forceinline__ void pair_fwd_body(const CUtensorMap* tmA, const CUte
             for (int mt = 0; mt < 2; ++mt)
 #pragma unroll
               for (int q = 0; q < 4; ++q) acc[x][i][mt][q] = 0.f;
+#ifdef HEFL_CONV_DEBUG
+        if (!(a.dbg & 2))
+#endif
         if constexpr (PK == kPairRS) {
           uint32_t bf[4];
           ld_b_kmajor<WB>(w_base, c0 * 8, (c0 + 2) * 8, 0, lane, bf);
@@ -753,66 +778,106 @@ __device__ __forceinline__ void pair_fwd_body(const CUtensorMap* tmA, const CUte
           __syncwarp();
           if (lane == 0) mbar_arrive(&empty[buf]);
         }
+        // Pool on the fragments: the four accumulators of a window share one fragment layout (element q of m16 tile
+        // mt is window qd*32 + mt*16 + (q >> 1)*8 + lane/4, channel ch*8 + (lane%4)*2 + (q & 1)), so the 2x2 max
+        // and its arg-max are element-wise; only the pooled value (bf16 pair) and code (byte pair) reach the
+        // staged output tile. The windows of a fragment row are 8k + lane / 4, and 8 rows span one swizzle repeat of
+        // either tile, so the swizzle (address bits 7.. XORed into the 16-byte chunk bits 4..6) is a per-lane constant.
+        const uint32_t vx = swz<CO * 2>((lane >> 2) * CO * 2) ^ ((lane >> 2) * CO * 2);
+        const uint32_t cx = swz<CO>((lane >> 2) * CO) ^ ((lane >> 2) * CO);
 #pragma unroll
         for (int i = 0; i < 2; ++i) {
-          const int ch = c0 + 2 * i;
-          float v00[8], v01[8], v10[8], v11[8];
-          frag_rows(scr, acc[0][i][0], acc[0][i][1], lane, v00);
-          frag_rows(scr, acc[1][i][0], acc[1][i][1], lane, v01);
-          frag_rows(scr, acc[2][i][0], acc[2][i][1], lane, v10);
-          frag_rows(scr, acc[3][i][0], acc[3][i][1], lane, v11);
-          const float4 bA = __ldg(reinterpret_cast<const float4*>(a.bias + ch * 8));
-          const float4 bB = __ldg(reinterpret_cast<const float4*>(a.bias + ch * 8 + 4));
-          const float bias8[8] = {bA.x, bA.y, bA.z, bA.w, bB.x, bB.y, bB.z, bB.w};
-          uint32_t packed[4], idx[2] = {0u, 0u};
+          const int col = (c0 + 2 * i) * 8 + (lane & 3) * 2;   // this lane's first channel
+#ifdef HEFL_CONV_DEBUG
+          if (a.dbg & 4) continue;
+#endif
+          const float2 bb = *reinterpret_cast<const float2*>(sBias + col);
 #pragma unroll
-          for (int c = 0; c < 8; c += 2) {
-            float x[2];
+          for (int mt = 0; mt < 2; ++mt)
 #pragma unroll
-            for (int h = 0; h < 2; ++h) {
-              // same tie-breaking as G1: lower row wins only if strictly greater, then right column likewise
-              const bool l0 = v10[c + h] > v00[c + h];
-              const bool l1 = v11[c + h] > v01[c + h];
-              const float m0 = l0 ? v10[c + h] : v00[c + h];
-              const float m1 = l1 ? v11[c + h] : v01[c + h];
-              const bool rw = m1 > m0;
-              const uint32_t rowbit = (rw ? l1 : l0) ? 1u : 0u;
-              const float y = (rw ? m1 : m0) + bias8[c + h];
-              idx[(c + h) >> 2] |= ((rowbit << 1) | (rw ? 1u : 0u) | (y > 0.f ? 4u : 0u)) << (((c + h) & 3) * 8);
-              x[h] = y > 0.f ? y : 0.f;
+            for (int hh = 0; hh < 2; ++hh) {
+              const int win = qd * 32 + mt * 16 + hh * 8 + (lane >> 2);
+              float x[2];
+              uint32_t code = 0u;
+#pragma unroll
+              for (int e = 0; e < 2; ++e) {
+                const int q = hh * 2 + e;
+                const float a00 = acc[0][i][mt][q], a01 = acc[1][i][mt][q];
+                const float a10 = acc[2][i][mt][q], a11 = acc[3][i][mt][q];
+                // same tie-breaking as G1: lower row wins only if strictly greater, then right column likewise
+                const bool l0 = a10 > a00;
+                const bool l1 = a11 > a01;
+                const float m0 = l0 ? a10 : a00;
+                const float m1 = l1 ? a11 : a01;
+                const bool rw = m1 > m0;
+                const uint32_t rowbit = (rw ? l1 : l0) ? 1u : 0u;
+                const float y = (rw ? m1 : m0) + (e ? bb.y : bb.x);
+                // bits 0-1: arg-max position (row*2 + col) in the window, bit 2: unit active (ReLU mask)
+                code |= ((rowbit << 1) | (rw ? 1u : 0u) | (y > 0.f ? 4u : 0u)) << (e * 8);
+                x[e] = y > 0.f ? y : 0.f;
+              }
+              const uint32_t o = (uint32_t)(win * CO + col);
+              sts_u32(sv + ((o * 2) ^ vx), pack_bf16x2(x[0], x[1]));
+              sts_u16(sc + (o ^ cx), (uint16_t)code);        // staged always, stored only with an arg-max buffer
             }
-            packed[c >> 1] = pack_bf16x2(x[0], x[1]);
-          }
-          if (j < a.Wp) {
-            const size_t o = (row_out + j) * CO + ch * 8;
-            *reinterpret_cast<uint4*>(a.out + o) = make_uint4(packed[0], packed[1], packed[2], packed[3]);
-            if (a.argmax) *reinterpret_cast<uint2*>(a.argmax + o) = make_uint2(idx[0], idx[1]);
-          }
         }
       }
+      // The pooled row t = b * Hp + hp is rows t*Wp .. t*Wp + Wp-1 of the [B*Hp*Wp, CO] outputs: one TMA store
+      // each, whose box of Wp rows leaves the staged windows past the row's end behind. Thread 0 issues the stores
+      // after the eight warps' writes are visible to the async proxy; it first waits until the previous tile's
+      // stores have read the other buffer, which the next tile fills, so one barrier per tile suffices.
+      fence_proxy_async();
+      if (threadIdx.x == 0) tma_wait_read<0>();
+      named_barrier_sync(1, 256);
+      if (threadIdx.x == 0
+#ifdef HEFL_CONV_DEBUG
+          && !(a.dbg & 4)
+#endif
+      ) {
+        const uint8_t* tile = sOut + ob * Cfg::OUT_BYTES;
+        tma_store_2d(&tmO, 0, t * a.Wp, tile);
+        if (a.argmax) tma_store_2d(&tmC, 0, t * a.Wp, tile + Cfg::OUT_V);
+        tma_commit();
+      }
+      ob ^= 1;
       if (++buf == Cfg::NBUF) { buf = 0; phase ^= 1; }
     }
+    if (threadIdx.x == 0) tma_wait_all<0>();
   }
 }
 
 template <int CK, int CO, bool SP>
 __global__ void __launch_bounds__(288, PairFwdCfg<CK, CO>::OCC)
 pair_fwd_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmW,
-                const PairFwdArgs a) {
-  pair_fwd_body<CK, CO, SP ? kPairS : kPairPlain>(&tmA, tmW, a);
+                const __grid_constant__ CUtensorMap tmO, const __grid_constant__ CUtensorMap tmC, const PairFwdArgs a) {
+  pair_fwd_body<CK, CO, SP ? kPairS : kPairPlain>(&tmA, tmW, tmO, tmC, a);
 }
 
 // the one-channel layer 1 on the rs-packed input (CK = 16, CO = 32)
 __global__ void __launch_bounds__(288, PairCfgOf<16, 32, kPairRS>::OCC)
 pair_fwd_rs_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmW,
+                   const __grid_constant__ CUtensorMap tmO, const __grid_constant__ CUtensorMap tmC,
                    const PairFwdArgs a) {
-  pair_fwd_body<16, 32, kPairRS>(&tmA, tmW, a);
+  pair_fwd_body<16, 32, kPairRS>(&tmA, tmW, tmO, tmC, a);
 }
 
 // the RGB layer 1 on the compact input (CK = 16, CO = 32): rows are bulk-copied from X, no input tensor map
 __global__ void __launch_bounds__(288, PairCfgOf<16, 32, kPairC>::OCC)
-pair_fwd_compact_kernel(const __grid_constant__ CUtensorMap tmW, const PairFwdArgs a, const __nv_bfloat16* __restrict__ X) {
-  pair_fwd_body<16, 32, kPairC>(nullptr, tmW, a, X);
+pair_fwd_compact_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constant__ CUtensorMap tmO,
+                        const __grid_constant__ CUtensorMap tmC, const PairFwdArgs a,
+                        const __nv_bfloat16* __restrict__ X) {
+  pair_fwd_body<16, 32, kPairC>(nullptr, tmW, tmO, tmC, a, X);
+}
+
+// Store maps of the pooled outputs, both viewed as [B*Hp*Wp rows][CO]: one box is one pooled row (Wp rows), with the
+// swizzle the epilogue stages it in. Without arg-max codes the code map is left empty and never used.
+static void make_pair_out_maps(const PairFwdArgs& a, int CO, CUtensorMap& tmO, CUtensorMap& tmC) {
+  const uint64_t rows = (uint64_t)a.B * a.Hp * a.Wp;
+  tmO = make_map(a.out, CO, rows, (uint64_t)CO * 2, CO, a.Wp);
+  tmC = CUtensorMap{};
+  if (a.argmax)
+    tmC = tensor_map(a.argmax, CU_TENSOR_MAP_DATA_TYPE_UINT8, {(uint64_t)CO, rows}, {(uint64_t)CO},
+                     {(uint32_t)CO, (uint32_t)a.Wp}, swizzle_for(CO));
 }
 
 template <int CK, int CO, int PK = kPairPlain>
@@ -822,23 +887,27 @@ static void launch_pair_fwd(const __nv_bfloat16* X, const __nv_bfloat16* Wt, Pai
   const CUtensorMap tmA = make_map(X, 2 * CK, pair_rows, (uint64_t)Cfg::ROW_BYTES, 2 * CK, Cfg::SEG_ROWS);
   const int ntap = PK == kPairRS ? 1 : (PK == kPairS ? 3 : 9);
   const CUtensorMap tmW = make_map(Wt, CK, (uint64_t)ntap * CO, (uint64_t)CK * 2, CK, CO);
-  void (*kern)(const CUtensorMap, const CUtensorMap, const PairFwdArgs);
+  CUtensorMap tmO, tmC;
+  make_pair_out_maps(a, CO, tmO, tmC);
+  void (*kern)(const CUtensorMap, const CUtensorMap, const CUtensorMap, const CUtensorMap, const PairFwdArgs);
   if constexpr (PK == kPairRS) kern = pair_fwd_rs_kernel;
   else kern = pair_fwd_kernel<CK, CO, PK == kPairS>;
   cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM);
   int gx = hefl::cuda::device_sm_count() * Cfg::OCC;
   if (gx > a.num_tiles) gx = a.num_tiles;
-  launch_pdl(kern, dim3(gx), dim3(288), Cfg::SMEM, st, tmA, tmW, a);
+  launch_pdl(kern, dim3(gx), dim3(288), Cfg::SMEM, st, tmA, tmW, tmO, tmC, a);
   hefl::cuda::note_launch();
 }
 
 static void launch_pair_fwd_compact(const __nv_bfloat16* X, const __nv_bfloat16* Wt, PairFwdArgs a, cudaStream_t st) {
   using Cfg = PairCfgOf<16, 32, kPairC>;
   const CUtensorMap tmW = make_map(Wt, 16, 6 * 32, 32, 16, 32);
+  CUtensorMap tmO, tmC;
+  make_pair_out_maps(a, 32, tmO, tmC);
   cudaFuncSetAttribute(pair_fwd_compact_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM);
   int gx = hefl::cuda::device_sm_count() * Cfg::OCC;
   if (gx > a.num_tiles) gx = a.num_tiles;
-  launch_pdl(pair_fwd_compact_kernel, dim3(gx), dim3(288), Cfg::SMEM, st, tmW, a, X);
+  launch_pdl(pair_fwd_compact_kernel, dim3(gx), dim3(288), Cfg::SMEM, st, tmW, tmO, tmC, a, X);
   hefl::cuda::note_launch();
 }
 
@@ -854,6 +923,9 @@ void conv_fwd_pool_pair(const void* X, const void* Wf, const float* bias, void* 
   if (compact && !(CK == 16 && CO == 32 && in_channels == 3 && W <= 256))
     throw std::runtime_error("conv_fwd_pool_pair: the compact input is the RGB first layer (CK=16, CO=32, W <= 256)");
   PairFwdArgs a{};
+#ifdef HEFL_CONV_DEBUG
+  a.dbg = g_dbg;
+#endif
   a.B = B; a.H = H; a.W = W;
   a.Hp = (H - 2) / 2; a.Wp = (W - 2) / 2;
   a.num_tiles = B * a.Hp;

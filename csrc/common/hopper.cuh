@@ -161,6 +161,19 @@ inline CUtensorMapSwizzle swizzle_for(uint32_t inner_box_bytes) {
                                  : CU_TENSOR_MAP_SWIZZLE_32B;
 }
 
+// The driver call needs a current context on the calling thread. A thread that has made no runtime call yet has none
+// (autograd's device thread, for one: the first CUDA work of a backward can be a GEMM's tensor-map encode, which then
+// failed with CUDA_ERROR_INVALID_CONTEXT), so bind the current device's primary context once per thread.
+inline void bind_primary_context() {
+  thread_local bool bound = false;
+  if (!bound) {
+    int dev = 0;
+    cudaGetDevice(&dev);
+    cudaSetDevice(dev);
+    bound = true;
+  }
+}
+
 // Tiled map of the tensor at `ptr`, rank = dims.size(): dims innermost first, strides = the byte strides of
 // dims[1..], one box per copy. Element strides 1, no interleave, 128-byte L2 promotion, out-of-bounds elements
 // zero-filled. Throws with every parameter when the driver rejects the map.
@@ -170,6 +183,7 @@ inline CUtensorMap tensor_map(const void* ptr, CUtensorMapDataType type, std::in
   const uint32_t rank = (uint32_t)dims.size();
   CUtensorMap m;
   CUresult r = CUDA_ERROR_INVALID_VALUE;
+  bind_primary_context();
   if (rank >= 1 && rank <= 5 && strides.size() == rank - 1 && box.size() == rank) {
     const cuuint32_t estr[5] = {1, 1, 1, 1, 1};
     r = encode_tiled_fn()(&m, type, rank, const_cast<void*>(ptr), dims.begin(), strides.begin(), box.begin(), estr,

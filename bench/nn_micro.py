@@ -76,15 +76,10 @@ def main():
         loss.backward()
         return feat.grad.to(torch.bfloat16)
     res["head(torch fwd+bwd)"] = timeit(head)
-    head_call = lambda: ops.head_forward_backward(eng.X[eng.n], pack.flat, pack.grad, eng.head_offs, y, eng.dfeat, eng.h1_buf, eng.dh1_buf, out, None, B, eng.F, eng.H1, eng.H2, eng.C, True)
-    ops.set_head_cluster(0)
-    res["head(4 kernels)"] = timeit(head_call)
-    ops.set_head_cluster(1)
+    head_call = lambda: ops.head_forward_backward(eng.X[eng.n], pack.flat, pack.grad, eng.head_offs, y, eng.dfeat, eng.h1_buf, eng.dh1_buf, out, B, eng.F, eng.H1, eng.H2, eng.C, True)
     res["head(cluster kernel)"] = timeit(head_call)
     m = torch.zeros_like(pack.grad); v = torch.zeros_like(pack.grad); st = torch.ones(1, dtype=torch.int64, device="cuda")
-    res["fused_update(legacy, off)"] = timeit(lambda: ops.fused_update(eng.dW32, eng.table, pack.flat, pack.grad, m, v, eng.shadow, eng.Wf, eng.Wd, st, None, 1e-3, 1e-4, 0.9, 0.999, 1e-7, eng.dense_off, pack.n_trainable))
     res["adam"] = timeit(lambda: ops.adam_step_(pack.trainable(), pack.grad, m, v, eng.shadow, st, None, 1e-3, 1e-4, 0.9, 0.999, 1e-7))
-    eng.step_ref = st
     from hefl_b200.fl.trainer import LocalTrainer
     tr = LocalTrainer(model, pack, cfg, dev, backend="tcgen05", use_graph=False)
     eng = tr.engine
@@ -100,7 +95,7 @@ def main():
     with torch.cuda.graph(gph):
         full_step()
     res["train_step(graph)"] = timeit(lambda: gph.replay(), iters=10)
-    skip = ("train_step", "head(torch", "head(4", "make_theta", "fused_update", "unpool0", "wgrad0(tcgen05)")
+    skip = ("train_step", "head(torch", "make_theta", "unpool0", "wgrad0(tcgen05)")
     tot = sum(v for k, v in res.items() if not k.startswith(skip))
     for k, v in res.items():
         print(f"{k:24s} {v:9.1f} us")

@@ -3,7 +3,6 @@
 
 Pairs, each timed alternately 5 times (the two arms share the clock and the neighbours' load):
   * ``adam_step_`` without / with the anchor, at the medical CNN's 222,722 parameters and at ResNet-18's count;
-  * ``fused_update`` (the one-launch engine update) without / with the anchor;
   * one ``train_step`` (CUDA graph) of the medical-CNN engine at mu = 0 / mu = 0.01.
 The proximal term adds one fp32 read of the anchor per parameter (0.9 MB per medical-CNN step).
 
@@ -93,15 +92,6 @@ def main():
         model = create_model("medcnn").to(dev)
         pack = ParamPack(model)
         return LocalTrainer(model, pack, cfg, dev, backend="tcgen05", use_graph=True, augment=True), pack
-
-    tr, pack = trainer(0.0)
-    eng = tr.engine
-    anchor = pack.trainable().clone()
-    st = torch.ones(1, dtype=torch.int64, device=dev)
-    fu = lambda a, mu: ops.fused_update(eng.dW32, eng.table, pack.flat, pack.grad, tr.m, tr.v, eng.shadow, eng.Wf,  # noqa: E731
-                                        eng.Wd, st, None, 1e-3, 1e-4, 0.9, 0.999, 1e-7, eng.dense_off,
-                                        pack.n_trainable, a, mu)
-    pair("fused_update medcnn", lambda: fu(None, 0.0), lambda: fu(anchor, 0.01))
 
     g = torch.Generator(device="cuda").manual_seed(1)
     x = torch.randint(0, 256, (32, 256, 256, 3), dtype=torch.uint8, device=dev, generator=g)

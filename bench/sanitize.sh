@@ -17,10 +17,10 @@ run he_racecheck racecheck tests/test_gpu_he.py -k "ntt_gpu_matches_cpu and 12 o
 run he_synccheck synccheck tests/test_gpu_he.py -k "fedavg_end_to_end or encrypt_decrypt_gpu_bit_exact and 4096"
 run conv_memcheck memcheck tests/test_gpu_conv.py -k "unpool or preprocess or (fwd_pool and 20) or (wgrad and 20) or (dgrad and 14)"
 fi
-# kernels added later: gather wgrad (66-pixel case), cluster head (DSMEM), s-packed first layer (70-pixel case),
-# fused un-pool dgrad, BatchNorm / avg-pool / fp8 quantise
+# kernels added later: gather wgrad (66-pixel case), dense head (cluster kernel with DSMEM, and the 4-kernel
+# fallback), s-packed first layer (70-pixel case), BatchNorm / avg-pool / fp8 quantise
 if [ "${1:-all}" = "new" ] || [ "${1:-all}" = "all" ]; then
-run new_memcheck memcheck tests/test_gpu_conv.py -k "(gather and 66) or (head and 8-2-True) or (spack and 70) or fused_unpool"
-run new_racecheck racecheck tests/test_gpu_conv.py -k "(gather and 66) or (head and 8-2-True-1)"
+run new_memcheck memcheck tests/test_gpu_conv.py -k "(gather and 66) or (head and 8-2-True) or (spack and 70)"
+run new_racecheck racecheck tests/test_gpu_conv.py -k "(gather and 66) or (head and 8-2-True-512)"
 run resnet_memcheck memcheck tests/test_gpu_resnet.py -k "(bn_act and shape2) or avgpool or fp8_conv1x1"
 fi

@@ -1,5 +1,5 @@
 """Times the captured training-step CUDA graph of the medical CNN (tcgen05 engine): median of
-N replays on fresh data indices, L2 flushed between replays. HEFL_PDL=0/1 toggles PDL."""
+N replays on fresh data indices, L2 flushed between replays."""
 import os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__)))))
 import torch
@@ -31,4 +31,4 @@ s.record()
 for _ in range(50):
     tr.train_step(x, y)
 e.record(); torch.cuda.synchronize()
-print(f"PDL={os.environ.get('HEFL_PDL','1')} graph step median {ts[len(ts)//2]:.1f} us (L2 flushed), back-to-back {s.elapsed_time(e)*1e3/50:.1f} us/step, loss {tr.out_train.tolist()}")
+print(f"graph step median {ts[len(ts)//2]:.1f} us (L2 flushed), back-to-back {s.elapsed_time(e)*1e3/50:.1f} us/step, loss {tr.out_train.tolist()}")

@@ -80,11 +80,6 @@ struct TapGemmArgs {
   const float* bias;    // [CO] (POOL)
   __nv_bfloat16* out;   // POOL: [B,Hp,Wp,CO]; else [P,CO]
   uint8_t* argmax;      // POOL, may be null
-  // dgrad with the un-pooling of the PREVIOUS layer fused into the epilogue: the gradient of pixel m of this
-  // layer's input (= pooled output of the previous layer) is scattered straight to the arg-max position of its
-  // 2x2 window on the previous layer's conv grid (up_W x up_W per image), zeros to the other three positions.
-  const uint8_t* up_amax;   // [P, co_total] codes of the previous layer (bits 0-1 position, bit 2 active) or null
-  int up_W;
   // tile -> (image, row pair, column tile) without integer division: q = umulhi(n, magic) is exact for
   // n, d < 2^16 with magic = ceil(2^32 / d) (the epilogue warps spent ~40 of their ~100 per-tile set-up
   // instructions in two software divisions)
@@ -363,32 +358,9 @@ tap_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
             frag_rows(scr, acc[0][i][0], acc[0][i][1], lane, v);
             if (m < a.P) {
               const int c0 = blockIdx.y * CO + ch * 8;
-              const uint32_t pk[4] = {pack_bf16x2(v[0], v[1]), pack_bf16x2(v[2], v[3]), pack_bf16x2(v[4], v[5]),
-                                      pack_bf16x2(v[6], v[7])};
-              if (a.up_amax == nullptr) {
-                *reinterpret_cast<uint4*>(a.out + (size_t)m * a.co_total + c0) = make_uint4(pk[0], pk[1], pk[2], pk[3]);
-              } else {
-                const int hw = a.H * a.W;
-                const int b = m / hw, rem = m - b * hw;
-                const int y = rem / a.W, x = rem - y * a.W;
-                const size_t up_base = ((size_t)b * a.up_W + 2 * y) * a.up_W + 2 * x;   // window's top-left pixel
-                const uint2 code = *reinterpret_cast<const uint2*>(a.up_amax + (size_t)m * a.co_total + c0);
-                const uint32_t cw[2] = {code.x, code.y};
-#pragma unroll
-                for (int q = 0; q < 4; ++q) {
-                  uint32_t o[4];
-#pragma unroll
-                  for (int e = 0; e < 4; ++e) {
-                    const uint32_t ca = (cw[e >> 1] >> ((e & 1) * 16)) & 0xFFu;          // channel 2e
-                    const uint32_t cb = (cw[e >> 1] >> ((e & 1) * 16 + 8)) & 0xFFu;      // channel 2e+1
-                    const uint32_t lo = (ca == (4u | q)) ? (pk[e] & 0xFFFFu) : 0u;
-                    const uint32_t hi = (cb == (4u | q)) ? (pk[e] & 0xFFFF0000u) : 0u;
-                    o[e] = lo | hi;
-                  }
-                  const size_t px = up_base + (size_t)(q >> 1) * a.up_W + (q & 1);
-                  *reinterpret_cast<uint4*>(a.out + px * a.co_total + c0) = make_uint4(o[0], o[1], o[2], o[3]);
-                }
-              }
+              *reinterpret_cast<uint4*>(a.out + (size_t)m * a.co_total + c0) =
+                  make_uint4(pack_bf16x2(v[0], v[1]), pack_bf16x2(v[2], v[3]), pack_bf16x2(v[4], v[5]),
+                             pack_bf16x2(v[6], v[7]));
             }
           }
         }
@@ -481,11 +453,8 @@ void conv_fwd_pool(const void* X, const void* Wf, const float* bias, void* out, 
   else launch_tap_gemm<64, 128, true>(x, w, a, st);
 }
 
-void conv_dgrad(const void* dY, const void* Wd, void* dX, int B, int H, int W, int CK, int CO, const uint8_t* up_amax,
-                int up_W, cudaStream_t st) {
+void conv_dgrad(const void* dY, const void* Wd, void* dX, int B, int H, int W, int CK, int CO, cudaStream_t st) {
   TapGemmArgs a{};
-  a.up_amax = up_amax;
-  a.up_W = up_W;
   a.B = B; a.H = H; a.W = W;
   a.P = B * H * W;
   a.num_tiles = (a.P + 127) / 128;

@@ -62,7 +62,6 @@ struct HeadClusterArgs {
   float *gW1, *gb1, *gW2, *gb2, *gW3, *gb3;
   __nv_bfloat16* dfeat;        // [B][F]
   float* out;                  // [2] loss, ncorrect
-  int64_t* step;               // may be null
   int B, C, train;
 };
 
@@ -246,7 +245,6 @@ __global__ void __launch_bounds__(hc::NT, 1) head_cluster_kernel(const HeadClust
     if (t == 0 && r == 0) {
       a.out[0] = l / B;
       a.out[1] = nc;
-      if (a.train && a.step) *a.step += 1;
     }
   }
   __syncthreads();
@@ -374,10 +372,10 @@ bool head_cluster_supported(int B, int F, int H1, int H2, int C) {
 
 void head_cluster(const void* feat, const float* W1, const float* b1, const float* W2, const float* b2,
                   const float* W3, const float* b3, const int64_t* y, float* gW1, float* gb1, float* gW2, float* gb2,
-                  float* gW3, float* gb3, void* dfeat, float* out, int64_t* step, int B, int C, int train,
+                  float* gW3, float* gb3, void* dfeat, float* out, int B, int C, int train,
                   cudaStream_t st) {
   HeadClusterArgs a{reinterpret_cast<const __nv_bfloat16*>(feat), W1, b1, W2, b2, W3, b3, y, gW1, gb1, gW2, gb2, gW3, gb3,
-                    reinterpret_cast<__nv_bfloat16*>(dfeat), out, step, B, C, train};
+                    reinterpret_cast<__nv_bfloat16*>(dfeat), out, B, C, train};
   cudaFuncSetAttribute(head_cluster_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, hc::SMEM_BYTES);
   cudaLaunchConfig_t cfg = {};
   cfg.gridDim = dim3(hc::R);
@@ -390,7 +388,7 @@ void head_cluster(const void* feat, const float* W1, const float* b1, const floa
   attr[0].val.clusterDim.y = 1;
   attr[0].val.clusterDim.z = 1;
   attr[1].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[1].val.programmaticStreamSerializationAllowed = g_pdl ? 1 : 0;
+  attr[1].val.programmaticStreamSerializationAllowed = 1;
   cfg.attrs = attr;
   cfg.numAttrs = 2;
   cudaLaunchKernelEx(&cfg, head_cluster_kernel, a);

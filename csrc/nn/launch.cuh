@@ -5,14 +5,12 @@
 // their set-up while the previous kernel drains. griddepcontrol.wait returns only when the previous
 // grid has completed and its memory is visible, so data dependencies are unchanged (and transitive,
 // because every kernel in the chain waits before it exits). Captured into the CUDA graph as
-// programmatic edges. HEFL_PDL=0 (or set_pdl(false)) turns the attribute off for A/B timing.
+// programmatic edges.
 #pragma once
 #include <cuda_runtime.h>
 
 namespace hefl {
 namespace nn {
-
-extern int g_pdl;
 
 __device__ __forceinline__ void pdl_trigger() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
@@ -20,7 +18,7 @@ __device__ __forceinline__ void pdl_prologue() {
   pdl_trigger();
   pdl_wait();
 }
-// Kernels that WRITE the parameters (Adam, weight re-layout, fused update) call only pdl_wait(): they never
+// Kernels that WRITE the parameters (Adam, weight re-layout) call only pdl_wait(): they never
 // trigger their dependents early, so no later kernel can be resident before the new weights are complete.
 // That is what allows the dense-head kernels to stage their weight tiles BEFORE griddepcontrol.wait (while
 // the previous kernel is still running) — activations are only touched after the wait.
@@ -35,7 +33,7 @@ inline cudaError_t launch_pdl(void (*kern)(KArgs...), dim3 grid, dim3 block, siz
   cfg.stream = st;
   cudaLaunchAttribute attr[1];
   attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[0].val.programmaticStreamSerializationAllowed = g_pdl ? 1 : 0;
+  attr[0].val.programmaticStreamSerializationAllowed = 1;
   cfg.attrs = attr;
   cfg.numAttrs = 1;
   return cudaLaunchKernelEx(&cfg, kern, static_cast<KArgs>(args)...);

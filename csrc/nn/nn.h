@@ -25,8 +25,7 @@ bool conv_fwd_pool_pair_supported(int H, int W, int CK, int CO);
 void conv_fwd_pool_pair(const void* X, const void* Wf, const float* bias, void* out, uint8_t* argmax, int B, int H,
                         int W, int CK, int CO, int spack, int in_channels, int compact, cudaStream_t st);
 void conv_set_debug(int mask);
-void conv_dgrad(const void* dY, const void* Wd, void* dX, int B, int H, int W, int CK, int CO, const uint8_t* up_amax,
-                int up_W, cudaStream_t st);
+void conv_dgrad(const void* dY, const void* Wd, void* dX, int B, int H, int W, int CK, int CO, cudaStream_t st);
 // Split-K weight gradients write one partial per CTA into a workspace and add the partials to dW32 in a fixed order
 // (fp32 atomics would make the sum, and so training, depend on timing). ws: conv_wgrad_ws_floats(...) floats.
 int64_t conv_wgrad_ws_floats(int B, int H, int W, int CK, int Co);
@@ -37,13 +36,11 @@ void conv_wgrad(const void* X, const void* DY, float* dW32, float* ws, int B, in
 void head_forward_backward(const void* feat, const float* W1, const float* b1, const float* W2, const float* b2,
                            const float* W3, const float* b3, const int64_t* y, float* gW1, float* gb1, float* gW2,
                            float* gb2, float* gW3, float* gb3, void* dfeat, float* h1_buf, float* dh1_buf,
-                           float* out, int64_t* step, int B, int F, int H1, int H2, int C, int train, cudaStream_t st);
-void set_pdl(int on);
+                           float* out, int B, int F, int H1, int H2, int C, int train, cudaStream_t st);
 bool head_cluster_supported(int B, int F, int H1, int H2, int C);
 void head_cluster(const void* feat, const float* W1, const float* b1, const float* W2, const float* b2,
                   const float* W3, const float* b3, const int64_t* y, float* gW1, float* gb1, float* gW2, float* gb2,
-                  float* gW3, float* gb3, void* dfeat, float* out, int64_t* step, int B, int C, int train,
-                  cudaStream_t st);
+                  float* gW3, float* gb3, void* dfeat, float* out, int B, int C, int train, cudaStream_t st);
 bool wgrad0_gather_supported(int W, int Wp, int CK, int Ci, int Co);
 // layer-1 partials: [wgrad0_parts(B, Hp)][kWgrad0Part] floats of workspace
 constexpr int kWgrad0Part = 28 * 32;
@@ -106,10 +103,6 @@ void unpool_relu(const void* g, const uint8_t* amax, const void* ypool, void* dY
 void conv_weight_relayout(const void* shadow, const ConvLayerTable& t, void* Wf, void* Wd, int l0, int l1,
                           int spack0, int compact0, cudaStream_t st);
 void conv_grad_finalize(float* dW32, const ConvLayerTable& t, float* grad, int l0, int l1, cudaStream_t st);
-void fused_update(float* dW32, const ConvLayerTable& t, float* flat, float* grad, float* m, float* v, void* shadow,
-                  void* Wf, void* Wd, const int64_t* step, const float* lr_scale, float lr, float decay, float beta1,
-                  float beta2, float eps, int64_t dense_off, int64_t n_trainable, const float* anchor, float mu,
-                  cudaStream_t st);
 
 }  // namespace nn
 }  // namespace hefl

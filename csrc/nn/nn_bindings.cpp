@@ -111,8 +111,6 @@ void conv_fwd_pool(const Tensor& X, const Tensor& Wf, const Tensor& bias, Tensor
                           (int)W, (int)CK, (int)CO, spack ? 1 : 0, (int)in_channels, cur());
 }
 
-// up_amax given: the un-pooling of the previous layer is fused into the epilogue — dX is then that layer's
-// conv-grid gradient [B*up_W*up_W, CO] (H = W = (up_W - 2) / 2 of this call), written at the arg-max positions.
 // Pair-row forward kernel (conv_tcgen05.cu G1b): same contract as conv_fwd_pool with the plain [9, CO, CK] weights.
 void conv_fwd_pool_pair(const Tensor& X, const Tensor& Wf, const Tensor& bias, Tensor out,
                         const c10::optional<Tensor>& argmax, int64_t B, int64_t H, int64_t W, int64_t CK, int64_t CO,
@@ -140,19 +138,11 @@ void conv_fwd_pool_pair(const Tensor& X, const Tensor& Wf, const Tensor& bias, T
 }
 
 void conv_dgrad(const Tensor& dY, const Tensor& Wd, Tensor dX, int64_t B, int64_t H, int64_t W, int64_t CK,
-                int64_t CO, const c10::optional<Tensor>& up_amax, int64_t up_W) {
+                int64_t CO) {
   chk_bf16(dY, "dY"); chk_bf16(Wd, "Wd"); chk_bf16(dX, "dX");
   TORCH_CHECK(dY.numel() == B * H * W * CK && Wd.numel() == 9 * CO * CK, "shape mismatch");
-  const uint8_t* up = nullptr;
-  if (up_amax.has_value()) {
-    TORCH_CHECK(up_amax->is_cuda() && up_amax->scalar_type() == at::kByte && up_amax->numel() == B * H * W * CO, "bad up_amax");
-    TORCH_CHECK(H == W && (up_W - 2) / 2 == H && dX.numel() == B * up_W * up_W * CO, "fused un-pool: dX must be [B*up_W*up_W, CO]");
-    up = up_amax->data_ptr<uint8_t>();
-  } else {
-    TORCH_CHECK(dX.numel() == B * H * W * CO, "dX must be [B*H*W, CO]");
-  }
-  hefl::nn::conv_dgrad(dY.data_ptr(), Wd.data_ptr(), dX.data_ptr(), (int)B, (int)H, (int)W, (int)CK, (int)CO, up, (int)up_W,
-                       cur());
+  TORCH_CHECK(dX.numel() == B * H * W * CO, "dX must be [B*H*W, CO]");
+  hefl::nn::conv_dgrad(dY.data_ptr(), Wd.data_ptr(), dX.data_ptr(), (int)B, (int)H, (int)W, (int)CK, (int)CO, cur());
 }
 
 void conv_wgrad(const Tensor& X, const Tensor& DY, Tensor dW32, int64_t B, int64_t H, int64_t W, int64_t CK, int64_t Co) {
@@ -204,12 +194,9 @@ void unpool_relu(const Tensor& g, const Tensor& amax, const Tensor& ypool, Tenso
                         (int)W, (int)Hp, (int)Wp, (int)Co, cur());
 }
 
-static int g_head_cluster = 1;
-
 // flat / grad are the ParamPack buffers; offs = [W1, b1, W2, b2, W3, b3] element offsets.
 void head_forward_backward(const Tensor& feat, const Tensor& flat, Tensor grad, at::IntArrayRef offs, const Tensor& y,
-                           Tensor dfeat, Tensor h1_buf, Tensor dh1_buf, Tensor out, const c10::optional<Tensor>& step,
-                           int64_t B, int64_t F, int64_t H1, int64_t H2, int64_t C, bool train) {
+                           Tensor dfeat, Tensor h1_buf, Tensor dh1_buf, Tensor out, int64_t B, int64_t F, int64_t H1, int64_t H2, int64_t C, bool train) {
   chk_bf16(feat, "feat"); chk_bf16(dfeat, "dfeat");
   TORCH_CHECK(offs.size() == 6, "need six parameter offsets");
   TORCH_CHECK(B <= 32 && B >= 1, "the head kernels handle up to 32 samples per step");
@@ -219,26 +206,22 @@ void head_forward_backward(const Tensor& feat, const Tensor& flat, Tensor grad, 
   TORCH_CHECK(h1_buf.numel() >= B * H1 && dh1_buf.numel() >= B * (H1 + H2) && out.numel() >= 2, "scratch too small");
   const float* p = flat.data_ptr<float>();
   float* g = grad.data_ptr<float>();
-  if (g_head_cluster && hefl::nn::head_cluster_supported((int)B, (int)F, (int)H1, (int)H2, (int)C)) {
+  if (hefl::nn::head_cluster_supported((int)B, (int)F, (int)H1, (int)H2, (int)C)) {
     // one launch on a cluster of 8 CTAs (csrc/nn/head_cluster.cu)
     hefl::nn::head_cluster(feat.data_ptr(), p + offs[0], p + offs[1], p + offs[2], p + offs[3], p + offs[4], p + offs[5],
                            y.data_ptr<int64_t>(), g + offs[0], g + offs[1], g + offs[2], g + offs[3], g + offs[4],
-                           g + offs[5], dfeat.data_ptr(), out.data_ptr<float>(),
-                           step.has_value() ? step->data_ptr<int64_t>() : nullptr, (int)B, (int)C, train ? 1 : 0, cur());
+                           g + offs[5], dfeat.data_ptr(), out.data_ptr<float>(), (int)B, (int)C, train ? 1 : 0, cur());
     return;
   }
   TORCH_CHECK(B % 2 == 0 && H2 % 4 == 0 && H1 % 4 == 0 && F % 8 == 0, "head dims must be even / multiples of 4 / 8");
   hefl::nn::head_forward_backward(feat.data_ptr(), p + offs[0], p + offs[1], p + offs[2], p + offs[3], p + offs[4],
                                   p + offs[5], y.data_ptr<int64_t>(), g + offs[0], g + offs[1], g + offs[2],
                                   g + offs[3], g + offs[4], g + offs[5], dfeat.data_ptr(), h1_buf.data_ptr<float>(),
-                                  dh1_buf.data_ptr<float>(), out.data_ptr<float>(),
-                                  step.has_value() ? step->data_ptr<int64_t>() : nullptr, (int)B, (int)F, (int)H1, (int)H2,
+                                  dh1_buf.data_ptr<float>(), out.data_ptr<float>(), (int)B, (int)F, (int)H1, (int)H2,
                                   (int)C, train ? 1 : 0, cur());
 }
 
 void conv_set_debug(int64_t mask) { hefl::nn::conv_set_debug((int)mask); }
-
-hefl::nn::ConvLayerTable table_from(const Tensor& t);
 
 // x, res, y: NHWC bf16 viewed as [P, C]. Returns nothing; mean/invstd/sums are caller-provided fp32 scratch.
 void bn_forward(const Tensor& x, const c10::optional<Tensor>& res, const Tensor& gamma, const Tensor& beta,
@@ -409,27 +392,6 @@ void fp8_quantize(const Tensor& x, Tensor q, const Tensor& scale, Tensor amax) {
                          x.numel(), cur());
 }
 
-void fused_update(Tensor dW32, const Tensor& table, Tensor flat, Tensor grad, Tensor m, Tensor v, Tensor shadow, Tensor Wf,
-                  Tensor Wd, const Tensor& step, const c10::optional<Tensor>& lr_scale, double lr, double decay,
-                  double beta1, double beta2, double eps, int64_t dense_off, int64_t n_trainable,
-                  const c10::optional<Tensor>& anchor, double mu) {
-  chk_bf16(shadow, "shadow"); chk_bf16(Wf, "Wf"); chk_bf16(Wd, "Wd");
-  TORCH_CHECK(flat.scalar_type() == at::kFloat && grad.scalar_type() == at::kFloat && m.scalar_type() == at::kFloat &&
-              v.scalar_type() == at::kFloat && dW32.scalar_type() == at::kFloat, "float32 buffers required");
-  TORCH_CHECK(step.is_cuda() && step.scalar_type() == at::kLong, "step must be a CUDA int64 tensor");
-  const float* ap = nullptr;
-  if (anchor.has_value() && (float)mu != 0.0f) {
-    TORCH_CHECK(anchor->is_cuda() && anchor->scalar_type() == at::kFloat && anchor->is_contiguous() &&
-                anchor->numel() >= n_trainable, "anchor must be a contiguous float32 CUDA tensor of n_trainable values");
-    ap = anchor->data_ptr<float>();
-  }
-  hefl::nn::fused_update(dW32.data_ptr<float>(), table_from(table), flat.data_ptr<float>(), grad.data_ptr<float>(),
-                         m.data_ptr<float>(), v.data_ptr<float>(), shadow.data_ptr(), Wf.data_ptr(), Wd.data_ptr(),
-                         step.data_ptr<int64_t>(), lr_scale.has_value() ? lr_scale->data_ptr<float>() : nullptr,
-                         (float)lr, (float)decay, (float)beta1, (float)beta2, (float)eps, dense_off, n_trainable,
-                         ap, (float)mu, cur());
-}
-
 Tensor umma_shift_probe(const Tensor& A, const Tensor& Bm, int64_t CK, int64_t shift_rows) {
   chk_bf16(A, "A"); chk_bf16(Bm, "Bm");
   TORCH_CHECK(A.numel() == 144 * CK && Bm.numel() == 32 * CK, "A must be [144,CK], B [32,CK]");
@@ -479,15 +441,12 @@ TORCH_LIBRARY_FRAGMENT(hefl, m) {
   m.def("gather_h2d_(Tensor(a!) dst, Tensor src, Tensor indices) -> ()", &gather_h2d_);
   m.def("conv_fwd_pool(Tensor X, Tensor Wf, Tensor bias, Tensor(a!) out, Tensor(b!)? argmax, int B, int H, int W, int CK, int CO, bool spack=False, int in_channels=3) -> ()", &conv_fwd_pool);
   m.def("conv_fwd_pool_pair(Tensor X, Tensor Wf, Tensor bias, Tensor(a!) out, Tensor(b!)? argmax, int B, int H, int W, int CK, int CO, bool spack=False, int in_channels=3, bool compact=False) -> ()", &conv_fwd_pool_pair);
-  m.def("conv_dgrad(Tensor dY, Tensor Wd, Tensor(a!) dX, int B, int H, int W, int CK, int CO, Tensor? up_amax=None, int up_W=0) -> ()", &conv_dgrad);
+  m.def("conv_dgrad(Tensor dY, Tensor Wd, Tensor(a!) dX, int B, int H, int W, int CK, int CO) -> ()", &conv_dgrad);
   m.def("conv_wgrad(Tensor X, Tensor DY, Tensor(a!) dW32, int B, int H, int W, int CK, int Co) -> ()", &conv_wgrad);
   m.def("preprocess_u8(Tensor x, Tensor? theta, Tensor(a!) X, int aug_seed, Tensor? step, bool spack=False, bool compact=False) -> ()", &preprocess_u8);
   m.def("unpool_relu(Tensor g, Tensor amax, Tensor ypool, Tensor(a!) dY, int B, int H, int W, int Co) -> ()", &unpool_relu);
-  m.def("head_forward_backward(Tensor feat, Tensor flat, Tensor(a!) grad, int[] offs, Tensor y, Tensor(b!) dfeat, Tensor(c!) h1_buf, Tensor(d!) dh1_buf, Tensor(e!) out, Tensor(f!)? step, int B, int F, int H1, int H2, int C, bool train) -> ()", &head_forward_backward);
-  m.def("fused_update(Tensor(a!) dW32, Tensor table, Tensor(b!) flat, Tensor(c!) grad, Tensor(d!) m, Tensor(e!) v, Tensor(f!) shadow, Tensor(g!) Wf, Tensor(h!) Wd, Tensor step, Tensor? lr_scale, float lr, float decay, float beta1, float beta2, float eps, int dense_off, int n_trainable, Tensor? anchor=None, float mu=0.0) -> ()", &fused_update);
+  m.def("head_forward_backward(Tensor feat, Tensor flat, Tensor(a!) grad, int[] offs, Tensor y, Tensor(b!) dfeat, Tensor(c!) h1_buf, Tensor(d!) dh1_buf, Tensor(e!) out, int B, int F, int H1, int H2, int C, bool train) -> ()", &head_forward_backward);
   m.def("conv_set_debug(int mask) -> ()", &conv_set_debug);
-  m.def("set_head_cluster(int on) -> ()", [](int64_t on) { g_head_cluster = (int)on; });
-  m.def("set_pdl(int on) -> ()", [](int64_t on) { hefl::nn::set_pdl((int)on); });
   m.def("wgrad0_gather(Tensor X, Tensor g, Tensor amax, Tensor(a!) dW32, int B, int H, int W, bool spack=False, int in_channels=3, bool compact=False) -> ()", &wgrad0_gather);
   m.def("fp8_quantize(Tensor x, Tensor(a!) q, Tensor scale, Tensor(b!) amax) -> ()", &fp8_quantize);
   m.def("gemm_taps(Tensor A, Tensor B, Tensor(a!) out, int N, int K, int[] shifts, int padded, int Bn, int H, int W, Tensor? scale_a, Tensor? scale_b) -> ()", &gemm_taps);

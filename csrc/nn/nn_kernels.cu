@@ -10,9 +10,6 @@
 namespace hefl {
 namespace nn {
 
-int g_pdl = 1;
-void set_pdl(int on) { g_pdl = on; }
-
 // PROX: FedProx local objective, the gradient of (mu/2)*||p - anchor||^2 is added to g before the moments
 // (anchor = the round's global model). The extra arguments come last so that <false> keeps today's code.
 template <bool PROX>
@@ -401,96 +398,6 @@ void conv_grad_finalize(float* dW32, const ConvLayerTable& t, float* grad, int l
 }  // namespace nn
 }  // namespace hefl
 
-namespace hefl {
-namespace nn {
-
-// One launch for the whole parameter update of the tcgen05 engine: consumes the wgrad buffers
-// (dW32, rows = tap*CK + ci, last row = bias gradient), applies Adam to the matching entries of the
-// flat fp32 parameters, writes the bf16 shadow and both tensor-core weight layouts (Wf [tap][Co][CK],
-// Wd [tap][Ci][Co]) and clears dW32; the last grid row updates the dense-head parameters from the
-// flat gradient. Replaces finalize + zero + step increment + Adam + relayout (5 launches).
-struct AdamHyper {
-  float lr, decay, beta1, beta2, eps;
-};
-
-__device__ __forceinline__ float adam_one(float p, float g, float& mi, float& vi, float alpha, float b1, float b2,
-                                          float eps) {
-  mi = b1 * mi + (1.f - b1) * g;
-  vi = b2 * vi + (1.f - b2) * g * g;
-  return p - alpha * mi / (sqrtf(vi) + eps);
-}
-
-// PROX: the FedProx term of adam_kernel<true>, applied to the conv entries and the dense tail alike.
-template <bool PROX>
-__global__ void fused_update_kernel(float* __restrict__ dW32, const ConvLayerTable t, float* __restrict__ flat,
-                                    float* __restrict__ grad, float* __restrict__ m, float* __restrict__ v,
-                                    __nv_bfloat16* __restrict__ shadow, __nv_bfloat16* __restrict__ Wf,
-                                    __nv_bfloat16* __restrict__ Wd, const int64_t* __restrict__ step,
-                                    const float* __restrict__ lr_scale, AdamHyper h, int64_t dense_off,
-                                    int64_t n_trainable, const float* __restrict__ anchor, float mu) {
-  pdl_wait();   // parameter writer: no early trigger (see launch.cuh)
-  const float tt = (float)(*step);
-  const float lr_t = h.lr * (lr_scale ? *lr_scale : 1.f) / (1.f + h.decay * (tt - 1.f));
-  const float alpha = lr_t * sqrtf(1.f - powf(h.beta2, tt)) / (1.f - powf(h.beta1, tt));
-  const int l = blockIdx.y;
-  if (l < t.n) {
-    const int Ci = t.Ci[l], CK = t.CK[l], Co = t.Co[l];
-    float* src = dW32 + t.dw_off[l];
-    const int total = (9 * CK + 1) * Co;
-    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < total; i += gridDim.x * blockDim.x) {
-      const int R = i / Co, co = i - R * Co;
-      float g = src[i];
-      src[i] = 0.f;
-      int64_t pi;
-      int tap = 0, ci = 0;
-      if (R == 9 * CK) {
-        pi = t.b_off[l] + co;
-      } else {
-        tap = R / CK;
-        ci = R - tap * CK;
-        if (ci >= Ci) continue;                      // zero-padded input channels of layer 1
-        pi = t.w_off[l] + ((int64_t)co * Ci + ci) * 9 + tap;
-      }
-      if (PROX) g += mu * (flat[pi] - anchor[pi]);
-      float mi = m[pi], vi = v[pi];
-      const float p = adam_one(flat[pi], g, mi, vi, alpha, h.beta1, h.beta2, h.eps);
-      flat[pi] = p; m[pi] = mi; v[pi] = vi;
-      const __nv_bfloat16 pb = __float2bfloat16(p);
-      shadow[pi] = pb;
-      if (R != 9 * CK) {
-        Wf[t.wf_off[l] + ((int64_t)tap * Co + co) * CK + ci] = pb;
-        if (l > 0) Wd[t.wd_off[l] + ((int64_t)tap * Ci + ci) * Co + co] = pb;
-      }
-    }
-  } else {
-    for (int64_t i = dense_off + (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n_trainable;
-         i += (int64_t)gridDim.x * blockDim.x) {
-      float mi = m[i], vi = v[i];
-      float gi = grad[i];
-      if (PROX) gi += mu * (flat[i] - anchor[i]);
-      const float p = adam_one(flat[i], gi, mi, vi, alpha, h.beta1, h.beta2, h.eps);
-      flat[i] = p; m[i] = mi; v[i] = vi;
-      grad[i] = 0.f;
-      shadow[i] = __float2bfloat16(p);
-    }
-  }
-}
-
-void fused_update(float* dW32, const ConvLayerTable& t, float* flat, float* grad, float* m, float* v, void* shadow,
-                  void* Wf, void* Wd, const int64_t* step, const float* lr_scale, float lr, float decay, float beta1,
-                  float beta2, float eps, int64_t dense_off, int64_t n_trainable, const float* anchor, float mu,
-                  cudaStream_t st) {
-  dim3 grid(48, t.n + 1);
-  AdamHyper h{lr, decay, beta1, beta2, eps};
-  launch_pdl(anchor && mu != 0.0f ? fused_update_kernel<true> : fused_update_kernel<false>, dim3(grid), dim3(256), 0, st,
-             dW32, t, flat, grad, m, v, reinterpret_cast<__nv_bfloat16*>(shadow), reinterpret_cast<__nv_bfloat16*>(Wf),
-             reinterpret_cast<__nv_bfloat16*>(Wd), step, lr_scale, h, dense_off, n_trainable, anchor, mu);
-  hefl::cuda::note_launch();
-}
-
-}  // namespace nn
-}  // namespace hefl
-
 // ------------------------------------------------------------------------------------------
 // Dense head of the sequential CNNs: Flatten -> Dense(H1, ReLU) -> Dense(H2, ReLU) -> Dense(C)
 // -> softmax cross-entropy (FLPyfhelin.py:133-136, :141), forward AND backward in four launches
@@ -566,7 +473,6 @@ struct HeadMidArgs {
   float *gW3, *gb3;
   float* dh2;           // [B][H2] out
   float* out;           // [2]: loss, ncorrect
-  int64_t* step;        // optimiser step counter, incremented here once per training step (may be null)
   int B, H1, H2, C, train;
 };
 
@@ -659,7 +565,6 @@ head_mid_kernel(const HeadMidArgs a) {
     if (tid == 0) {
       a.out[0] = l / B;
       a.out[1] = nc;
-      if (a.train && a.step) *a.step += 1;     // read by the update kernel after this one; no other reader now
     }
   }
   __syncthreads();
@@ -796,13 +701,13 @@ head_fc1_bwd_kernel(const float* __restrict__ dh1, const __nv_bfloat16* __restri
 void head_forward_backward(const void* feat, const float* W1, const float* b1, const float* W2, const float* b2,
                            const float* W3, const float* b3, const int64_t* y, float* gW1, float* gb1, float* gW2,
                            float* gb2, float* gW3, float* gb3, void* dfeat, float* h1_buf, float* dh1_buf,
-                           float* out, int64_t* step, int B, int F, int H1, int H2, int C, int train, cudaStream_t st) {
+                           float* out, int B, int F, int H1, int H2, int C, int train, cudaStream_t st) {
   const auto* f = reinterpret_cast<const __nv_bfloat16*>(feat);
   float* dh2_buf = dh1_buf + (size_t)B * H1;                  // scratch tail: [B][H2]
   const int smem_a = (B + 4) * (F + 1) * 4;
   cudaFuncSetAttribute(head_fc1_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_a);
   launch_pdl(head_fc1_fwd_kernel, dim3((H1 + 3) / 4), dim3(128), smem_a, st, f, W1, b1, h1_buf, B, F, H1);
-  HeadMidArgs a{h1_buf, W2, b2, W3, b3, y, gW3, gb3, dh2_buf, out, step, B, H1, H2, C, train};
+  HeadMidArgs a{h1_buf, W2, b2, W3, b3, y, gW3, gb3, dh2_buf, out, B, H1, H2, C, train};
   const int smem_b = (B * (H1 + 1) + H2 * (H1 + 1) + B * (H2 + 1) + B * C + 2 * B + C * H2) * 4;
   cudaFuncSetAttribute(head_mid_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_b);
   launch_pdl(head_mid_kernel, dim3(1), dim3(256), smem_b, st, a);

@@ -95,7 +95,6 @@ class LocalTrainer:
             from ..ops.conv_engine import MedCNNEngine
 
             self.engine = MedCNNEngine(model, pack, cfg, device)
-            self.engine.step_ref = self.step_t
             # staged input pipeline: batch i+1 is pre-processed into the other X0 slot on `prep_stream`
             # while the graph of step i runs; one captured graph per (train/eval, slot)
             self.static_y2 = [torch.zeros(B, dtype=torch.int64, device=device) for _ in range(2)]
@@ -125,26 +124,19 @@ class LocalTrainer:
         return self.model(x)
 
     def _train_eager(self, x_u8: torch.Tensor, y: torch.Tensor) -> None:
-        if self.engine is not None and not self.engine.fused_step:
+        if self.engine is not None:
             self.engine.train_step(x_u8, y, self.out_train, augment=self.augment, opt=self)
             return
-        if self.engine is not None:
-            self.engine.train_step(x_u8, y, self.out_train, augment=self.augment)
-        else:
-            logits = self._forward(x_u8, True)
-            loss = F.cross_entropy(logits, y)
-            loss.backward()
-            self.out_train[0] = loss.detach()
-            self.out_train[1] = (logits.argmax(1) == y).sum()
+        logits = self._forward(x_u8, True)
+        loss = F.cross_entropy(logits, y)
+        loss.backward()
+        self.out_train[0] = loss.detach()
+        self.out_train[1] = (logits.argmax(1) == y).sum()
         self._optimizer_step()
 
     def _train_staged(self, slot: int) -> None:
         """Graph body of the tcgen05 engine: forward/backward on the pre-processed batch of ``slot`` + update."""
-        if self.engine.fused_step:
-            self.engine.train_step_staged(slot, self.static_y2[slot], self.out_train2[slot])
-            self._optimizer_step()
-        else:
-            self.engine.train_step_staged(slot, self.static_y2[slot], self.out_train2[slot], opt=self)
+        self.engine.train_step_staged(slot, self.static_y2[slot], self.out_train2[slot], opt=self)
 
     # update hooks driven by the engine (it knows when each layer's gradient is final)
     def bump(self) -> None:
@@ -159,17 +151,11 @@ class LocalTrainer:
                             self.anchor[lo:hi] if self.anchor is not None else None, self.mu)
 
     def _optimizer_step(self) -> None:
+        """Adam over every parameter after an autograd step (the cudnn and ResNet backends)."""
         c = self.cfg
-        if self.engine is not None and self.engine.fused_step:
-            # step counter bumped by the head kernel
-            self.engine.fused_update(self.m, self.v, self.step_t, self.lr_scale, c, self.anchor, self.mu)
-            return
         self.step_t += 1
-        self.ops.adam_step_(self.pack.trainable(), self.pack.grad, self.m, self.v,
-                            self.engine.shadow if self.engine is not None else None,
+        self.ops.adam_step_(self.pack.trainable(), self.pack.grad, self.m, self.v, None,
                             self.step_t, self.lr_scale, c.lr, c.lr_decay, 0.9, 0.999, 1e-7, self.anchor, self.mu)
-        if self.engine is not None:
-            self.engine.after_update()
 
     def _eval_eager(self, x_u8: torch.Tensor, y: torch.Tensor) -> None:
         with torch.no_grad():

@@ -29,7 +29,7 @@ from __future__ import annotations
 import os
 
 import math
-from typing import List, Optional
+from typing import List
 
 import torch
 import torch.nn.functional as F
@@ -48,8 +48,6 @@ class MedCNNEngine:
         if device.type != "cuda":
             raise RuntimeError("the tcgen05 engine needs a CUDA device (sm_90a)")
         self.ops = _ext.ops()
-        self.ops.set_head_cluster(0 if os.environ.get("HEFL_HEAD_CLUSTER", "1") == "0" else 1)
-        self.ops.set_pdl(0 if os.environ.get("HEFL_PDL", "1") == "0" else 1)   # programmatic dependent launch
         self.model, self.pack, self.cfg, self.device = model, pack, cfg, device
         B, S = cfg.batch_size, cfg.image_size
         if cfg.in_channels not in (1, 3):
@@ -82,15 +80,11 @@ class MedCNNEngine:
         # (conv_tcgen05.cu TS=1); grayscale carries the whole 3x3 neighbourhood, one GEMM (rs layout, TS=kTapsRS)
         self.spack0 = (os.environ.get("HEFL_SPACK0", "1") != "0" and self.Ci[0] in (1, 3) and self.CK[0] == 16
                        and self.Co[0] == 32)
-        # un-pool inside the dgrad epilogue: correct (bit-exact test) but measured 10 us/step SLOWER than the
-        # separate un-pool kernels (the epilogue is issue-bound; 4x the stores), so off by default
         # pair-row forward kernel (both columns of a pooling window in one thread, conv_tcgen05.cu G1b): on by
         # default for layer 1, where it reads the same s-packed input as the tap-GEMM forward (same outputs, tests).
         # On the small layers it runs one 128-window tile per pooled row, so HEFL_FWD_PAIR=all is only for experiments.
         mode = os.environ.get("HEFL_FWD_PAIR", "1")
         self.fwd_pair = {"0": 0, "1": 1, "all": self.n}.get(mode, 0)      # number of leading layers that may use it
-        self.fuse_unpool = os.environ.get("HEFL_FUSE_UNPOOL", "0") != "0"
-        self.fuse_from = int(os.environ.get("HEFL_FUSE_UNPOOL_FROM", "0"))     # fuse only into layers >= this index
         # layer-1 weight gradient by gather from the pooled gradient (csrc/nn/wgrad_gather.cu)
         self.gather_wgrad0 = (os.environ.get("HEFL_GATHER_WGRAD0", "1") != "0" and self.Co[0] == 32
                               and self.CK[0] == 16 and self.H[0] <= 256)
@@ -149,18 +143,11 @@ class MedCNNEngine:
             self.h1_buf = torch.zeros(B * self.H1, dtype=torch.float32, device=device)
             self.dh1_buf = torch.zeros(B * (self.H1 + self.H2), dtype=torch.float32, device=device)
             self.dfeat = torch.zeros(B, self.F, **bf)
-        # one-launch parameter update needs the fused head (it owns the step increment) and the dense
-        # parameters as one contiguous tail of the flat buffer
-        self.dense_off = min(self.head_offs) if self.fused_head else 0
-        # measured: 43 us fused (scattered m/v/flat accesses) vs 24 us for finalize+Adam+relayout -> off by default
-        self.fused_step = os.environ.get("HEFL_FUSED_STEP", "0") == "1" and self.fused_head
         self.theta = torch.zeros(B, 2, 3, dtype=torch.float32, device=device)
         self.aug_seed = (cfg.seed * 2654435761 + 12345) & 0x7FFFFFFFFFFFFFFF or 1
         self.prep_count = 0          # augmented batches pre-processed so far (keys the in-kernel Philox draw)
         # weight gradients run on a side stream, concurrently with the dgrad / un-pool chain
         self.side = torch.cuda.Stream(device)
-        self.two_streams = True
-        self.step_ref: Optional[torch.Tensor] = None     # device step counter (set by the trainer)
         self.after_restore()
 
     @property
@@ -265,14 +252,13 @@ class MedCNNEngine:
         """Forward + backward on the already pre-processed batch in ``slot`` (CUDA-graph body).
 
         ``opt`` (optional) applies the parameter update: ``opt.bump()`` advances the step counter and
-        ``opt.apply(lo, hi)`` runs Adam on flat parameters [lo, hi). With two streams, everything but
-        layer 1 is updated on the side stream while layer 1's weight-gradient kernel still runs; only
-        the layer-1 parameters (896 for RGB, 320 for grayscale) are left for the tail of the step."""
+        ``opt.apply(lo, hi)`` runs Adam on flat parameters [lo, hi). Everything but layer 1 is updated on the side
+        stream while layer 1's weight-gradient kernel still runs; only the layer-1 parameters (896 for RGB, 320 for
+        grayscale) are left for the tail of the step."""
         feat_bf = self.forward_convs(slot, True)
         if self.fused_head:
             self.ops.head_forward_backward(feat_bf, self.pack.flat, self.pack.grad, self.head_offs, y, self.dfeat,
-                                           self.h1_buf, self.dh1_buf, out, self.step_ref if self.fused_step else None,
-                                           self.B, self.F, self.H1, self.H2, self.C, True)
+                                           self.h1_buf, self.dh1_buf, out, self.B, self.F, self.H1, self.H2, self.C, True)
             g = self.dfeat.view_as(feat_bf)
         else:
             feat = feat_bf.view(self.B, -1).float().requires_grad_(True)
@@ -284,11 +270,10 @@ class MedCNNEngine:
             g = feat.grad.to(torch.bfloat16).view_as(feat_bf).contiguous()
         main = torch.cuda.current_stream(self.device)
         split = False
-        dy_ready = False
         for l in range(self.n - 1, -1, -1):
             h = self.H[l]
             if l == 0 and self.gather_wgrad0:
-                if opt is not None and self.two_streams and not self.fused_step and self.n > 1 and self.p0 > 0:
+                if opt is not None and self.n > 1 and self.p0 > 0:
                     split = True
                     ev = torch.cuda.Event()
                     ev.record(main)                     # dgrad of layer 2 (last reader of Wd) is enqueued
@@ -305,32 +290,17 @@ class MedCNNEngine:
             xin = self.X0[slot] if l == 0 else self.X[l]
             if self.dY[l] is None:
                 self.dY[l] = torch.zeros(self.P[l], self.Co[l], dtype=torch.bfloat16, device=self.device)
-            if not dy_ready:
-                self.ops.unpool_relu(g, self.amax[l], self.X[l + 1], self.dY[l], self.B, h, h, self.Co[l])
-            dy_ready = False
-            if self.two_streams and l > 0:
+            self.ops.unpool_relu(g, self.amax[l], self.X[l + 1], self.dY[l], self.B, h, h, self.Co[l])
+            if l > 0:
                 # wgrad(l) only needs X[l] and dY[l]; dgrad(l) -> unpool(l-1) -> ... proceeds meanwhile
                 self.side.wait_stream(main)
                 with torch.cuda.stream(self.side):
                     self.ops.conv_wgrad(xin, self.dY[l], self._dw(l), self.B, h, h, self.CK[l], self.Co[l])
+                self.ops.conv_dgrad(self.dY[l], self._wd(l), self.gX[l], self.B, h, h, self.Co[l], self.Ci[l])
+                g = self.gX[l]
             else:
                 self.ops.conv_wgrad(xin, self.dY[l], self._dw(l), self.B, h, h, self.CK[l], self.Co[l])
-            if l > 0:
-                # dgrad(l) scatters its result straight into the conv-grid gradient of layer l-1 (un-pool fused
-                # into the epilogue) unless that layer takes the gather path, which wants the pooled gradient
-                if self.fuse_unpool and l - 1 >= self.fuse_from and not (l == 1 and self.gather_wgrad0):
-                    if self.dY[l - 1] is None:
-                        self.dY[l - 1] = torch.zeros(self.P[l - 1], self.Co[l - 1], dtype=torch.bfloat16, device=self.device)
-                    self.ops.conv_dgrad(self.dY[l], self._wd(l), self.dY[l - 1], self.B, h, h, self.Co[l], self.Ci[l],
-                                        self.amax[l - 1], self.H[l - 1])
-                    dy_ready = True
-                else:
-                    self.ops.conv_dgrad(self.dY[l], self._wd(l), self.gX[l], self.B, h, h, self.Co[l], self.Ci[l])
-                    g = self.gX[l]
-        if self.two_streams:
-            main.wait_stream(self.side)
-        if self.fused_step:
-            return
+        main.wait_stream(self.side)
         if opt is None:
             self.ops.conv_grad_finalize(self.dW32, self.table, self.pack.grad)
         elif split:
@@ -343,16 +313,6 @@ class MedCNNEngine:
             opt.apply(0, self.pack.n_trainable)
             self.after_update()
 
-    def fused_update(self, m: torch.Tensor, v: torch.Tensor, step: torch.Tensor, lr_scale: torch.Tensor, cfg,
-                     anchor: Optional[torch.Tensor] = None, mu: float = 0.0) -> None:
-        """finalize + Adam + bf16 shadow + tensor-core weight layouts + dW32 clear, one launch. ``anchor`` and
-        ``mu``: the FedProx term, as in ``adam_step_``."""
-        self.ops.fused_update(self.dW32, self.table, self.pack.flat, self.pack.grad, m, v, self.shadow, self.Wf, self.Wd,
-                              step, lr_scale, cfg.lr, cfg.lr_decay, 0.9, 0.999, 1e-7, self.dense_off,
-                              self.pack.n_trainable, anchor, mu)
-        if self.spack0:
-            self.ops.conv_weight_relayout(self.shadow, self.table, self.Wf, self.Wd, 0, 1, True, self.compact0)
-
     def eval_step(self, x_u8: torch.Tensor, y: torch.Tensor, out: torch.Tensor) -> None:
         self.preprocess(x_u8, 0, False, False)
         self.eval_step_staged(0, y, out)
@@ -361,7 +321,7 @@ class MedCNNEngine:
         feat_bf = self.forward_convs(slot, False)
         if self.fused_head:
             self.ops.head_forward_backward(feat_bf, self.pack.flat, self.pack.grad, self.head_offs, y, self.dfeat,
-                                           self.h1_buf, self.dh1_buf, out, None, self.B, self.F, self.H1, self.H2, self.C, False)
+                                           self.h1_buf, self.dh1_buf, out, self.B, self.F, self.H1, self.H2, self.C, False)
             return
         feat = feat_bf.view(self.B, -1).float()
         logits = self._head(feat)

@@ -202,7 +202,6 @@ def test_gray_engine_gradients_match_autograd(packed, gather):
     layer-1 weight gradient) vs PyTorch autograd on the same bf16-rounded weights."""
     model, pack, eng = _gray_engine(8)
     assert eng.spack0 and eng.p0 == 320
-    eng.fused_step = False
     eng.gather_wgrad0 = gather
     if not packed:
         eng.spack0 = False
@@ -264,45 +263,7 @@ def test_gray_engine_rejects_other_channel_counts():
         MedCNNEngine(model, ParamPack(model), FLConfig(model="medcnn", batch_size=8, in_channels=2), torch.device("cuda"))
 
 
-# ------------------------------------------------------------------ 5. fused update
-@pytest.mark.parametrize("packed", [False, True])
-def test_gray_fused_update_matches_separate_path(packed):
-    """finalize + Adam + re-layout in one launch (plus the rs re-layout of layer 1 when packed) == the separate path."""
-    from hefl_b200.config import FLConfig
-    from hefl_b200.fl.trainer import LocalTrainer
-    from hefl_b200.models import ParamPack, create_model
-
-    def run(fused):
-        torch.manual_seed(1)
-        cfg = FLConfig(model="medcnn", batch_size=8, nn_backend="tcgen05", in_channels=1)
-        dev = torch.device("cuda")
-        model = create_model("medcnn", in_channels=1).to(dev)
-        pack = ParamPack(model)
-        tr = LocalTrainer(model, pack, cfg, dev, backend="tcgen05", use_graph=False, augment=False)
-        tr.engine.fused_step = fused
-        tr.engine.two_streams = fused
-        tr.engine.spack0 = packed
-        tr.engine.after_restore()
-        g = torch.Generator(device="cuda").manual_seed(3)
-        x = torch.randint(0, 256, (8, 256, 256, 1), dtype=torch.uint8, device="cuda", generator=g)
-        y = torch.randint(0, 2, (8,), device="cuda", generator=g)
-        for _ in range(3):
-            tr.train_step(x, y)
-        torch.cuda.synchronize()
-        Wf = tr.engine.Wf.clone()
-        if packed:    # layer 1 reads only [1][Co][16]; the one-launch update also leaves its 9-tap layout behind it
-            Wf = torch.cat([Wf[: Co * 16], Wf[tr.engine.wf_off[1]:]])
-        return pack.flat.clone(), Wf, tr.engine.Wd.clone(), int(tr.step_t.item()), tr.out_train.clone()
-
-    a, b = run(True), run(False)
-    assert a[3] == b[3] == 3
-    assert (a[0] - b[0]).abs().max() < 2e-3
-    assert (a[1].float() - b[1].float()).abs().max() < 2e-2
-    assert (a[2].float() - b[2].float()).abs().max() < 2e-2
-    assert abs(float(a[4][0]) - float(b[4][0])) < 5e-3
-
-
-# ------------------------------------------------------------------ 6. training
+# ------------------------------------------------------------------ 5. training
 def _setup(backend, dtype, use_graph, n_img=256, seed=5):
     from hefl_b200.config import FLConfig
     from hefl_b200.fl.data import BatchFeeder, SyntheticImageDataset
@@ -318,6 +279,16 @@ def _setup(backend, dtype, use_graph, n_img=256, seed=5):
     ds = SyntheticImageDataset(n_img, 256, 1, 2, seed=11)
     feed = BatchFeeder(ds, range(0, n_img), 32, dev, shuffle=True, seed=3)
     return tr, pack, feed
+
+
+def _layouts_follow_weights(tr):
+    """After the update (the layers above layer 1 on the side stream, layer 1 in the tail), the bf16 shadow and both
+    tensor-core weight layouts hold exactly the fp32 weights."""
+    eng = tr.engine
+    assert torch.equal(eng.shadow, tr.pack.trainable().to(torch.bfloat16))
+    Wf, Wd = torch.zeros_like(eng.Wf), torch.zeros_like(eng.Wd)
+    tr.ops.conv_weight_relayout(eng.shadow, eng.table, Wf, Wd, 0, -1, eng.spack0, eng.compact0)
+    assert torch.equal(eng.Wf, Wf) and torch.equal(eng.Wd, Wd)
 
 
 def test_three_gray_epochs_of_the_bf16_engine_track_fp32_pytorch():
@@ -349,6 +320,8 @@ def test_gray_graph_and_pipeline_path_equals_the_eager_path_over_eight_steps():
     b.fit(feed_b, None, 1, early_stopping=None, reduce_lr_patience=None)
     torch.cuda.synchronize()
     assert int(a.step_t.item()) == int(b.step_t.item()) == 8
+    _layouts_follow_weights(a)
+    _layouts_follow_weights(b)
     d = (pack_a.flat - pack_b.flat).abs()
     print("gray graph vs eager: max", float(d.max()), "mean", float(d.mean()))
     assert float(d.max()) <= 2 * 8 * 1e-3
@@ -356,7 +329,7 @@ def test_gray_graph_and_pipeline_path_equals_the_eager_path_over_eight_steps():
     assert F.cosine_similarity(pack_a.flat, pack_b.flat, dim=0).item() > 0.9995
 
 
-# ------------------------------------------------------------------ 7. end to end
+# ------------------------------------------------------------------ 6. end to end
 def test_gray_encrypted_fedavg_round():
     """One client, one round: train on the engine, encrypt, aggregate, decrypt; CKKS error as for RGB input."""
     from hefl_b200.config import FLConfig

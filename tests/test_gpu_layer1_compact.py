@@ -154,7 +154,6 @@ def test_engine_gradients_match_autograd_on_the_compact_layout():
     pack = ParamPack(model)
     pack.flat.copy_(pack.flat.to(torch.bfloat16).float())
     eng = MedCNNEngine(model, pack, cfg, dev)
-    eng.fused_step = False
     assert eng.compact0
     g = torch.Generator(device="cuda").manual_seed(7)
     x = torch.randint(0, 256, (8, 256, 256, 3), dtype=torch.uint8, device="cuda", generator=g)

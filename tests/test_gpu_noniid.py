@@ -1,6 +1,6 @@
-"""Non-IID clients on the H100: the FedProx term of the Adam kernels (adam_kernel<true>, fused_update_kernel<true>),
-the engine trained with it, its pull towards the round's global model, sample-weighted encrypted FedAvg on CUDA,
-and the multi-GPU round on the fused transport."""
+"""Non-IID clients on the H100: the FedProx term of the Adam kernel (adam_kernel<true>), the engine trained with it,
+its pull towards the round's global model, sample-weighted encrypted FedAvg on CUDA, and the multi-GPU round on the
+fused transport."""
 import json
 import os
 import subprocess
@@ -66,80 +66,7 @@ def test_prox_adam_kernel_matches_cpu_twin_and_float64(n):
     assert not torch.equal(gpu[0], b[0])
 
 
-# ------------------------------------------------------------------ 2. fused_update with the anchor
-def test_prox_fused_update_matches_finalize_adam_relayout():
-    """fused_update(anchor) == conv_grad_finalize -> adam_step_(anchor) -> conv_weight_relayout on the same
-    gradients, to the last fp32 bits (the op-level twin of test_fused_update_matches_separate_path)."""
-    from hefl_b200.config import FLConfig
-    from hefl_b200.fl.trainer import LocalTrainer
-    from hefl_b200.models import ParamPack, create_model
-
-    ops = _ops()
-    torch.manual_seed(1)
-    dev = torch.device("cuda")
-    cfg = FLConfig(model="medcnn", batch_size=8, nn_backend="tcgen05")
-    model = create_model("medcnn").to(dev)
-    pack = ParamPack(model)
-    tr = LocalTrainer(model, pack, cfg, dev, backend="tcgen05", use_graph=False, augment=False)
-    eng = tr.engine
-    eng.spack0 = False                     # the one-launch update writes the plain 9-tap layer-1 layout
-    eng.after_restore()
-    g = torch.Generator(device="cuda").manual_seed(7)
-    nt = pack.n_trainable
-    dW = torch.randn(eng.dW32.shape, device=dev, generator=g) * 1e-2
-    grad = torch.randn(nt, device=dev, generator=g) * 1e-2
-    m0 = torch.randn(nt, device=dev, generator=g) * 1e-3
-    v0 = torch.rand(nt, device=dev, generator=g) * 1e-4
-    anchor = pack.trainable() + torch.randn(nt, device=dev, generator=g) * 0.05
-    step = torch.tensor([5], dtype=torch.int64, device=dev)
-    lr_scale = torch.ones(1, device=dev)
-    flat0 = pack.flat.clone()
-
-    def state(m, v):    # the one-launch update reads the conv gradients from dW32 and clears only the dense tail
-        return [pack.flat.clone(), m.clone(), v.clone(), eng.shadow.clone(), eng.Wf.clone(), eng.Wd.clone(),
-                pack.grad[eng.dense_off:].clone(), eng.dW32.clone()]
-
-    def fused(mu):
-        pack.flat.copy_(flat0); eng.after_restore(); eng.dW32.copy_(dW); pack.grad.copy_(grad)
-        m, v = m0.clone(), v0.clone()
-        ops.fused_update(eng.dW32, eng.table, pack.flat, pack.grad, m, v, eng.shadow, eng.Wf, eng.Wd, step, lr_scale,
-                         1e-3, 1e-4, 0.9, 0.999, 1e-7, eng.dense_off, nt, anchor, mu)
-        torch.cuda.synchronize()
-        return state(m, v)
-
-    def separate(mu):
-        pack.flat.copy_(flat0); eng.after_restore(); eng.dW32.copy_(dW); pack.grad.copy_(grad)
-        m, v = m0.clone(), v0.clone()
-        ops.conv_grad_finalize(eng.dW32, eng.table, pack.grad)
-        ops.adam_step_(pack.trainable(), pack.grad, m, v, eng.shadow, step, lr_scale, 1e-3, 1e-4, 0.9, 0.999, 1e-7,
-                       anchor, mu)
-        ops.conv_weight_relayout(eng.shadow, eng.table, eng.Wf, eng.Wd, 0, -1, False)
-        torch.cuda.synchronize()
-        return state(m, v)
-
-    # The two kernels evaluate the same Adam expressions, but nvcc contracts them into FMAs differently (m and v of
-    # adam_kernel<false> and fused_update_kernel<false> already differ that way, unchanged by the FedProx template),
-    # so the fp32 results may differ in the last bit or two and a bf16 copy may round to the neighbouring value.
-    # An m that cancels (beta1*m ~ -(1-beta1)*g) keeps the absolute error of its ~1e-3 terms, hence the floors.
-    # Measured on H100s: max |diff| 0 or flat 7.5e-9, m 4.7e-10, v 7.3e-12, bf16 copies 0, with mu = 0.05 and 0.
-    names = ["flat", "m", "v", "shadow", "Wf", "Wd", "grad", "dW32"]
-    for mu in (0.05, 0.0):
-        a, b = fused(mu), separate(mu)
-        diffs = {k: float((x.float() - y.float()).abs().max()) for k, x, y in zip(names, a, b)}
-        print(f"mu={mu}: fused vs separate max |diff|", diffs)
-        # one bf16 ulp, or a few fp32 ulps; floors: 1e-6 of an Adam step (~lr) for the weights, ~8 ulps of the
-        # terms of m and v
-        floor = {"flat": 1e-9, "m": 1e-9, "v": 1e-13}
-        for k, x, y in zip(names, a, b):
-            x, y = x.float(), y.float()
-            ulps = 2.0 ** -7 if k in ("shadow", "Wf", "Wd") else 2.0 ** -21
-            tol = ulps * torch.maximum(x.abs(), y.abs()) + floor.get(k, 0.0)
-            assert bool(((x - y).abs() <= tol).all()), (k, diffs)
-    moved = (fused(0.05)[0] - fused(0.0)[0]).abs().max()
-    assert float(moved) > 1e-6                         # the proximal term itself is far above that rounding
-
-
-# ------------------------------------------------------------------ 3. the engine with FedProx
+# ------------------------------------------------------------------ 2. the engine with FedProx
 def _setup(backend, dtype, use_graph, mu, n_img=256, seed=5):
     from hefl_b200.config import FLConfig
     from hefl_b200.fl.data import BatchFeeder, SyntheticImageDataset
@@ -211,7 +138,7 @@ def test_proximal_term_pulls_towards_the_anchor():
     assert dist[1.0] < dist[0.0]
 
 
-# ------------------------------------------------------------------ 4. sample-weighted encrypted FedAvg on CUDA
+# ------------------------------------------------------------------ 3. sample-weighted encrypted FedAvg on CUDA
 def test_simulated_noniid_clients_on_cuda():
     from hefl_b200.config import FLConfig
     from hefl_b200.fl import simulate_clients
@@ -226,7 +153,7 @@ def test_simulated_noniid_clients_on_cuda():
     assert r["max_abs_err"] < 1e-6
 
 
-# ------------------------------------------------------------------ 5. two GPUs
+# ------------------------------------------------------------------ 4. two GPUs
 @pytest.mark.multigpu
 def test_noniid_round_across_two_gpus():
     if torch.cuda.device_count() < 2:

@@ -28,6 +28,16 @@ def _setup(backend, dtype, use_graph, n_img=256, seed=5):
     return tr, pack, feed
 
 
+def _layouts_follow_weights(tr):
+    """After the update (the layers above layer 1 on the side stream, layer 1 in the tail), the bf16 shadow and both
+    tensor-core weight layouts hold exactly the fp32 weights."""
+    eng = tr.engine
+    assert torch.equal(eng.shadow, tr.pack.trainable().to(torch.bfloat16))
+    Wf, Wd = torch.zeros_like(eng.Wf), torch.zeros_like(eng.Wd)
+    tr.ops.conv_weight_relayout(eng.shadow, eng.table, Wf, Wd, 0, -1, eng.spack0, eng.compact0)
+    assert torch.equal(eng.Wf, Wf) and torch.equal(eng.Wd, Wd)
+
+
 def test_three_epochs_of_the_bf16_engine_track_fp32_pytorch():
     eng, pack_e, feed_e = _setup("tcgen05", "bf16", True)
     ref, pack_r, feed_r = _setup("cudnn", "fp32", False)
@@ -60,6 +70,8 @@ def test_graph_and_pipeline_path_equals_the_eager_path_over_eight_steps():
     b.fit(feed_b, None, 1, early_stopping=None, reduce_lr_patience=None)
     torch.cuda.synchronize()
     assert int(a.step_t.item()) == int(b.step_t.item()) == 8
+    _layouts_follow_weights(a)
+    _layouts_follow_weights(b)
     # same kernels, same order of operations; only the fp32 atomics of the weight gradients reorder. Adam moves
     # every weight by ~lr per step whatever the size of its gradient, so a weight whose gradient is pure rounding
     # noise may drift by up to steps * lr = 8e-3 in EACH run, in opposite directions in the worst case (observed

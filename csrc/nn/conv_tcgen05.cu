@@ -20,7 +20,8 @@
 //
 // Warp roles: eight compute warps (mma.sync with fp32 accumulators in registers, then the epilogue), one TMA
 // producer warp; a smem ring of halo tiles with full/empty mbarriers lets TMA fill tile i+1 while tile i is
-// multiplied. Weights for all 9 taps stay resident in shared memory for the CTA's lifetime.
+// multiplied (the tap-GEMM's compute warps are two groups of four that take alternate tiles, so one group's epilogue
+// runs under the other's MMAs). Weights for all 9 taps stay resident in shared memory for the CTA's lifetime.
 #include <cuda_bf16.h>
 
 #include <stdexcept>
@@ -121,21 +122,31 @@ struct TapGemmCfg {
   static constexpr int BAR_BYTES = 384;
   static constexpr int SCR_BYTES = 8 * 1024;              // 1 KB accumulator staging per compute warp
   static constexpr int FIXED = W_BYTES + BAR_BYTES + SCR_BYTES + 1024;
-  static constexpr int NBUF_RAW = (kSmemMax - FIXED) / HALO;
-  // a ring deeper than 2 halo tiles measured no gain; the second tile overlaps TMA with the MMAs
-  static constexpr int NBUF = NBUF_RAW > 2 ? 2 : NBUF_RAW;
+  // 8-channel chunks per warp and pass: accumulators = NACC x NCH x 2 m16 tiles x 4 floats = 64 registers or fewer
+  static constexpr int NCH = (CO / 8) < (8 / NACC) ? (CO / 8) : (8 / NACC);
+  static constexpr int NPASS = CO / 8 / NCH;
+  static constexpr int ACC_REGS = NACC * NCH * 8;
+  // Two CTAs per SM when a two-tile ring fits twice and the accumulators leave room in the 96 registers a thread
+  // then gets (64 accumulators spill there); otherwise one CTA per SM. The ring takes what the CTA's share of shared
+  // memory holds, up to 4 tiles. Two consumer groups need a ring of at least 2 (one tile per group in flight); a ring
+  // of 1 leaves one group.
+  static constexpr int OCC = blocks_fit(FIXED + 2 * HALO, 2) && ACC_REGS <= 32 ? 2 : 1;
+  static constexpr int SMEM_CAP = OCC == 2 ? 228 * 1024 / 2 - 1024 : kSmemMax;
+  static constexpr int NBUF_FIT = (SMEM_CAP - FIXED) / HALO;
+  static constexpr int NBUF = NBUF_FIT > 4 ? 4 : NBUF_FIT;
   static constexpr int SMEM = FIXED + NBUF * HALO;
-  // 8-channel chunks per warp and pass: accumulators = NACC x NG x 2 m16 tiles x 4 floats = 64 registers or fewer
-  static constexpr int NG = (CO / 16) < (8 / NACC) ? (CO / 16) : (8 / NACC);
-  static constexpr int OCC = blocks_fit(SMEM, 2) ? 2 : 1;
+  static constexpr int NGRP = NBUF >= 2 ? 2 : 1;
   static_assert(NBUF >= 1, "halo tile does not fit in shared memory");
-  static_assert(NG % 2 == 0 && (CO / 16) % NG == 0, "chunk groups");
+  static_assert(blocks_fit(SMEM, OCC), "occupancy");
+  static_assert(NCH % 2 == 0 && (CO / 8) % NCH == 0, "chunk passes");
   static_assert(CO % 32 == 0 && CO <= 128, "CO must be 32, 64, 96 or 128");
 };
 
-// Warp roles: warps 0..7 compute and run the epilogue (warp w owns GEMM rows 32*(w%4) .. +31 and the 8-channel
-// chunks w/4, w/4 + 2, ...), warp 8 is the TMA producer. Accumulators live in registers (mma.sync m16n8k16); the
-// halo ring of NBUF tiles lets TMA fill tile i+1 while tile i is multiplied.
+// Warp roles (DESIGN.md §4): warps 0..7 are two consumer groups of four; group w/4 takes the CTA's tiles k = w/4,
+// w/4 + 2, ... and warp w owns GEMM rows 32*(w%4) .. +31 and all CO channels of the column block (NPASS passes of NCH
+// 8-channel chunks). The groups hand the MMA loop to each other in tile order (named barriers 1 and 2), so one
+// group's epilogue runs under the other group's MMAs and the two groups stay within one tile of each other. Warp 8 is
+// the TMA producer and fills the ring in tile order. Accumulators live in registers (mma.sync m16n8k16).
 template <int CK, int CO, bool POOL, int TS>
 __global__ void __launch_bounds__(288, TapGemmCfg<CK, CO, POOL, TS>::OCC)
 tap_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmW,
@@ -158,7 +169,7 @@ tap_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
   if (warp == 8 && lane == 0) {
     prefetch_tmap(&tmA);
     prefetch_tmap(&tmW);
-    for (int s = 0; s < Cfg::NBUF; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 8); }
+    for (int s = 0; s < Cfg::NBUF; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 4); }
     mbar_init(wfull, 1);
     fence_barrier_init();
   }
@@ -220,70 +231,48 @@ tap_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
       }
     }
   } else {
-    // ===== compute + epilogue warps (0..7): rows qd*32 .. +31, channel chunks grp, grp + 2, ...
+    // ===== consumer group grp (warps 4*grp .. +3): tiles kt = grp, grp + NGRP, ...; rows qd*32 .. +31, all channels
     const int qd = warp & 3;
     const int grp = warp >> 2;
+    if (grp >= Cfg::NGRP) return;
     float* scr = scr_all + warp * 256;
     const uint32_t w_base = smem_u32(sW);
     mbar_wait(wfull, 0);
-    int buf = 0;
-    uint32_t phase = 0;
-    for (int t = blockIdx.x; t < a.num_tiles; t += gridDim.x) {
-      mbar_wait(&full[buf], phase);
+    for (int kt = grp, t = blockIdx.x + grp * gridDim.x; t < a.num_tiles; kt += Cfg::NGRP, t += Cfg::NGRP * gridDim.x) {
+      const int buf = kt % Cfg::NBUF;
+      mbar_wait(&full[buf], (kt / Cfg::NBUF) & 1);
       const uint32_t a_base = smem_u32(sA + buf * Cfg::HALO);
-      // POOL: pooled pixel of this lane's conv column (window = this lane and lane ^ 1) and whether it is stored
-      int pix = 0;
-      bool writer = false;
-      if (POOL) {
-        if (a.pairs_per_tile) {
-          // W even: m and w have the same parity, so lane ^ 1 is the other column of the same window
-          const int m = qd * 32 + lane;
-          const int k = fast_div(m, a.W, a.magic_w);
-          const int w = m - k * a.W;
-          const int half_h = a.H >> 1;
-          const int q = t * a.pairs_per_tile + k;
-          const int b = fast_div(q, half_h, a.magic_half_h);
-          const int hp = q - b * half_h;                      // the last pair of an image is never a pooled row
-          writer = k < a.pairs_per_tile && b < a.B && hp < a.Hp && (w >> 1) < a.Wp;
-          pix = (b * a.Hp + hp) * a.Wp + (w >> 1);
-        } else {
-          const int per_img = a.Hp * a.tiles_w;
-          const int b = fast_div(t, per_img, a.magic_per_img);
-          const int rem = t - b * per_img;
-          const int hp = fast_div(rem, a.tiles_w, a.magic_tiles_w);
-          const int tw = rem - hp * a.tiles_w;
-          const int wp = (tw * 128 + qd * 32 + lane) >> 1;   // conv-output column of this thread, halved
-          writer = wp < a.Wp;
-          pix = (b * a.Hp + hp) * a.Wp + wp;
-        }
-      }
+      // MMA turn: the CTA's tile kt starts its MMAs once tile kt-1 (the other group's) has finished its own
+      if (Cfg::NGRP == 2 && kt > 0) named_barrier_sync(1 + grp, 256);
 #pragma unroll 1
-      for (int g = 0; g < CO / 16 / Cfg::NG; ++g) {
-        float acc[Cfg::NACC][Cfg::NG][2][4];
+      for (int g = 0; g < Cfg::NPASS; ++g) {
+        float acc[Cfg::NACC][Cfg::NCH][2][4];
 #pragma unroll
         for (int j = 0; j < Cfg::NACC; ++j)
 #pragma unroll
-          for (int i = 0; i < Cfg::NG; ++i)
+          for (int i = 0; i < Cfg::NCH; ++i)
 #pragma unroll
             for (int mt = 0; mt < 2; ++mt)
 #pragma unroll
               for (int q = 0; q < 4; ++q) acc[j][i][mt][q] = 0.f;
+        // three taps per iteration (one filter row): their row shifts are constants, and the next tap's fragment loads
+        // are issued under the current tap's MMAs instead of after a loop back-edge
 #ifdef HEFL_CONV_DEBUG
         if (!(a.dbg & 2))
 #endif
-#pragma unroll 1
+#pragma unroll 3
         for (int tap = 0; tap < Cfg::NTAP; ++tap) {
           const int r = TS ? tap / (TS ? TS : 1) : 0, s = TS ? tap % (TS ? TS : 1) : 0;
           const int shift = POOL ? s : (2 - s);
 #pragma unroll
           for (int kb = 0; kb < Cfg::NKB; ++kb) {
 #pragma unroll
-            for (int k = 0; k < Cfg::KB / 16; ++k) {
-              uint32_t bf[Cfg::NG / 2][4];
+            for (int ks = 0; ks < Cfg::KB / 16; ++ks) {
+              uint32_t bf[Cfg::NCH / 2][4];
 #pragma unroll
-              for (int i = 0; i < Cfg::NG; i += 2) {
-                const int c0 = grp + 2 * (g * Cfg::NG + i);
-                ld_b_kmajor<RB>(w_base + tap * Cfg::W_TAP + kb * Cfg::W_SUB, c0 * 8, (c0 + 2) * 8, k * 32, lane,
+              for (int i = 0; i < Cfg::NCH; i += 2) {
+                const int c0 = g * Cfg::NCH + i;
+                ld_b_kmajor<RB>(w_base + tap * Cfg::W_TAP + kb * Cfg::W_SUB, c0 * 8, (c0 + 1) * 8, ks * 32, lane,
                                 bf[i / 2]);
               }
 #pragma unroll
@@ -293,22 +282,49 @@ tap_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
 #pragma unroll
                 for (int mt = 0; mt < 2; ++mt) {
                   uint32_t af[4];
-                  ld_a_kmajor<RB>(seg_base, shift + qd * 32 + mt * 16, k * 32, lane, af);
+                  ld_a_kmajor<RB>(seg_base, shift + qd * 32 + mt * 16, ks * 32, lane, af);
 #pragma unroll
-                  for (int i = 0; i < Cfg::NG; ++i)
+                  for (int i = 0; i < Cfg::NCH; ++i)
                     mma_bf16(acc[j][i][mt], af, bf[i / 2][(i & 1) * 2], bf[i / 2][(i & 1) * 2 + 1]);
                 }
               }
             }
           }
         }
-        if (g == CO / 16 / Cfg::NG - 1) {
+        if (g == Cfg::NPASS - 1) {
           __syncwarp();
           if (lane == 0) mbar_arrive(&empty[buf]);     // this warp's last read of the halo tile is done
+          if (Cfg::NGRP == 2 && t + (int)gridDim.x < a.num_tiles) named_barrier_arrive(2 - grp, 256);
+        }
+        // POOL: pooled pixel of this lane's conv column (window = this lane and lane ^ 1) and whether it is stored
+        int pix = 0;
+        bool writer = false;
+        if (POOL) {
+          if (a.pairs_per_tile) {
+            // W even: m and w have the same parity, so lane ^ 1 is the other column of the same window
+            const int m = qd * 32 + lane;
+            const int k = fast_div(m, a.W, a.magic_w);
+            const int w = m - k * a.W;
+            const int half_h = a.H >> 1;
+            const int q = t * a.pairs_per_tile + k;
+            const int b = fast_div(q, half_h, a.magic_half_h);
+            const int hp = q - b * half_h;                      // the last pair of an image is never a pooled row
+            writer = k < a.pairs_per_tile && b < a.B && hp < a.Hp && (w >> 1) < a.Wp;
+            pix = (b * a.Hp + hp) * a.Wp + (w >> 1);
+          } else {
+            const int per_img = a.Hp * a.tiles_w;
+            const int b = fast_div(t, per_img, a.magic_per_img);
+            const int rem = t - b * per_img;
+            const int hp = fast_div(rem, a.tiles_w, a.magic_tiles_w);
+            const int tw = rem - hp * a.tiles_w;
+            const int wp = (tw * 128 + qd * 32 + lane) >> 1;   // conv-output column of this thread, halved
+            writer = wp < a.Wp;
+            pix = (b * a.Hp + hp) * a.Wp + wp;
+          }
         }
 #pragma unroll
-        for (int i = 0; i < Cfg::NG; ++i) {
-          const int ch = grp + 2 * (g * Cfg::NG + i);
+        for (int i = 0; i < Cfg::NCH; ++i) {
+          const int ch = g * Cfg::NCH + i;
 #ifdef HEFL_CONV_DEBUG
           if (a.dbg & 4) continue;
 #endif
@@ -365,7 +381,6 @@ tap_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
           }
         }
       }
-      if (++buf == Cfg::NBUF) { buf = 0; phase ^= 1; }
     }
   }
 }
@@ -455,6 +470,9 @@ void conv_fwd_pool(const void* X, const void* Wf, const float* bias, void* out, 
 
 void conv_dgrad(const void* dY, const void* Wd, void* dX, int B, int H, int W, int CK, int CO, cudaStream_t st) {
   TapGemmArgs a{};
+#ifdef HEFL_CONV_DEBUG
+  a.dbg = g_dbg;
+#endif
   a.B = B; a.H = H; a.W = W;
   a.P = B * H * W;
   a.num_tiles = (a.P + 127) / 128;

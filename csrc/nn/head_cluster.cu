@@ -13,6 +13,9 @@
 //       dh2[:, own 8]                                     -> all-gather, cluster.sync
 //   P4  dW2 / db2 (own rows), dh1[:, own 16]              -> all-gather (transposed), cluster.sync
 //   P5  dW1 / db1 (own rows), dfeat[:, own 64 features]   (needs all dh1 and the W1 column slice)
+// ``depth`` says how far the backward runs: 0 eval (P3's loss only), 1 everything, and for a head-only step of
+// personalised federated learning (DESIGN.md §10) 2 = P5 without dfeat, 3 = up to P4's dW2 / db2, 4 = up to P3's
+// dW3 / db3. Every early exit follows the last cluster barrier after which no CTA writes into another's shared memory.
 // Four cluster barriers replace three kernel boundaries; nothing but parameters gradients, dfeat and the
 // two result scalars touches global memory.
 #include <cooperative_groups.h>
@@ -62,7 +65,7 @@ struct HeadClusterArgs {
   float *gW1, *gb1, *gW2, *gb2, *gW3, *gb3;
   __nv_bfloat16* dfeat;        // [B][F]
   float* out;                  // [2] loss, ncorrect
-  int B, C, train;
+  int B, C, depth;           // 0 eval, 1 full backward, 2 / 3 / 4 stop after dW1 / dW2 / dW3 (no dfeat)
 };
 
 __global__ void __launch_bounds__(hc::NT, 1) head_cluster_kernel(const HeadClusterArgs a) {
@@ -248,7 +251,7 @@ __global__ void __launch_bounds__(hc::NT, 1) head_cluster_kernel(const HeadClust
     }
   }
   __syncthreads();
-  if (!a.train) return;          // nobody writes into this CTA's shared memory after the P2 barrier
+  if (!a.depth) return;          // nobody writes into this CTA's shared memory after the P2 barrier
   if (r == 0) {
     for (int o = t; o < C * H2 + C; o += NT) {
       if (o < C * H2) {
@@ -264,6 +267,7 @@ __global__ void __launch_bounds__(hc::NT, 1) head_cluster_kernel(const HeadClust
       }
     }
   }
+  if (a.depth == 4) return;      // as above: the dh2 all-gather below is the first remote write after P2
   {
     const int b = t >> 3, jj = t & 7;
     if (b < B) {
@@ -295,6 +299,7 @@ __global__ void __launch_bounds__(hc::NT, 1) head_cluster_kernel(const HeadClust
       a.gb2[r * J2 + t] = s;
     }
   }
+  if (a.depth == 3) return;      // the dh1 all-gather below is the first remote write after the P3 barrier
   {
     const int b = t >> 3, iq = t & 7;
     if (b < B) {
@@ -343,6 +348,7 @@ __global__ void __launch_bounds__(hc::NT, 1) head_cluster_kernel(const HeadClust
       a.gb1[r * J1 + t] = s;
     }
   }
+  if (a.depth == 2) return;      // P5 reads and writes this CTA's shared memory only
   {
     const int kk = t & (KS - 1), bg = t >> 6;                   // 4 groups of 8 samples
     float acc[8];
@@ -372,10 +378,10 @@ bool head_cluster_supported(int B, int F, int H1, int H2, int C) {
 
 void head_cluster(const void* feat, const float* W1, const float* b1, const float* W2, const float* b2,
                   const float* W3, const float* b3, const int64_t* y, float* gW1, float* gb1, float* gW2, float* gb2,
-                  float* gW3, float* gb3, void* dfeat, float* out, int B, int C, int train,
+                  float* gW3, float* gb3, void* dfeat, float* out, int B, int C, int depth,
                   cudaStream_t st) {
   HeadClusterArgs a{reinterpret_cast<const __nv_bfloat16*>(feat), W1, b1, W2, b2, W3, b3, y, gW1, gb1, gW2, gb2, gW3, gb3,
-                    reinterpret_cast<__nv_bfloat16*>(dfeat), out, B, C, train};
+                    reinterpret_cast<__nv_bfloat16*>(dfeat), out, B, C, depth};
   cudaFuncSetAttribute(head_cluster_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, hc::SMEM_BYTES);
   cudaLaunchConfig_t cfg = {};
   cfg.gridDim = dim3(hc::R);

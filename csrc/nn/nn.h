@@ -32,15 +32,16 @@ int64_t conv_wgrad_ws_floats(int B, int H, int W, int CK, int Co);
 void conv_wgrad(const void* X, const void* DY, float* dW32, float* ws, int B, int H, int W, int CK, int Co,
                 cudaStream_t st);
 
-// Dense head (Flatten -> Dense/ReLU -> Dense/ReLU -> Dense -> softmax-CE) forward + backward.
+// Dense head (Flatten -> Dense/ReLU -> Dense/ReLU -> Dense -> softmax-CE) forward + backward. depth: 0 forward and
+// loss only, 1 every gradient and dfeat, 2 / 3 / 4 the gradients of the last 3 / 2 / 1 Dense layers and no dfeat.
 void head_forward_backward(const void* feat, const float* W1, const float* b1, const float* W2, const float* b2,
                            const float* W3, const float* b3, const int64_t* y, float* gW1, float* gb1, float* gW2,
                            float* gb2, float* gW3, float* gb3, void* dfeat, float* h1_buf, float* dh1_buf,
-                           float* out, int B, int F, int H1, int H2, int C, int train, cudaStream_t st);
+                           float* out, int B, int F, int H1, int H2, int C, int depth, cudaStream_t st);
 bool head_cluster_supported(int B, int F, int H1, int H2, int C);
 void head_cluster(const void* feat, const float* W1, const float* b1, const float* W2, const float* b2,
                   const float* W3, const float* b3, const int64_t* y, float* gW1, float* gb1, float* gW2, float* gb2,
-                  float* gW3, float* gb3, void* dfeat, float* out, int B, int C, int train, cudaStream_t st);
+                  float* gW3, float* gb3, void* dfeat, float* out, int B, int C, int depth, cudaStream_t st);
 bool wgrad0_gather_supported(int W, int Wp, int CK, int Ci, int Co);
 // layer-1 partials: [wgrad0_parts(B, Hp)][kWgrad0Part] floats of workspace
 constexpr int kWgrad0Part = 28 * 32;

@@ -194,10 +194,12 @@ void unpool_relu(const Tensor& g, const Tensor& amax, const Tensor& ypool, Tenso
                         (int)W, (int)Hp, (int)Wp, (int)Co, cur());
 }
 
-// flat / grad are the ParamPack buffers; offs = [W1, b1, W2, b2, W3, b3] element offsets.
+// flat / grad are the ParamPack buffers; offs = [W1, b1, W2, b2, W3, b3] element offsets. depth: 0 forward + loss,
+// 1 full backward with dfeat, 2 / 3 / 4 only the gradients of the last 3 / 2 / 1 Dense layers (a head-only step).
 void head_forward_backward(const Tensor& feat, const Tensor& flat, Tensor grad, at::IntArrayRef offs, const Tensor& y,
-                           Tensor dfeat, Tensor h1_buf, Tensor dh1_buf, Tensor out, int64_t B, int64_t F, int64_t H1, int64_t H2, int64_t C, bool train) {
+                           Tensor dfeat, Tensor h1_buf, Tensor dh1_buf, Tensor out, int64_t B, int64_t F, int64_t H1, int64_t H2, int64_t C, int64_t depth) {
   chk_bf16(feat, "feat"); chk_bf16(dfeat, "dfeat");
+  TORCH_CHECK(depth >= 0 && depth <= 4, "head depth must be 0 (eval), 1 (full backward) or 2..4 (head-only), got ", depth);
   TORCH_CHECK(offs.size() == 6, "need six parameter offsets");
   TORCH_CHECK(B <= 32 && B >= 1, "the head kernels handle up to 32 samples per step");
   TORCH_CHECK(feat.numel() == B * F && dfeat.numel() == B * F, "feat/dfeat must be [B,F]");
@@ -210,7 +212,7 @@ void head_forward_backward(const Tensor& feat, const Tensor& flat, Tensor grad, 
     // one launch on a cluster of 8 CTAs (csrc/nn/head_cluster.cu)
     hefl::nn::head_cluster(feat.data_ptr(), p + offs[0], p + offs[1], p + offs[2], p + offs[3], p + offs[4], p + offs[5],
                            y.data_ptr<int64_t>(), g + offs[0], g + offs[1], g + offs[2], g + offs[3], g + offs[4],
-                           g + offs[5], dfeat.data_ptr(), out.data_ptr<float>(), (int)B, (int)C, train ? 1 : 0, cur());
+                           g + offs[5], dfeat.data_ptr(), out.data_ptr<float>(), (int)B, (int)C, (int)depth, cur());
     return;
   }
   TORCH_CHECK(B % 2 == 0 && H2 % 4 == 0 && H1 % 4 == 0 && F % 8 == 0, "head dims must be even / multiples of 4 / 8");
@@ -218,7 +220,7 @@ void head_forward_backward(const Tensor& feat, const Tensor& flat, Tensor grad, 
                                   p + offs[5], y.data_ptr<int64_t>(), g + offs[0], g + offs[1], g + offs[2],
                                   g + offs[3], g + offs[4], g + offs[5], dfeat.data_ptr(), h1_buf.data_ptr<float>(),
                                   dh1_buf.data_ptr<float>(), out.data_ptr<float>(), (int)B, (int)F, (int)H1, (int)H2,
-                                  (int)C, train ? 1 : 0, cur());
+                                  (int)C, (int)depth, cur());
 }
 
 void conv_set_debug(int64_t mask) { hefl::nn::conv_set_debug((int)mask); }
@@ -445,7 +447,7 @@ TORCH_LIBRARY_FRAGMENT(hefl, m) {
   m.def("conv_wgrad(Tensor X, Tensor DY, Tensor(a!) dW32, int B, int H, int W, int CK, int Co) -> ()", &conv_wgrad);
   m.def("preprocess_u8(Tensor x, Tensor? theta, Tensor(a!) X, int aug_seed, Tensor? step, bool spack=False, bool compact=False) -> ()", &preprocess_u8);
   m.def("unpool_relu(Tensor g, Tensor amax, Tensor ypool, Tensor(a!) dY, int B, int H, int W, int Co) -> ()", &unpool_relu);
-  m.def("head_forward_backward(Tensor feat, Tensor flat, Tensor(a!) grad, int[] offs, Tensor y, Tensor(b!) dfeat, Tensor(c!) h1_buf, Tensor(d!) dh1_buf, Tensor(e!) out, int B, int F, int H1, int H2, int C, bool train) -> ()", &head_forward_backward);
+  m.def("head_forward_backward(Tensor feat, Tensor flat, Tensor(a!) grad, int[] offs, Tensor y, Tensor(b!) dfeat, Tensor(c!) h1_buf, Tensor(d!) dh1_buf, Tensor(e!) out, int B, int F, int H1, int H2, int C, int depth) -> ()", &head_forward_backward);
   m.def("conv_set_debug(int mask) -> ()", &conv_set_debug);
   m.def("wgrad0_gather(Tensor X, Tensor g, Tensor amax, Tensor(a!) dW32, int B, int H, int W, bool spack=False, int in_channels=3, bool compact=False) -> ()", &wgrad0_gather);
   m.def("fp8_quantize(Tensor x, Tensor(a!) q, Tensor scale, Tensor(b!) amax) -> ()", &fp8_quantize);

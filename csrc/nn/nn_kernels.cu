@@ -408,6 +408,7 @@ void conv_grad_finalize(float* dW32, const ConvLayerTable& t, float* grad, int l
 //   k2  h2, logits, loss, dlogits, dW3, db3, dh2                   1 CTA (0.3 MFLOP)
 //   k3  dW2, db2, dh1 (column slices of 16)                        grid H1/16
 //   k4  dW1, db1, dfeat (column slices of 16)                      grid F/16
+// A head-only step (depth 2 / 3 / 4, DESIGN.md §10) skips dfeat, k4, or k3 and k4 with k2's dh2.
 // ------------------------------------------------------------------------------------------
 namespace hefl {
 namespace nn {
@@ -473,7 +474,7 @@ struct HeadMidArgs {
   float *gW3, *gb3;
   float* dh2;           // [B][H2] out
   float* out;           // [2]: loss, ncorrect
-  int B, H1, H2, C, train;
+  int B, H1, H2, C, depth;
 };
 
 // k2: fc2 (each thread: 2 samples x 4 neurons, operands reused from registers), fc3, loss, dW3, dh2.
@@ -568,7 +569,7 @@ head_mid_kernel(const HeadMidArgs a) {
     }
   }
   __syncthreads();
-  if (!a.train) return;
+  if (!a.depth) return;
   for (int o = tid; o < C * H2 + C; o += nt) {                 // dW3, db3
     if (o < C * H2) {
       const int c = o / H2, j = o % H2;
@@ -582,6 +583,7 @@ head_mid_kernel(const HeadMidArgs a) {
       a.gb3[c] = acc;
     }
   }
+  if (a.depth == 4) return;
   for (int o = tid; o < B * H2; o += nt) {                     // dh2 -> global for k3
     const int b = o / H2, j = o % H2;
     float acc = 0.f;
@@ -678,7 +680,7 @@ head_fc1_bwd_kernel(const float* __restrict__ dh1, const __nv_bfloat16* __restri
     for (; b < B; ++b) a0 = fmaf(d[b * (H1 + 1) + j], fs[b * 16 + k], a0);
     if (k0 + k < F) gW1[(size_t)j * F + k0 + k] = a0 + a1;
   }
-  for (int o = tid; o < B * 16; o += nt) {
+  for (int o = tid; dfeat != nullptr && o < B * 16; o += nt) {
     const int b = o >> 4, k = o & 15;
     float a0 = 0.f, a1 = 0.f;
     int j = 0;
@@ -701,25 +703,28 @@ head_fc1_bwd_kernel(const float* __restrict__ dh1, const __nv_bfloat16* __restri
 void head_forward_backward(const void* feat, const float* W1, const float* b1, const float* W2, const float* b2,
                            const float* W3, const float* b3, const int64_t* y, float* gW1, float* gb1, float* gW2,
                            float* gb2, float* gW3, float* gb3, void* dfeat, float* h1_buf, float* dh1_buf,
-                           float* out, int B, int F, int H1, int H2, int C, int train, cudaStream_t st) {
+                           float* out, int B, int F, int H1, int H2, int C, int depth, cudaStream_t st) {
   const auto* f = reinterpret_cast<const __nv_bfloat16*>(feat);
   float* dh2_buf = dh1_buf + (size_t)B * H1;                  // scratch tail: [B][H2]
   const int smem_a = (B + 4) * (F + 1) * 4;
   cudaFuncSetAttribute(head_fc1_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_a);
   launch_pdl(head_fc1_fwd_kernel, dim3((H1 + 3) / 4), dim3(128), smem_a, st, f, W1, b1, h1_buf, B, F, H1);
-  HeadMidArgs a{h1_buf, W2, b2, W3, b3, y, gW3, gb3, dh2_buf, out, B, H1, H2, C, train};
+  HeadMidArgs a{h1_buf, W2, b2, W3, b3, y, gW3, gb3, dh2_buf, out, B, H1, H2, C, depth};
   const int smem_b = (B * (H1 + 1) + H2 * (H1 + 1) + B * (H2 + 1) + B * C + 2 * B + C * H2) * 4;
   cudaFuncSetAttribute(head_mid_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_b);
   launch_pdl(head_mid_kernel, dim3(1), dim3(256), smem_b, st, a);
   hefl::cuda::note_launch(2);
-  if (train) {
+  if (depth >= 1 && depth <= 3) {
     const int smem_c = (B * (H2 + 1) + B * 16 + H2 * 17) * 4;
     launch_pdl(head_fc2_bwd_kernel, dim3((H1 + 15) / 16), dim3(256), smem_c, st, dh2_buf, h1_buf, W2, gW2, gb2, dh1_buf, B, H1, H2);
+    hefl::cuda::note_launch();
+  }
+  if (depth == 1 || depth == 2) {
     const int smem_d = (B * (H1 + 1) + B * 16 + H1 * 17) * 4;
     cudaFuncSetAttribute(head_fc1_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_d);
     launch_pdl(head_fc1_bwd_kernel, dim3((F + 15) / 16), dim3(256), smem_d, st, dh1_buf, f, W1, gW1, gb1,
-                                                            reinterpret_cast<__nv_bfloat16*>(dfeat), B, F, H1);
-    hefl::cuda::note_launch(2);
+               depth == 1 ? reinterpret_cast<__nv_bfloat16*>(dfeat) : nullptr, B, F, H1);
+    hefl::cuda::note_launch();
   }
 }
 

@@ -12,6 +12,8 @@
     torchrun --nproc-per-node 8 -m hefl_b200 --dirichlet-alpha 0.3 --server-opt fedadam --server-lr 0.1
     # 8 clients on one GPU, half of them sampled per round (DESIGN.md §9)
     python -m hefl_b200 --clients-per-rank 8 --client-fraction 0.5 --dirichlet-alpha 0.3 --fedavg-weighting samples
+    # personalised: every client keeps its three Dense layers, 2 head-only epochs before the joint ones (DESIGN.md §10)
+    python -m hefl_b200 --clients-per-rank 8 --dirichlet-alpha 0.3 --personal-layers 3 --personal-head-epochs 2
 
 Every ``FLConfig`` field is a flag (``--local-epochs 10``) or an environment variable
 (``HEFL_LOCAL_EPOCHS=10``); the reference hard-codes all of them (FLPyfhelin.py:31-36, notebook N:24-32).
@@ -19,7 +21,8 @@ Extra flags: ``--data-dir DIR`` (the reference's ``image/Train`` layout ``DIR/<l
 its own IID contiguous shard, or with ``--dirichlet-alpha`` its label-skew part of the folder, 10 % of it validates;
 without it a synthetic set of the configured shape is used),
 ``--test-dir DIR`` (same layout; after the last round rank 0 prints the reference's four metrics — weighted
-precision / recall / F1 and accuracy, notebook N:267-270 — of the aggregated model),
+precision / recall / F1 and accuracy, notebook N:267-270 — of the aggregated model; with ``--personal-layers`` of
+rank 0's first client's personal model, named by ``"client"``),
 ``--checkpoint PATH`` (written by rank 0 after every round, resumed from if it exists),
 ``--simulate`` (all ``--clients`` in this one process through the loopback transport: the reference's own
 structure, clients as loop iterations, FLPyfhelin.py:184).
@@ -82,9 +85,10 @@ def main(argv=None) -> int:
             dist.init_process_group("nccl", device_id=device)
         else:
             dist.init_process_group("gloo")
-    from .fl.runner import check_client_options
+    from .fl.runner import check_client_options, check_personal_options
 
     check_client_options(cfg)
+    check_personal_options(cfg)
     M = cfg.clients_per_rank
     cfg.clients = world * M
     dataset = None
@@ -121,7 +125,10 @@ def main(argv=None) -> int:
         from .fl.data import ImageFolderDataset
 
         test = ImageFolderDataset(ns.test_dir, cfg.image_size, cfg.in_channels, shuffle_seed=None, pin=False)
-        print(json.dumps({"test_images": len(test), **run.evaluate(test)}))
+        if cfg.personal_layers:
+            print(json.dumps({"test_images": len(test), "client": run.client_ids[0], **run.evaluate(test, client=0)}))
+        else:
+            print(json.dumps({"test_images": len(test), **run.evaluate(test)}))
     if world > 1:
         dist.barrier()
         dist.destroy_process_group()

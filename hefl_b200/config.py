@@ -78,6 +78,9 @@ class FLConfig:
     dirichlet_alpha: float = 0.0              # 0: equal IID shards; > 0: Dirichlet(alpha) label-skew shards of one pool
     fedavg_weighting: str = "uniform"         # uniform (1/K) | samples (n_k / N, McMahan et al.'s FedAvg)
     fedprox_mu: float = 0.0                   # FedProx coefficient: local loss + (mu/2)*||w - w_global||^2; 0 = plain Adam
+    # personalised FL (DESIGN.md §10): each client keeps its trailing Dense layers; only the conv base is encrypted
+    personal_layers: int = 0                  # trailing Dense layers kept per client (medcnn: 0..3, cnn2: 0..1); 0 = FedAvg
+    personal_head_epochs: int = 0             # head-only epochs (conv base frozen, FedRep) before the local_epochs joint ones
     # server optimizer (DESIGN.md §8): the key holder steps the global model along avg - x_t, fused into the decode
     server_opt: str = "fedavg"                # fedavg (the model becomes the average) | fedavgm | fedadagrad | fedyogi | fedadam
     server_lr: float = 1.0                    # eta

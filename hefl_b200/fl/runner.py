@@ -33,6 +33,7 @@ import torch.distributed as dist
 from ..config import FLConfig
 from ..he.context import CKKSContext, CtBatch
 from ..models import ParamPack, create_model
+from ..models.cnn import MedCNN, SmallCNN
 from ..parallel import LoopbackTransport, make_transport
 from ..utils import DeviceTimer, JsonlLogger, StageTimes
 from .data import BatchFeeder, SyntheticImageDataset, dirichlet_partition, shard_range, split_train_val
@@ -70,18 +71,49 @@ def check_noniid_options(cfg: FLConfig) -> None:
         raise ValueError(f"fedavg_weighting must be one of {FEDAVG_WEIGHTINGS}, got {cfg.fedavg_weighting!r}")
 
 
+# the sequential CNNs, whose Dense layers are the tail of the parameter vector (DESIGN.md §10), and how many they have
+PERSONAL_MODELS = {"medcnn": len(MedCNN.dense_units) + 1, "cnn2": len(SmallCNN.dense_units) + 1}
+
+
+def check_personal_options(cfg: FLConfig) -> None:
+    """Reject personalisation settings the round cannot honour (they arrive from flags and environment variables)."""
+    p, e = cfg.personal_layers, cfg.personal_head_epochs
+    if not (isinstance(p, int) and p >= 0):
+        raise ValueError(f"personal_layers must be an integer >= 0 (0 = one global model), got {p!r}")
+    if not (isinstance(e, int) and e >= 0):
+        raise ValueError(f"personal_head_epochs must be an integer >= 0, got {e!r}")
+    if e > 0 and p == 0:
+        raise ValueError("personal_head_epochs > 0 trains personal layers: it needs personal_layers > 0")
+    if p == 0:
+        return
+    if cfg.model not in PERSONAL_MODELS:
+        raise ValueError(f"personal_layers needs one of the sequential CNNs {tuple(PERSONAL_MODELS)}, got model "
+                         f"{cfg.model!r} (a ResNet's fc sits between its trainable parameters and BatchNorm statistics)")
+    if p > PERSONAL_MODELS[cfg.model]:
+        raise ValueError(f"personal_layers must be at most {PERSONAL_MODELS[cfg.model]}, the Dense layers of "
+                         f"{cfg.model}, got {p}")
+    if cfg.compat_sequential_clients:
+        raise ValueError("personal_layers does not combine with compat_sequential_clients")
+
+
 class FederatedRunner:
     def __init__(self, cfg: FLConfig, rank: int = 0, world: int = 1, group=None,
                  device: Optional[torch.device] = None, samples_per_client: Optional[int] = None, dataset=None):
         check_noniid_options(cfg)
         check_server_options(cfg)
         check_client_options(cfg)
+        check_personal_options(cfg)
         self.cfg = cfg
         self.rank, self.world, self.group = rank, world, group
         self.device = device or torch.device(cfg.device if torch.cuda.is_available() or cfg.device == "cpu" else "cpu")
         torch.manual_seed(cfg.seed)                     # the reference seeds nothing (Q12)
         self.model = create_model(cfg.model, cfg.in_channels, cfg.num_classes, cfg.image_size).to(self.device)
         self.pack = ParamPack(self.model)
+        # personalisation (DESIGN.md §10): flat[:n_shared] is federated, the trailing Dense layers stay with each client;
+        # every client starts from head0, the personal layers of the seeded initial model
+        self.n_shared = self.pack.dense_tail_start(cfg.personal_layers) if cfg.personal_layers else self.pack.numel
+        self.n_personal = self.pack.numel - self.n_shared
+        self.head0 = self.pack.flat[self.n_shared:].clone() if self.n_personal else None
         self.trainer = LocalTrainer(self.model, self.pack, cfg, self.device)
         hp = cfg.he_params()
         self.ctx = CKKSContext(hp["n"], prime_bits=hp["prime_bits"], scale_bits=hp["scale_bits"],
@@ -95,7 +127,7 @@ class FederatedRunner:
             raise ValueError(f"key_holder {self.key_holder} is not a rank of this {world}-client federation")
         self.has_sk = world == 1 or self.key_holder < 0 or rank == self.key_holder
         self._setup_keys()
-        self.n_ct = self.ctx.num_ct(self.pack.numel, cfg.packing)
+        self.n_ct = self.ctx.num_ct(self.n_shared, cfg.packing)
         self.ct_numel = self.n_ct * 2 * self.ctx.L * self.ctx.n
         kind = cfg.transport
         if self.device.type == "cpu" and kind == "fused":
@@ -159,6 +191,7 @@ class FederatedRunner:
             self._c_v = torch.empty(M, n, dtype=torch.float32, device=self.device)
             self._c_step = torch.empty(M, 1, dtype=torch.int64, device=self.device)
             self._c_lr = torch.empty(M, 1, dtype=torch.float32, device=self.device)
+            self._c_head = self.head0.repeat(M, 1) if self.n_personal else None
             self._load_clients_state(None)              # every client starts fresh
         self._selected: List[int] = list(range(self.num_clients))
         self._plain_sum: Optional[torch.Tensor] = None
@@ -173,7 +206,7 @@ class FederatedRunner:
         self.global_flat = self.pack.flat.clone()       # x_t: the global model of the round, snapshot by run_round
         # server optimizer (DESIGN.md §8): the state lives with whoever decrypts -- the key holder, or every rank
         # when every rank holds sk (each then applies the same deterministic step)
-        self.server_opt = (ServerOptimizer.from_config(cfg, self.pack.n_trainable, self.device)
+        self.server_opt = (ServerOptimizer.from_config(cfg, self.pack.n_trainable - self.n_personal, self.device)
                            if cfg.server_opt != "fedavg" and self.has_sk else None)
         self._avg_out = None                  # debug_precision with a server step: the decoded average of the round
         self.history: List[Dict] = []
@@ -260,7 +293,7 @@ class FederatedRunner:
         self._clear_pending()
         self._enc_buf = self.transport.buffer(self.ct_numel)
         weighted = self.cfg.fedavg_weighting == "samples"
-        self._plain_sum = (torch.zeros(self.pack.numel, dtype=torch.float64, device=self.device)
+        self._plain_sum = (torch.zeros(self.n_shared, dtype=torch.float64, device=self.device)
                            if self.cfg.debug_precision else None)
         hists: Dict[int, list] = {}
         for j, i in enumerate(order):
@@ -270,11 +303,14 @@ class FederatedRunner:
                     if self.trainer.engine is not None:
                         self.trainer.engine.after_restore()
                 val = self._swap_in(i) if swap else self.val_feed
-                hists[i] = self.trainer.fit(self.train_feed, val, self.cfg.local_epochs, early_stopping=early_stopping)
+                head = (self.trainer.fit(self.train_feed, val, self.cfg.personal_head_epochs, head_only=True)
+                        if self.cfg.personal_head_epochs else [])
+                hists[i] = head + self.trainer.fit(self.train_feed, val, self.cfg.local_epochs,
+                                                   early_stopping=early_stopping)
                 if swap:
                     self._swap_out(i)
             if self._plain_sum is not None and self._client_takes_part(i):
-                self._plain_sum.add_(self.pack.flat.double(), alpha=self.clients[i]["n_train"] if weighted else 1)
+                self._plain_sum.add_(self.shared().double(), alpha=self.clients[i]["n_train"] if weighted else 1)
             if j + 1 < len(order):
                 with self.timer.stage("encrypt"):
                     self._accumulate(i, self._enc_buf)
@@ -297,6 +333,8 @@ class FederatedRunner:
         tr.m.copy_(self._c_m[i]); tr.v.copy_(self._c_v[i]); tr.step_t.copy_(self._c_step[i]); tr.lr_scale.copy_(self._c_lr[i])
         if tr.engine is not None:
             tr.engine.prep_count = self._c_prep[i]
+        if self.n_personal:
+            self.pack.flat[self.n_shared:].copy_(self._c_head[i])        # over the global base
         self._set_rng_state(self._c_rng[i])
         self.train_feed.retarget(c["dataset"], range(c["nval"], c["per"]), self._c_gen[i][0])
         if not c["nval"]:
@@ -309,7 +347,17 @@ class FederatedRunner:
         self._c_m[i].copy_(tr.m); self._c_v[i].copy_(tr.v); self._c_step[i].copy_(tr.step_t); self._c_lr[i].copy_(tr.lr_scale)
         if tr.engine is not None:
             self._c_prep[i] = tr.engine.prep_count
+        if self.n_personal:
+            self._c_head[i].copy_(self.pack.flat[self.n_shared:])
         self._c_rng[i] = self._rng_state()
+
+    def shared(self) -> torch.Tensor:
+        """The federated part of the installed model: all of it, or the base before the personal layers."""
+        return self.pack.flat[: self.n_shared]
+
+    def _install_shared(self, vec: torch.Tensor) -> None:
+        """Install the new global model (the federated part only: personal layers stay as they are)."""
+        self.shared().copy_(vec.to(self.pack.flat.device, torch.float32).reshape(-1)[: self.n_shared])
 
     def _client_takes_part(self, i: int) -> bool:
         p = self.participating
@@ -321,7 +369,7 @@ class FederatedRunner:
         self._agree_on_participants()
         if not self._client_takes_part(i):
             return
-        self.ctx.encrypt(self.pack.flat, self.pk, seed=self._encrypt_seed(self.client_ids[i]), packing=self.cfg.packing,
+        self.ctx.encrypt(self.shared(), self.pk, seed=self._encrypt_seed(self.client_ids[i]), packing=self.cfg.packing,
                          out=buf, weight=self.fedavg_weight(i), accumulate=self._enc_count > 0)
         self._enc_count += 1
 
@@ -386,10 +434,10 @@ class FederatedRunner:
         last, acc = self._last_client, self._enc_count > 0
         self._clear_pending()
         if last is not None and self._client_takes_part(last):
-            return buf, self.pack.flat, self.fedavg_weight(last), self._encrypt_seed(self.client_ids[last]), acc
+            return buf, self.shared(), self.fedavg_weight(last), self._encrypt_seed(self.client_ids[last]), acc
         if acc:
             return buf, None, 1.0, 0, True
-        return buf, torch.zeros_like(self.pack.flat), 1.0, self._encrypt_seed(self.num_clients + self.rank), False
+        return buf, torch.zeros_like(self.shared()), 1.0, self._encrypt_seed(self.num_clients + self.rank), False
 
     def encrypt_update(self) -> CtBatch:
         """The rank's ciphertext of the round: the last trained client added into the buffer its co-located clients
@@ -400,7 +448,7 @@ class FederatedRunner:
                 self.ctx.encrypt(flat, self.pk, seed=seed, packing=self.cfg.packing, out=buf, weight=weight,
                                  accumulate=acc)
             ct = CtBatch(buf[: self.ct_numel].view(self.n_ct, 2, self.ctx.L, self.ctx.n), self.ctx.scale,
-                         self.pack.numel, self.cfg.packing)
+                         self.n_shared, self.cfg.packing)
             self._mask(ct.data)
             return ct
 
@@ -416,18 +464,19 @@ class FederatedRunner:
                 return
             if self.server_opt is not None:
                 # x_{t+1} = step(x_t, average): decoded and stepped in one launch, broadcast where the average was
-                avg = torch.empty_like(self.pack.flat)
-                self.server_opt.step(self.ctx, agg, self.sk, float(k), self.global_flat, avg, avg_out=self._avg_out)
+                avg = torch.empty_like(self.shared())
+                self.server_opt.step(self.ctx, agg, self.sk, float(k), self.global_flat[: self.n_shared], avg,
+                                     avg_out=self._avg_out)
             elif self.has_sk:
                 avg = self.ctx.decrypt(agg, self.sk, divide_by=float(k))
             else:
-                avg = torch.empty_like(self.pack.flat)
+                avg = torch.empty_like(self.shared())
             if self.key_holder >= 0:
                 avg = avg.to(self.pack.flat.dtype).contiguous()
                 dist.broadcast(avg, src=self.key_holder, group=self.group)
                 if self._avg_out is not None:
                     dist.broadcast(self._avg_out, src=self.key_holder, group=self.group)
-            self.pack.load_flat(avg)
+            self._install_shared(avg)
             if self.trainer.engine is not None:
                 self.trainer.engine.after_restore()
 
@@ -443,7 +492,7 @@ class FederatedRunner:
         per_ct = 2 * ctx.L * ctx.n
         # the rank's other clients are already in the buffer; the last one is encrypted chunk by chunk into it
         buf, flat, weight, seed, acc = self._rank_update()
-        out = torch.empty_like(self.pack.flat)
+        out = torch.empty_like(self.shared())
         k = self._contributors()
         if k == 0:
             return
@@ -487,7 +536,7 @@ class FederatedRunner:
             chunks = [(c0, min(n_ct, c0 + chunk_cts)) for c0 in range(0, n_ct, chunk_cts)]
             t_origin = mark(cur) if timeline is not None else None
             for ci, (c0, c1) in enumerate(chunks):
-                nv = min(self.pack.numel, c1 * vpc) - c0 * vpc
+                nv = min(self.n_shared, c1 * vpc) - c0 * vpc
                 view = buf[c0 * per_ct: c1 * per_ct]
                 rec = {"chunk": ci}
                 with torch.cuda.stream(s_enc):
@@ -512,7 +561,7 @@ class FederatedRunner:
                         rec["dec0"] = mark(s_dec)
                     if self.server_opt is not None:
                         self.server_opt.step(ctx, CtBatch(data, ct.scale, ct.nvals, ct.packing), self.sk, k,
-                                             self.global_flat, out, offset=c0 * vpc, avg_out=self._avg_out)
+                                             self.global_flat[: self.n_shared], out, offset=c0 * vpc, avg_out=self._avg_out)
                     elif self.has_sk:
                         avg = ctx.decrypt(CtBatch(data, ct.scale, ct.nvals, ct.packing), self.sk, divide_by=k)
                         out[c0 * vpc: c0 * vpc + avg.numel()].copy_(avg)
@@ -539,7 +588,7 @@ class FederatedRunner:
                 dist.broadcast(out, src=self.key_holder, group=self.group)
                 if self._avg_out is not None:
                     dist.broadcast(self._avg_out, src=self.key_holder, group=self.group)
-            self.pack.load_flat(out)
+            self._install_shared(out)
 
     def guard_finite(self) -> None:
         """NaN/Inf guard on decoded weights (failure detection, SURVEY.md §5.3)."""
@@ -555,7 +604,7 @@ class FederatedRunner:
         # in-process loopback federation of several ranks has no process group to sum them over.
         oracle = self.cfg.debug_precision and (self.world == 1 or not isinstance(self.transport, LoopbackTransport))
         # with a server step the error is the decoded average's, not the stepped model's: the decode also writes it here
-        self._avg_out = torch.empty_like(self.pack.flat) if oracle and self.cfg.server_opt != "fedavg" else None
+        self._avg_out = torch.empty_like(self.shared()) if oracle and self.cfg.server_opt != "fedavg" else None
         if pipelined is None:
             pipelined = self.device.type == "cuda" and self.n_ct > 512 and self.transport.name in ("fused", "nccl", "gloo")
         if pipelined:
@@ -579,6 +628,8 @@ class FederatedRunner:
                "transport": self.transport.name, "n_ct": self.n_ct, "ct_bytes": self.ct_numel * 8,
                "n_train": self.n_train, "fedavg_weight": self.fedavg_weight(), "label_counts": self.label_counts,
                "server_opt": self.cfg.server_opt}
+        if self.n_personal:                          # the personal model on the client's own held-out 10 %
+            rec["val_accuracy"] = hist[-1].val_accuracy if hist else None
         if self.clients_per_rank > 1 or self.cfg.client_fraction < 1:
             rec.update(self._client_records(hists))
         if oracle:
@@ -586,7 +637,7 @@ class FederatedRunner:
                 dist.all_reduce(self._plain_sum, op=dist.ReduceOp.SUM, group=self.group)
             kk = self._n_total if self._n_total is not None else self._contributors()
             if kk > 0:
-                avg = self._avg_out if self._avg_out is not None else self.pack.flat
+                avg = self._avg_out if self._avg_out is not None else self.shared()
                 err = float((avg.double() - self._plain_sum / kk).abs().max())
                 rec["ckks_max_abs_err"] = err
                 rec["ckks_precision_bits"] = float(-math.log2(err)) if err > 0 else float("inf")
@@ -606,12 +657,16 @@ class FederatedRunner:
             clients.append({"id": c["id"], "n_train": c["n_train"], "fedavg_weight": w,
                             "loss": h[-1].loss if h else None, "accuracy": h[-1].accuracy if h else None,
                             "label_counts": c["label_counts"]})
+            if self.n_personal:
+                clients[-1]["val_accuracy"] = h[-1].val_accuracy if h else None
             if self._client_takes_part(i):
                 n_sum, w_sum = n_sum + c["n_train"], w_sum + w
                 counts = [a + b for a, b in zip(counts, c["label_counts"])]
         scored = [(c["n_train"], c) for c in clients if c["loss"] is not None]
         tot = sum(n for n, _ in scored)
-        return {"loss": sum(n * c["loss"] for n, c in scored) / tot if tot else None,
+        personal = {"val_accuracy": sum(n * c["val_accuracy"] for n, c in scored) / tot if tot else None} \
+            if self.n_personal else {}
+        return {**personal,"loss": sum(n * c["loss"] for n, c in scored) / tot if tot else None,
                 "accuracy": sum(n * c["accuracy"] for n, c in scored) / tot if tot else None,
                 "n_train": n_sum, "fedavg_weight": w_sum, "label_counts": counts,
                 "selected": list(self._selected), "clients": clients}
@@ -641,10 +696,21 @@ class FederatedRunner:
 
     # ------------------------------------------------------------------ evaluation (notebook N:262-270)
     @torch.no_grad()
-    def evaluate(self, dataset, batch_size: Optional[int] = None) -> Dict[str, float]:
+    def evaluate(self, dataset, batch_size: Optional[int] = None, client: Optional[int] = None) -> Dict[str, float]:
         """Weighted precision / recall / F1 and accuracy of the current global model on ``dataset`` — the four
         numbers the reference's notebook reports after aggregation (sklearn ``average='weighted'``, N:267-270).
-        Runs the plain PyTorch forward of the model (any backend / device); not a hot path."""
+        Runs the plain PyTorch forward of the model (any backend / device); not a hot path. ``client``: a local slot
+        whose personal layers are installed for the evaluation (the installed ones are restored afterwards); None
+        scores the installed model."""
+        if client is not None and not 0 <= client < self.clients_per_rank:
+            raise ValueError(f"client slot {client} is not one of this rank's {self.clients_per_rank}")
+        if client is not None and self.n_personal and self.clients_per_rank > 1:
+            saved = self.pack.flat[self.n_shared:].clone()
+            self.pack.flat[self.n_shared:].copy_(self._c_head[client])
+            try:
+                return self.evaluate(dataset, batch_size)
+            finally:
+                self.pack.flat[self.n_shared:].copy_(saved)
         bs = batch_size or self.cfg.batch_size
         self.model.eval()
         preds = []
@@ -661,13 +727,29 @@ class FederatedRunner:
         feeders' shuffle generators and, with several clients per rank, every client's state (``path.rank{r}``) so
         that a resumed multi-round run equals an uninterrupted one (SURVEY.md §5.4)."""
         if self.rank == 0:
-            torch.save({"round": self.round, "flat": self.pack.flat.detach().cpu(), "config": self.cfg.to_json()}, path)
+            flat = self.pack.flat.detach().cpu()
+            if self.n_personal:                      # the global file holds no client's personal layers
+                flat = torch.cat([flat[: self.n_shared], self.head0.cpu()])
+            torch.save({"round": self.round, "flat": flat, "config": self.cfg.to_json()}, path)
         torch.save({"round": self.round, "opt": self.trainer.state_dict(), "rng": torch.get_rng_state(),
                     "cuda_rng": torch.cuda.get_rng_state(self.device) if self.device.type == "cuda" else None,
                     "feeds": [f.gen.get_state() if f is not None else None for f in (self.train_feed, self.val_feed)],
                     "server": self.server_opt.state_dict() if self.server_opt is not None else None,
-                    "clients": self._clients_state() if self.clients_per_rank > 1 else None},
+                    "clients": self._clients_state() if self.clients_per_rank > 1 else None,
+                    "heads": {"ids": torch.tensor(self.client_ids), "head": self._heads().cpu()} if self.n_personal else None},
                    f"{path}.rank{self.rank}")
+
+    def _heads(self) -> torch.Tensor:
+        """[M, n_personal]: every client's personal layers (a one-client rank's are the installed ones)."""
+        return self._c_head if self.clients_per_rank > 1 else self.pack.flat[self.n_shared:].unsqueeze(0)
+
+    def _load_heads(self, st: Optional[Dict]) -> None:
+        """The clients' personal layers from a rank file, or head0 for every client when it holds none of them."""
+        if not self.n_personal:
+            return
+        mine = st is not None and st["ids"].tolist() == self.client_ids
+        heads = st["head"].to(self.device) if mine else self.head0.expand(self.clients_per_rank, -1)
+        self._heads().copy_(heads)
 
     def _clients_state(self) -> Dict:
         """Every client's persistent state (several clients per rank): optimiser, augmentation position, shuffle
@@ -718,6 +800,7 @@ class FederatedRunner:
                     f.gen.set_state(gs)
             if self.clients_per_rank > 1:
                 self._load_clients_state(st.get("clients"))
+            self._load_heads(st.get("heads"))
             if self.server_opt is not None:          # the server state sits in the key holder's own file
                 if st.get("server") is not None:
                     self.server_opt.load_state_dict(st["server"])
@@ -727,6 +810,7 @@ class FederatedRunner:
             self.trainer.reset_optimizer()
             if self.clients_per_rank > 1:
                 self._load_clients_state(None)
+            self._load_heads(None)
             if self.server_opt is not None:
                 self.server_opt.reset()
         if self.trainer.engine is not None:
@@ -764,6 +848,9 @@ def simulate_clients(cfg: FLConfig, device: Optional[torch.device] = None, round
     ``encrypted_avg`` / ``plain_avg`` / ``max_abs_err`` keep describing the average."""
     check_noniid_options(cfg)
     check_server_options(cfg)
+    if cfg.personal_layers or cfg.personal_head_epochs:
+        raise ValueError("simulate_clients averages one global model: personal_layers / personal_head_epochs need "
+                         "FederatedRunner")
     device = device or torch.device("cpu")
     torch.manual_seed(cfg.seed)
     hp = cfg.he_params()

@@ -63,6 +63,8 @@ class LocalTrainer:
         # to the gradient. Allocated once, so captured graphs keep a valid pointer to it.
         self.mu = float(cfg.fedprox_mu)
         self.anchor = torch.zeros(n, dtype=torch.float32, device=device) if self.mu > 0 else None
+        # personal layers (DESIGN.md §10): a head-only step updates flat[head_lo:n]
+        self.head_lo = pack.dense_tail_start(cfg.personal_layers) if cfg.personal_layers else n
         # "fp8": bf16 autocast + e4m3 GEMMs for the 1x1 convolutions of the ResNets (ops/fp8.py)
         self.amp_dtype = {"bf16": torch.bfloat16, "fp16": torch.float16, "fp32": torch.float32,
                           "fp8": torch.bfloat16}[cfg.dtype]
@@ -77,6 +79,7 @@ class LocalTrainer:
         self._graph_train: Optional[torch.cuda.CUDAGraph] = None
         self._graph_eval: Optional[torch.cuda.CUDAGraph] = None
         self.graph_launches = [0, 0]      # our kernels inside one train / eval graph
+        self.head_launches = 0            # ... inside one head-only graph (captured by the first head-only fit)
         self.replayed_launches = 0        # ... summed over replays (bench.py gpu_launches)
         self.engine = None
         if self.backend == "cudnn" and self.cuda:
@@ -133,6 +136,40 @@ class LocalTrainer:
         self.out_train[0] = loss.detach()
         self.out_train[1] = (logits.argmax(1) == y).sum()
         self._optimizer_step()
+
+    def _head_eager(self, x_u8: torch.Tensor, y: torch.Tensor) -> None:
+        """Head-only step: the same augmented batch as a train step, the frozen layers under no_grad, Adam over the
+        personal layers alone."""
+        if self.engine is not None:
+            self.engine.preprocess(x_u8, 0, True, self.augment)
+            self.engine.head_step_staged(0, y, self.out_train, opt=self)
+            return
+        fcs = self.model.fcs
+        shared = len(fcs) - self.cfg.personal_layers
+        amp = self.amp_dtype != torch.float32 and self.cuda
+        with torch.autocast("cuda", dtype=self.amp_dtype, enabled=amp):
+            with torch.no_grad():
+                x = self.model.features(self._prep(x_u8, True)).permute(0, 2, 3, 1).flatten(1)   # Keras Flatten
+                for fc in fcs[:shared]:
+                    x = F.relu(fc(x))
+            for j in range(shared, len(fcs)):
+                x = fcs[j](x)
+                if j + 1 < len(fcs):
+                    x = F.relu(x)
+        logits = x.float()
+        loss = F.cross_entropy(logits, y)
+        loss.backward()
+        self.out_train[0] = loss.detach()
+        self.out_train[1] = (logits.argmax(1) == y).sum()
+        c = self.cfg
+        lo, hi = self.head_lo, self.pack.n_trainable
+        self.step_t += 1
+        self.ops.adam_step_(self.pack.trainable()[lo:hi], self.pack.grad[lo:hi], self.m[lo:hi], self.v[lo:hi], None,
+                            self.step_t, self.lr_scale, c.lr, c.lr_decay, 0.9, 0.999, 1e-7,
+                            self.anchor[lo:hi] if self.anchor is not None else None, self.mu)
+
+    def _head_staged(self, slot: int) -> None:
+        self.engine.head_step_staged(slot, self.static_y2[slot], self.out_train2[slot], opt=self)
 
     def _train_staged(self, slot: int) -> None:
         """Graph body of the tcgen05 engine: forward/backward on the pre-processed batch of ``slot`` + update."""
@@ -220,6 +257,37 @@ class LocalTrainer:
             self.engine.after_restore()
         torch.cuda.synchronize(self.device)
 
+    def _capture_head(self) -> None:
+        """Head-only graphs of the tcgen05 engine, one per input slot, captured by the first head-only fit only, so a
+        run without head epochs captures exactly the train / eval graphs."""
+        if not self._graphs:
+            self._capture()
+        eng, cur = self.engine, torch.cuda.current_stream(self.device)
+        snap = (self.pack.flat.clone(), self.m.clone(), self.v.clone(), self.step_t.clone())
+        side = torch.cuda.Stream(self.device)
+        side.wait_stream(cur)
+        side.wait_stream(self.prep_stream)
+        with torch.cuda.stream(side):
+            for slot in range(2):
+                eng.preprocess(self.static_x, slot, False, False)
+            for _ in range(3):
+                for slot in range(2):
+                    self._head_staged(slot)
+        cur.wait_stream(side)
+        torch.cuda.synchronize(self.device)
+        for slot in range(2):
+            a = int(self.ops.launch_count())
+            g = torch.cuda.CUDAGraph()
+            with torch.cuda.graph(g):
+                self._head_staged(slot)
+            self._graphs[("head", slot)] = g
+            if slot == 0:
+                self.head_launches = int(self.ops.launch_count()) - a + 1       # + the pre-process launch
+        self.pack.flat.copy_(snap[0]); self.m.copy_(snap[1]); self.v.copy_(snap[2]); self.step_t.copy_(snap[3])
+        self.pack.grad.zero_()
+        eng.after_restore()
+        torch.cuda.synchronize(self.device)
+
     # ------------------------------------------------------------------ public API
     def prepare(self) -> None:
         """Capture the CUDA graphs now rather than at the first step (a rank with several clients captures once,
@@ -244,6 +312,20 @@ class LocalTrainer:
             self._train_eager(x_u8, y)
         return self.out_train
 
+    def head_step(self, x_u8: torch.Tensor, y: torch.Tensor) -> torch.Tensor:
+        """One head-only step (personal layers only, conv base frozen). Graph-replayed on the tcgen05 engine; eager
+        on the autograd backends. Returns a device tensor [loss, ncorrect]."""
+        if self.use_graph and self.engine is not None:
+            if ("head", 0) not in self._graphs:
+                self._capture_head()
+            self.engine.preprocess(x_u8, 0, True, self.augment)
+            self.static_y2[0].copy_(y, non_blocking=True)
+            self._graphs[("head", 0)].replay()
+            self.replayed_launches += self.head_launches
+            return self.out_train2[0]
+        self._head_eager(x_u8, y)
+        return self.out_train
+
     def eval_step(self, x_u8: torch.Tensor, y: torch.Tensor) -> torch.Tensor:
         if self.use_graph:
             if self._graph_eval is None:
@@ -260,21 +342,24 @@ class LocalTrainer:
             self._eval_eager(x_u8, y)
         return self.out_eval
 
-    def _run_epoch(self, feeder, train: bool, stats: torch.Tensor, nxt=None) -> None:
+    def _run_epoch(self, feeder, train: bool, stats: torch.Tensor, nxt=None, head: bool = False) -> None:
         """One pass over ``feeder``; per-step [loss, ncorrect] land in ``stats`` (pinned host rows).
 
         tcgen05 engine + CUDA graphs: software pipeline over batches — batch i+1 is fetched (H2D or
         on-device gather) and pre-processed into the other X0 slot on ``prep_stream`` while the captured
         graph of step i runs on the main stream; events hand the slots back and forth. ``nxt`` =
         (feeder, train) of the pass that follows: its first batch is staged under this pass's last
-        step, so consecutive passes (train -> validation -> next epoch) have no pipeline-fill bubble."""
+        step, so consecutive passes (train -> validation -> next epoch) have no pipeline-fill bubble. ``head``: a
+        training pass of head-only steps (pre-processed and staged as a train pass)."""
         if self.engine is None or not self.use_graph:
             for i, (x, y) in enumerate(feeder.epoch()):
-                out = self.train_step(x, y) if train else self.eval_step(x, y)
+                out = self.head_step(x, y) if head else self.train_step(x, y) if train else self.eval_step(x, y)
                 stats[i].copy_(out, non_blocking=True)       # D2H of the step's loss/accuracy
             return
         if not self._graphs:
             self._capture()
+        if head and ("head", 0) not in self._graphs:
+            self._capture_head()
         main, prep, sst = torch.cuda.current_stream(self.device), self.prep_stream, self.stats_stream
         n = feeder.steps
         outs = self.out_train2 if train else self.out_eval2
@@ -308,13 +393,13 @@ class LocalTrainer:
                 self._pre = (nxt[0], nxt[1], nit, slot ^ 1)
             main.wait_event(self._slot_ready[slot])
             main.wait_event(self._stats_done[slot])           # result buffer of this slot has been read back
-            self._graphs[(train, slot)].replay()
+            self._graphs[("head" if head else train, slot)].replay()
             self._slot_free[slot].record(main)
             with torch.cuda.stream(sst):                      # D2H of the step's loss/accuracy, off the main stream
                 sst.wait_event(self._slot_free[slot])
                 stats[i].copy_(outs[slot], non_blocking=True)
                 self._stats_done[slot].record(sst)
-        self.replayed_launches += n * self.graph_launches[0 if train else 1]
+        self.replayed_launches += n * (self.head_launches if head else self.graph_launches[0 if train else 1])
         with torch.cuda.stream(prep):
             for _ in it:                                      # let the feeder finish its bookkeeping
                 pass
@@ -330,10 +415,12 @@ class LocalTrainer:
             early_stopping: Optional[int] = 5, restore_best: bool = True,
             reduce_lr_patience: Optional[int] = 2, reduce_lr_factor: float = 0.3, min_lr: float = 1e-6,
             checkpoint_path: Optional[str] = None,
-            on_epoch: Optional[Callable[[int, EpochStats], None]] = None) -> List[EpochStats]:
+            on_epoch: Optional[Callable[[int, EpochStats], None]] = None, head_only: bool = False) -> List[EpochStats]:
         """The reference's ``model.fit(train_ds, validation_data=val_ds, callbacks=[checkpoint,
         early, lr_red], epochs=epoch)`` (FLPyfhelin.py:193). With ``fedprox_mu > 0`` the model at entry is the
-        proximal anchor of every update; the reported losses stay the data loss."""
+        proximal anchor of every update; the reported losses stay the data loss. ``head_only``: FedRep's head phase
+        (DESIGN.md §10) -- only the personal layers train, with the same Adam state and step counter, and no
+        checkpoint, ReduceLROnPlateau or EarlyStopping callback runs."""
         if self.anchor is not None:
             self.anchor.copy_(self.pack.trainable())
         hist: List[EpochStats] = []
@@ -348,7 +435,7 @@ class LocalTrainer:
             ts = ts_all[: train.steps]
             has_val = val is not None and val.steps > 0
             again = (train, True) if ep + 1 < epochs else None
-            self._run_epoch(train, True, ts, nxt=(val, False) if has_val else again)
+            self._run_epoch(train, True, ts, nxt=(val, False) if has_val else again, head=head_only)
             vs = None
             if has_val:
                 self.model.eval()
@@ -364,6 +451,8 @@ class LocalTrainer:
             hist.append(st)
             if on_epoch:
                 on_epoch(ep, st)
+            if head_only:
+                continue
             # ModelCheckpoint(monitor='accuracy', save_best_only=True)
             if checkpoint_path and acc > best_acc:
                 torch.save({"flat": self.pack.flat.detach().cpu(), "epoch": ep, "accuracy": acc}, checkpoint_path)

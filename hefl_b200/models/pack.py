@@ -60,6 +60,20 @@ class ParamPack:
     def trainable(self) -> torch.Tensor:
         return self.flat[: self.n_trainable]
 
+    def dense_tail_start(self, layers: int) -> int:
+        """Offset of the last ``layers`` Dense layers, which must be the tail of the trainable prefix (the sequential
+        CNNs): [0, offset) is everything before them. ``layers = 0`` gives ``n_trainable``."""
+        dense = sorted({int(k.split("_")[1]) for k, *_ in self.entries if self._kind(k) == "dense"})
+        if not 0 <= layers <= len(dense):
+            raise ValueError(f"the model has {len(dense)} Dense layers, cannot keep the last {layers}")
+        if layers == 0:
+            return self.n_trainable
+        tail = {f"c_{li}" for li in dense[-layers:]}
+        lo = min(off for k, _, off, _ in self.entries if k.rsplit("_", 1)[0] in tail)
+        if any((k.rsplit("_", 1)[0] in tail) != (off >= lo) for k, _, off, _ in self.entries) or self.numel != self.n_trainable:
+            raise ValueError("the last Dense layers are not the tail of the parameter vector")
+        return lo
+
     def load_flat(self, vec: torch.Tensor) -> None:
         self.flat.copy_(vec.to(self.flat.device, torch.float32).reshape(-1)[: self.numel])
 

@@ -20,6 +20,8 @@ Replaces Keras' ``model.fit`` compute path (FLPyfhelin.py:118-136, :193) for the
   update    conv_grad_finalize + Adam + conv_weight_relayout: layers 2..6 and the head on the side
             stream under the layer-1 kernel, the 896 (RGB) or 320 (grayscale) layer-1 parameters in the
             tail (``opt`` hooks)
+  head-only (personalised FL, ``head_step_staged``) forward convs without arg-max codes, the head kernel at the
+            depth that yields the personal layers' gradients only, Adam over the personal layers
 
 All buffers are allocated once; a step is CUDA-graph capturable (one graph per input slot); every
 kernel uses programmatic dependent launch (csrc/nn/launch.cuh).
@@ -143,6 +145,11 @@ class MedCNNEngine:
             self.h1_buf = torch.zeros(B * self.H1, dtype=torch.float32, device=device)
             self.dh1_buf = torch.zeros(B * (self.H1 + self.H2), dtype=torch.float32, device=device)
             self.dfeat = torch.zeros(B, self.F, **bf)
+        # personal layers (DESIGN.md §10): a head-only step updates flat[head_lo:n_trainable]; the head kernel stops
+        # after the last personal layer's gradient (depth 5 - p: 4 = dW3 only, 3 = dW2 and dW3, 2 = all, no dfeat)
+        self.personal = int(cfg.personal_layers)
+        self.head_lo = pack.dense_tail_start(self.personal) if self.personal else pack.n_trainable
+        self.head_depth = 5 - self.personal
         self.theta = torch.zeros(B, 2, 3, dtype=torch.float32, device=device)
         self.aug_seed = (cfg.seed * 2654435761 + 12345) & 0x7FFFFFFFFFFFFFFF or 1
         self.prep_count = 0          # augmented batches pre-processed so far (keys the in-kernel Philox draw)
@@ -312,6 +319,36 @@ class MedCNNEngine:
             self.ops.conv_grad_finalize(self.dW32, self.table, self.pack.grad)
             opt.apply(0, self.pack.n_trainable)
             self.after_update()
+
+    def head_step_staged(self, slot: int, y: torch.Tensor, out: torch.Tensor, opt) -> None:
+        """Head-only step on the pre-processed batch in ``slot`` (CUDA-graph body): the conv base is frozen, so its
+        backward (un-pool, dgrad, wgrad, finalize, relayout) is dead work. Forward convs without arg-max codes, the
+        head forward and backward down to the first personal layer (no ``dfeat``), then ``opt.bump()`` and Adam on
+        the personal layers [head_lo, n_trainable)."""
+        if not self.personal:
+            raise RuntimeError("head_step_staged needs personal_layers > 0")
+        feat_bf = self.forward_convs(slot, False)
+        if self.fused_head:
+            self.ops.head_forward_backward(feat_bf, self.pack.flat, self.pack.grad, self.head_offs, y, self.dfeat,
+                                           self.h1_buf, self.dh1_buf, out, self.B, self.F, self.H1, self.H2, self.C,
+                                           self.head_depth)
+        else:
+            fcs = self.model.fcs
+            shared = len(fcs) - self.personal
+            with torch.no_grad():
+                x = feat_bf.view(self.B, -1).float()
+                for fc in fcs[:shared]:
+                    x = F.relu(fc(x))
+            for j in range(shared, len(fcs)):
+                x = fcs[j](x)
+                if j + 1 < len(fcs):
+                    x = F.relu(x)
+            loss = F.cross_entropy(x, y)
+            loss.backward()
+            out[0] = loss.detach()
+            out[1] = (x.argmax(1) == y).sum()
+        opt.bump()
+        opt.apply(self.head_lo, self.pack.n_trainable)
 
     def eval_step(self, x_u8: torch.Tensor, y: torch.Tensor, out: torch.Tensor) -> None:
         self.preprocess(x_u8, 0, False, False)

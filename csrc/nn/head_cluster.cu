@@ -16,6 +16,8 @@
 // ``depth`` says how far the backward runs: 0 eval (P3's loss only), 1 everything, and for a head-only step of
 // personalised federated learning (DESIGN.md §10) 2 = P5 without dfeat, 3 = up to P4's dW2 / db2, 4 = up to P3's
 // dW3 / db3. Every early exit follows the last cluster barrier after which no CTA writes into another's shared memory.
+// depth 5 (kHeadSaliency, Grad-CAM, DESIGN.md §11) seeds the backward with the one-hot of a target class (-1: the
+// arg-max of the logits) instead of p - y, CTA 0 writes the logits, and P3-P5 skip every dW / db: dfeat only.
 // Four cluster barriers replace three kernel boundaries; nothing but parameters gradients, dfeat and the
 // two result scalars touches global memory.
 #include <cooperative_groups.h>
@@ -65,7 +67,8 @@ struct HeadClusterArgs {
   float *gW1, *gb1, *gW2, *gb2, *gW3, *gb3;
   __nv_bfloat16* dfeat;        // [B][F]
   float* out;                  // [2] loss, ncorrect
-  int B, C, depth;           // 0 eval, 1 full backward, 2 / 3 / 4 stop after dW1 / dW2 / dW3 (no dfeat)
+  float* logits;               // [B][C], kHeadSaliency only
+  int B, C, depth;           // 0 eval, 1 full backward, 2 / 3 / 4 stop after dW1 / dW2 / dW3 (no dfeat), kHeadSaliency
 };
 
 __global__ void __launch_bounds__(hc::NT, 1) head_cluster_kernel(const HeadClusterArgs a) {
@@ -233,26 +236,35 @@ __global__ void __launch_bounds__(hc::NT, 1) head_cluster_kernel(const HeadClust
       float s = 0.f;
       for (int c = 0; c < C; ++c) s += __expf(lgS[t * CM + c] - mx);
       const int yy = (int)a.y[t];
-      l = -(lgS[t * CM + yy] - mx - __logf(s));
-      nc = am == yy ? 1.f : 0.f;
-      const float invB = 1.f / B;
-      for (int c = 0; c < C; ++c) {
-        const float p = __expf(lgS[t * CM + c] - mx) / s;
-        lgS[t * CM + c] = (p - (c == yy ? 1.f : 0.f)) * invB;   // dlogits
+      if (a.depth == kHeadSaliency) {                        // d logits[t, target] / d logits: one-hot
+        const int tt = yy < 0 ? am : yy;
+        for (int c = 0; c < C; ++c) {
+          if (r == 0) a.logits[t * C + c] = lgS[t * CM + c];
+          lgS[t * CM + c] = c == tt ? 1.f : 0.f;
+        }
+      } else {
+        l = -(lgS[t * CM + yy] - mx - __logf(s));
+        nc = am == yy ? 1.f : 0.f;
+        const float invB = 1.f / B;
+        for (int c = 0; c < C; ++c) {
+          const float p = __expf(lgS[t * CM + c] - mx) / s;
+          lgS[t * CM + c] = (p - (c == yy ? 1.f : 0.f)) * invB;   // dlogits
+        }
       }
     }
     for (int off = 16; off; off >>= 1) {
       l += __shfl_xor_sync(0xffffffffu, l, off);
       nc += __shfl_xor_sync(0xffffffffu, nc, off);
     }
-    if (t == 0 && r == 0) {
+    if (t == 0 && r == 0 && a.depth != kHeadSaliency) {
       a.out[0] = l / B;
       a.out[1] = nc;
     }
   }
   __syncthreads();
   if (!a.depth) return;          // nobody writes into this CTA's shared memory after the P2 barrier
-  if (r == 0) {
+  const bool params = a.depth != kHeadSaliency;
+  if (r == 0 && params) {
     for (int o = t; o < C * H2 + C; o += NT) {
       if (o < C * H2) {
         const int c = o / H2, j = o - c * H2;
@@ -282,7 +294,7 @@ __global__ void __launch_bounds__(hc::NT, 1) head_cluster_kernel(const HeadClust
   cluster.sync();
 
   // ---- P4: dW2 / db2 (own 8 rows), dh1[:, own 16]
-  {
+  if (params) {
     const int i = t & (H1 - 1), jh = t >> 7;                   // 2 groups of 4 rows
     float acc[4] = {0.f, 0.f, 0.f, 0.f};
     for (int b = 0; b < B; ++b) {
@@ -324,7 +336,7 @@ __global__ void __launch_bounds__(hc::NT, 1) head_cluster_kernel(const HeadClust
   cluster.sync();
 
   // ---- P5: dW1 / db1 (own 16 rows), dfeat[:, own 64 features]
-  {
+  if (params) {
     float acc[J1][2];
 #pragma unroll
     for (int j = 0; j < J1; ++j) acc[j][0] = acc[j][1] = 0.f;
@@ -378,10 +390,10 @@ bool head_cluster_supported(int B, int F, int H1, int H2, int C) {
 
 void head_cluster(const void* feat, const float* W1, const float* b1, const float* W2, const float* b2,
                   const float* W3, const float* b3, const int64_t* y, float* gW1, float* gb1, float* gW2, float* gb2,
-                  float* gW3, float* gb3, void* dfeat, float* out, int B, int C, int depth,
+                  float* gW3, float* gb3, void* dfeat, float* out, float* logits, int B, int C, int depth,
                   cudaStream_t st) {
   HeadClusterArgs a{reinterpret_cast<const __nv_bfloat16*>(feat), W1, b1, W2, b2, W3, b3, y, gW1, gb1, gW2, gb2, gW3, gb3,
-                    reinterpret_cast<__nv_bfloat16*>(dfeat), out, B, C, depth};
+                    reinterpret_cast<__nv_bfloat16*>(dfeat), out, logits, B, C, depth};
   cudaFuncSetAttribute(head_cluster_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, hc::SMEM_BYTES);
   cudaLaunchConfig_t cfg = {};
   cfg.gridDim = dim3(hc::R);

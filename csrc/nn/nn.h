@@ -34,14 +34,25 @@ void conv_wgrad(const void* X, const void* DY, float* dW32, float* ws, int B, in
 
 // Dense head (Flatten -> Dense/ReLU -> Dense/ReLU -> Dense -> softmax-CE) forward + backward. depth: 0 forward and
 // loss only, 1 every gradient and dfeat, 2 / 3 / 4 the gradients of the last 3 / 2 / 1 Dense layers and no dfeat.
+// kHeadSaliency (Grad-CAM): y holds a target class per sample (-1: the arg-max of the logits, lowest index on ties),
+// logits [B][C] are written, the backward is seeded with d logits[b, y_b] instead of the loss and yields dfeat only:
+// no parameter gradient, no loss (gW* and out are not touched).
+constexpr int kHeadSaliency = 5;
 void head_forward_backward(const void* feat, const float* W1, const float* b1, const float* W2, const float* b2,
                            const float* W3, const float* b3, const int64_t* y, float* gW1, float* gb1, float* gW2,
                            float* gb2, float* gW3, float* gb3, void* dfeat, float* h1_buf, float* dh1_buf,
-                           float* out, int B, int F, int H1, int H2, int C, int depth, cudaStream_t st);
+                           float* out, float* logits, int B, int F, int H1, int H2, int C, int depth, cudaStream_t st);
 bool head_cluster_supported(int B, int F, int H1, int H2, int C);
 void head_cluster(const void* feat, const float* W1, const float* b1, const float* W2, const float* b2,
                   const float* W3, const float* b3, const int64_t* y, float* gW1, float* gb1, float* gW2, float* gb2,
-                  float* gW3, float* gb3, void* dfeat, float* out, int B, int C, int depth, cudaStream_t st);
+                  float* gW3, float* gb3, void* dfeat, float* out, float* logits, int B, int C, int depth,
+                  cudaStream_t st);
+// ---- Grad-CAM (gradcam.cu) ----
+// X, G: bf16 [B*Hp*Hp][C] (a conv stage's output and the class score's gradient at it), C a multiple of 8 up to 128.
+// out: fp32 [nvalid][S][S], the bilinear (half-pixel) upsampling of relu(sum_c mean_hw(G) X) divided by the maximum of
+// the Hp x Hp map (0 where that maximum is 0). Scans >= nvalid are neither read nor written.
+bool gradcam_supported(int Hp, int C, int S);
+void gradcam(const void* X, const void* G, float* out, int Hp, int C, int S, int nvalid, cudaStream_t st);
 bool wgrad0_gather_supported(int W, int Wp, int CK, int Ci, int Co);
 // layer-1 partials: [wgrad0_parts(B, Hp)][kWgrad0Part] floats of workspace
 constexpr int kWgrad0Part = 28 * 32;

@@ -212,15 +212,62 @@ void head_forward_backward(const Tensor& feat, const Tensor& flat, Tensor grad, 
     // one launch on a cluster of 8 CTAs (csrc/nn/head_cluster.cu)
     hefl::nn::head_cluster(feat.data_ptr(), p + offs[0], p + offs[1], p + offs[2], p + offs[3], p + offs[4], p + offs[5],
                            y.data_ptr<int64_t>(), g + offs[0], g + offs[1], g + offs[2], g + offs[3], g + offs[4],
-                           g + offs[5], dfeat.data_ptr(), out.data_ptr<float>(), (int)B, (int)C, (int)depth, cur());
+                           g + offs[5], dfeat.data_ptr(), out.data_ptr<float>(), nullptr, (int)B, (int)C, (int)depth,
+                           cur());
     return;
   }
   TORCH_CHECK(B % 2 == 0 && H2 % 4 == 0 && H1 % 4 == 0 && F % 8 == 0, "head dims must be even / multiples of 4 / 8");
   hefl::nn::head_forward_backward(feat.data_ptr(), p + offs[0], p + offs[1], p + offs[2], p + offs[3], p + offs[4],
                                   p + offs[5], y.data_ptr<int64_t>(), g + offs[0], g + offs[1], g + offs[2],
                                   g + offs[3], g + offs[4], g + offs[5], dfeat.data_ptr(), h1_buf.data_ptr<float>(),
-                                  dh1_buf.data_ptr<float>(), out.data_ptr<float>(), (int)B, (int)F, (int)H1, (int)H2,
-                                  (int)C, (int)depth, cur());
+                                  dh1_buf.data_ptr<float>(), out.data_ptr<float>(), nullptr, (int)B, (int)F, (int)H1,
+                                  (int)H2, (int)C, (int)depth, cur());
+}
+
+// Grad-CAM seed of the head (DESIGN.md §11): logits_out [B, C] fp32 and dfeat = d logits[b, target_b] / d feat; a
+// target of -1 is the arg-max of the logits. No parameter gradient and no loss is written.
+void head_saliency(const Tensor& feat, const Tensor& flat, at::IntArrayRef offs, const Tensor& target, Tensor dfeat,
+                   Tensor h1_buf, Tensor dh1_buf, Tensor logits_out, int64_t B, int64_t F, int64_t H1, int64_t H2,
+                   int64_t C) {
+  chk_bf16(feat, "feat"); chk_bf16(dfeat, "dfeat");
+  TORCH_CHECK(offs.size() == 6, "need six parameter offsets");
+  TORCH_CHECK(B <= 32 && B >= 1, "the head kernels handle up to 32 samples per step");
+  TORCH_CHECK(feat.numel() == B * F && dfeat.numel() == B * F, "feat/dfeat must be [B,F]");
+  TORCH_CHECK(flat.is_cuda() && flat.scalar_type() == at::kFloat, "float32 parameter buffer required");
+  TORCH_CHECK(target.is_cuda() && target.scalar_type() == at::kLong && target.numel() == B && target.is_contiguous(),
+              "target must be int64 [B]");
+  TORCH_CHECK(logits_out.is_cuda() && logits_out.scalar_type() == at::kFloat && logits_out.is_contiguous() &&
+              logits_out.numel() == B * C, "logits_out must be a contiguous float32 [B, C]");
+  TORCH_CHECK(h1_buf.numel() >= B * H1 && dh1_buf.numel() >= B * (H1 + H2), "scratch too small");
+  const float* p = flat.data_ptr<float>();
+  if (hefl::nn::head_cluster_supported((int)B, (int)F, (int)H1, (int)H2, (int)C)) {
+    hefl::nn::head_cluster(feat.data_ptr(), p + offs[0], p + offs[1], p + offs[2], p + offs[3], p + offs[4], p + offs[5],
+                           target.data_ptr<int64_t>(), nullptr, nullptr, nullptr, nullptr, nullptr, nullptr,
+                           dfeat.data_ptr(), nullptr, logits_out.data_ptr<float>(), (int)B, (int)C,
+                           hefl::nn::kHeadSaliency, cur());
+    return;
+  }
+  TORCH_CHECK(B % 2 == 0 && H2 % 4 == 0 && H1 % 4 == 0 && F % 8 == 0, "head dims must be even / multiples of 4 / 8");
+  hefl::nn::head_forward_backward(feat.data_ptr(), p + offs[0], p + offs[1], p + offs[2], p + offs[3], p + offs[4],
+                                  p + offs[5], target.data_ptr<int64_t>(), nullptr, nullptr, nullptr, nullptr, nullptr,
+                                  nullptr, dfeat.data_ptr(), h1_buf.data_ptr<float>(), dh1_buf.data_ptr<float>(),
+                                  nullptr, logits_out.data_ptr<float>(), (int)B, (int)F, (int)H1, (int)H2, (int)C,
+                                  hefl::nn::kHeadSaliency, cur());
+}
+
+// Grad-CAM maps (csrc/nn/gradcam.cu): X, G bf16 [B*Hp*Hp, C]; out fp32 with at least nvalid * S * S elements, of which
+// the first nvalid maps are written.
+void gradcam(const Tensor& X, const Tensor& G, Tensor out, int64_t B, int64_t Hp, int64_t C, int64_t S, int64_t nvalid) {
+  chk_bf16(X, "X"); chk_bf16(G, "G");
+  TORCH_CHECK(X.numel() == B * Hp * Hp * C && G.numel() == X.numel(), "X and G must be [B*Hp*Hp, C]");
+  TORCH_CHECK(X.device() == G.device() && out.device() == X.device(), "X, G and out must be on one device");
+  TORCH_CHECK(out.scalar_type() == at::kFloat && out.is_contiguous(), "out must be contiguous float32");
+  TORCH_CHECK(nvalid >= 0 && nvalid <= B && out.numel() >= nvalid * S * S, "out must hold nvalid <= B maps of S x S");
+  TORCH_CHECK(hefl::nn::gradcam_supported((int)Hp, (int)C, (int)S),
+              "gradcam: C must be a multiple of 8 in [8, 128], Hp >= 1 with the Hp x Hp map in shared memory, S >= 1; got Hp=",
+              Hp, " C=", C, " S=", S);
+  if (nvalid == 0) return;
+  hefl::nn::gradcam(X.data_ptr(), G.data_ptr(), out.data_ptr<float>(), (int)Hp, (int)C, (int)S, (int)nvalid, cur());
 }
 
 void conv_set_debug(int64_t mask) { hefl::nn::conv_set_debug((int)mask); }
@@ -448,6 +495,8 @@ TORCH_LIBRARY_FRAGMENT(hefl, m) {
   m.def("preprocess_u8(Tensor x, Tensor? theta, Tensor(a!) X, int aug_seed, Tensor? step, bool spack=False, bool compact=False) -> ()", &preprocess_u8);
   m.def("unpool_relu(Tensor g, Tensor amax, Tensor ypool, Tensor(a!) dY, int B, int H, int W, int Co) -> ()", &unpool_relu);
   m.def("head_forward_backward(Tensor feat, Tensor flat, Tensor(a!) grad, int[] offs, Tensor y, Tensor(b!) dfeat, Tensor(c!) h1_buf, Tensor(d!) dh1_buf, Tensor(e!) out, int B, int F, int H1, int H2, int C, int depth) -> ()", &head_forward_backward);
+  m.def("head_saliency(Tensor feat, Tensor flat, int[] offs, Tensor target, Tensor(a!) dfeat, Tensor(b!) h1_buf, Tensor(c!) dh1_buf, Tensor(d!) logits_out, int B, int F, int H1, int H2, int C) -> ()", &head_saliency);
+  m.def("gradcam(Tensor X, Tensor G, Tensor(a!) out, int B, int Hp, int C, int S, int nvalid) -> ()", &gradcam);
   m.def("conv_set_debug(int mask) -> ()", &conv_set_debug);
   m.def("wgrad0_gather(Tensor X, Tensor g, Tensor amax, Tensor(a!) dW32, int B, int H, int W, bool spack=False, int in_channels=3, bool compact=False) -> ()", &wgrad0_gather);
   m.def("fp8_quantize(Tensor x, Tensor(a!) q, Tensor scale, Tensor(b!) amax) -> ()", &fp8_quantize);

@@ -408,7 +408,9 @@ void conv_grad_finalize(float* dW32, const ConvLayerTable& t, float* grad, int l
 //   k2  h2, logits, loss, dlogits, dW3, db3, dh2                   1 CTA (0.3 MFLOP)
 //   k3  dW2, db2, dh1 (column slices of 16)                        grid H1/16
 //   k4  dW1, db1, dfeat (column slices of 16)                      grid F/16
-// A head-only step (depth 2 / 3 / 4, DESIGN.md §10) skips dfeat, k4, or k3 and k4 with k2's dh2.
+// A head-only step (depth 2 / 3 / 4, DESIGN.md §10) skips dfeat, k4, or k3 and k4 with k2's dh2. Grad-CAM
+// (kHeadSaliency, DESIGN.md §11) seeds k2's dlogits with a one-hot target, writes the logits and runs k3 and k4 without
+// their dW / db (null gradient pointers).
 // ------------------------------------------------------------------------------------------
 namespace hefl {
 namespace nn {
@@ -474,6 +476,7 @@ struct HeadMidArgs {
   float *gW3, *gb3;
   float* dh2;           // [B][H2] out
   float* out;           // [2]: loss, ncorrect
+  float* logits;        // [B][C], kHeadSaliency only
   int B, H1, H2, C, depth;
 };
 
@@ -551,26 +554,34 @@ head_mid_kernel(const HeadMidArgs a) {
       float s = 0.f;
       for (int c = 0; c < C; ++c) s += __expf(lg[tid * C + c] - mx);
       const int yy = (int)a.y[tid];
-      l = -(lg[tid * C + yy] - mx - __logf(s));
-      nc = am == yy ? 1.f : 0.f;
-      const float invB = 1.f / B;
-      for (int c = 0; c < C; ++c) {
-        const float p = __expf(lg[tid * C + c] - mx) / s;
-        lg[tid * C + c] = (p - (c == yy ? 1.f : 0.f)) * invB;   // dlogits
+      if (a.depth == kHeadSaliency) {                          // d logits[b, target] / d logits: one-hot
+        const int tt = yy < 0 ? am : yy;
+        for (int c = 0; c < C; ++c) {
+          a.logits[tid * C + c] = lg[tid * C + c];
+          lg[tid * C + c] = c == tt ? 1.f : 0.f;
+        }
+      } else {
+        l = -(lg[tid * C + yy] - mx - __logf(s));
+        nc = am == yy ? 1.f : 0.f;
+        const float invB = 1.f / B;
+        for (int c = 0; c < C; ++c) {
+          const float p = __expf(lg[tid * C + c] - mx) / s;
+          lg[tid * C + c] = (p - (c == yy ? 1.f : 0.f)) * invB;   // dlogits
+        }
       }
     }
     for (int off = 16; off; off >>= 1) {                       // all 32 lanes take part (B <= 32)
       l += __shfl_xor_sync(0xffffffffu, l, off);
       nc += __shfl_xor_sync(0xffffffffu, nc, off);
     }
-    if (tid == 0) {
+    if (tid == 0 && a.depth != kHeadSaliency) {
       a.out[0] = l / B;
       a.out[1] = nc;
     }
   }
   __syncthreads();
   if (!a.depth) return;
-  for (int o = tid; o < C * H2 + C; o += nt) {                 // dW3, db3
+  for (int o = tid; a.depth != kHeadSaliency && o < C * H2 + C; o += nt) {   // dW3, db3
     if (o < C * H2) {
       const int c = o / H2, j = o % H2;
       float acc = 0.f;
@@ -611,7 +622,7 @@ head_fc2_bwd_kernel(const float* __restrict__ dh2g, const float* __restrict__ h1
 #pragma unroll 2
   for (int i = tid; i < B * 16; i += nt) hs[i] = (i0 + (i & 15)) < H1 ? h1g[(i >> 4) * H1 + i0 + (i & 15)] : 0.f;
   __syncthreads();
-  for (int o = tid; o < H2 * 16; o += nt) {                    // dW2[j][i0+k]
+  for (int o = tid; gW2 != nullptr && o < H2 * 16; o += nt) {  // dW2[j][i0+k]
     const int j = o >> 4, k = o & 15;
     float a0 = 0.f, a1 = 0.f;
     int b = 0;
@@ -633,7 +644,7 @@ head_fc2_bwd_kernel(const float* __restrict__ dh2g, const float* __restrict__ h1
     for (; j < H2; ++j) a0 = fmaf(d[b * (H2 + 1) + j], ws[j * 17 + k], a0);
     if (i0 + k < H1) dh1[b * H1 + i0 + k] = hs[b * 16 + k] > 0.f ? (a0 + a1) : 0.f;
   }
-  if (blockIdx.x == 0) {
+  if (blockIdx.x == 0 && gb2 != nullptr) {
     for (int j = tid; j < H2; j += nt) {
       float acc = 0.f;
       for (int b = 0; b < B; ++b) acc += d[b * (H2 + 1) + j];
@@ -669,7 +680,7 @@ head_fc1_bwd_kernel(const float* __restrict__ dh1, const __nv_bfloat16* __restri
     fs[i] = k0 + k < F ? __bfloat162float(feat[b * F + k0 + k]) : 0.f;
   }
   __syncthreads();
-  for (int o = tid; o < H1 * 16; o += nt) {
+  for (int o = tid; gW1 != nullptr && o < H1 * 16; o += nt) {
     const int j = o >> 4, k = o & 15;
     float a0 = 0.f, a1 = 0.f;
     int b = 0;
@@ -691,7 +702,7 @@ head_fc1_bwd_kernel(const float* __restrict__ dh1, const __nv_bfloat16* __restri
     for (; j < H1; ++j) a0 = fmaf(d[b * (H1 + 1) + j], ws[j * 17 + k], a0);
     if (k0 + k < F) dfeat[b * F + k0 + k] = __float2bfloat16(a0 + a1);
   }
-  if (blockIdx.x == 0) {
+  if (blockIdx.x == 0 && gb1 != nullptr) {
     for (int j = tid; j < H1; j += nt) {
       float acc = 0.f;
       for (int b = 0; b < B; ++b) acc += d[b * (H1 + 1) + j];
@@ -703,27 +714,31 @@ head_fc1_bwd_kernel(const float* __restrict__ dh1, const __nv_bfloat16* __restri
 void head_forward_backward(const void* feat, const float* W1, const float* b1, const float* W2, const float* b2,
                            const float* W3, const float* b3, const int64_t* y, float* gW1, float* gb1, float* gW2,
                            float* gb2, float* gW3, float* gb3, void* dfeat, float* h1_buf, float* dh1_buf,
-                           float* out, int B, int F, int H1, int H2, int C, int depth, cudaStream_t st) {
+                           float* out, float* logits, int B, int F, int H1, int H2, int C, int depth,
+                           cudaStream_t st) {
   const auto* f = reinterpret_cast<const __nv_bfloat16*>(feat);
+  const bool saliency = depth == kHeadSaliency;
   float* dh2_buf = dh1_buf + (size_t)B * H1;                  // scratch tail: [B][H2]
   const int smem_a = (B + 4) * (F + 1) * 4;
   cudaFuncSetAttribute(head_fc1_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_a);
   launch_pdl(head_fc1_fwd_kernel, dim3((H1 + 3) / 4), dim3(128), smem_a, st, f, W1, b1, h1_buf, B, F, H1);
-  HeadMidArgs a{h1_buf, W2, b2, W3, b3, y, gW3, gb3, dh2_buf, out, B, H1, H2, C, depth};
+  HeadMidArgs a{h1_buf, W2, b2, W3, b3, y, gW3, gb3, dh2_buf, out, logits, B, H1, H2, C, depth};
   const int smem_b = (B * (H1 + 1) + H2 * (H1 + 1) + B * (H2 + 1) + B * C + 2 * B + C * H2) * 4;
   cudaFuncSetAttribute(head_mid_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_b);
   launch_pdl(head_mid_kernel, dim3(1), dim3(256), smem_b, st, a);
   hefl::cuda::note_launch(2);
-  if (depth >= 1 && depth <= 3) {
+  if ((depth >= 1 && depth <= 3) || saliency) {
     const int smem_c = (B * (H2 + 1) + B * 16 + H2 * 17) * 4;
-    launch_pdl(head_fc2_bwd_kernel, dim3((H1 + 15) / 16), dim3(256), smem_c, st, dh2_buf, h1_buf, W2, gW2, gb2, dh1_buf, B, H1, H2);
+    launch_pdl(head_fc2_bwd_kernel, dim3((H1 + 15) / 16), dim3(256), smem_c, st, dh2_buf, h1_buf, W2,
+               saliency ? nullptr : gW2, saliency ? nullptr : gb2, dh1_buf, B, H1, H2);
     hefl::cuda::note_launch();
   }
-  if (depth == 1 || depth == 2) {
+  if (depth == 1 || depth == 2 || saliency) {
     const int smem_d = (B * (H1 + 1) + B * 16 + H1 * 17) * 4;
     cudaFuncSetAttribute(head_fc1_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_d);
-    launch_pdl(head_fc1_bwd_kernel, dim3((F + 15) / 16), dim3(256), smem_d, st, dh1_buf, f, W1, gW1, gb1,
-               depth == 1 ? reinterpret_cast<__nv_bfloat16*>(dfeat) : nullptr, B, F, H1);
+    launch_pdl(head_fc1_bwd_kernel, dim3((F + 15) / 16), dim3(256), smem_d, st, dh1_buf, f, W1,
+               saliency ? nullptr : gW1, saliency ? nullptr : gb1,
+               depth == 2 ? nullptr : reinterpret_cast<__nv_bfloat16*>(dfeat), B, F, H1);
     hefl::cuda::note_launch();
   }
 }

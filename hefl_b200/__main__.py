@@ -14,6 +14,8 @@
     python -m hefl_b200 --clients-per-rank 8 --client-fraction 0.5 --dirichlet-alpha 0.3 --fedavg-weighting samples
     # personalised: every client keeps its three Dense layers, 2 head-only epochs before the joint ones (DESIGN.md §10)
     python -m hefl_b200 --clients-per-rank 8 --dirichlet-alpha 0.3 --personal-layers 3 --personal-head-epochs 2
+    # after training, class probabilities and a Grad-CAM heatmap of every test scan (DESIGN.md §11)
+    python -m hefl_b200 --data-dir image/Train --test-dir image/Test --gradcam-dir cams --gradcam-stage 4
 
 Every ``FLConfig`` field is a flag (``--local-epochs 10``) or an environment variable
 (``HEFL_LOCAL_EPOCHS=10``); the reference hard-codes all of them (FLPyfhelin.py:31-36, notebook N:24-32).
@@ -23,6 +25,10 @@ without it a synthetic set of the configured shape is used),
 ``--test-dir DIR`` (same layout; after the last round rank 0 prints the reference's four metrics — weighted
 precision / recall / F1 and accuracy, notebook N:267-270 — of the aggregated model; with ``--personal-layers`` of
 rank 0's first client's personal model, named by ``"client"``),
+``--gradcam-dir DIR`` (needs ``--test-dir``; after the metrics, rank 0 writes ``DIR/predictions.csv`` — file, label,
+predicted, p_0 .. p_{C-1} — and one PNG per test scan blended with its Grad-CAM map, then prints
+``{"gradcam_dir", "images", "stage"}``), ``--gradcam-stage s`` (the conv stage of the map, default 4),
+``--gradcam-class c`` (the explained class; default each scan's predicted class),
 ``--checkpoint PATH`` (written by rank 0 after every round, resumed from if it exists),
 ``--simulate`` (all ``--clients`` in this one process through the loopback transport: the reference's own
 structure, clients as loop iterations, FLPyfhelin.py:184).
@@ -50,8 +56,13 @@ def main(argv=None) -> int:
     extra.add_argument("--stream-decode", action="store_true",
                        help="decode images per batch (flow_from_dataframe semantics) instead of the whole shard up front")
     extra.add_argument("--simulate", action="store_true")
+    extra.add_argument("--gradcam-dir", default=None)
+    extra.add_argument("--gradcam-stage", type=int, default=4)
+    extra.add_argument("--gradcam-class", type=int, default=None)
     extra.add_argument("-h", "--help", action="store_true")
     ns, rest = extra.parse_known_args(argv)
+    if ns.gradcam_dir and not ns.test_dir:
+        extra.error("--gradcam-dir explains the scans of --test-dir: give --test-dir DIR as well")
     if ns.help:
         print(__doc__)
         print("FLConfig fields:", ", ".join(f.name for f in __import__("dataclasses").fields(FLConfig)))
@@ -102,6 +113,10 @@ def main(argv=None) -> int:
                    for cid in range(rank * M, rank * M + M)]
         cfg.num_classes = max(cfg.num_classes, dataset[0].classes)
     run = FederatedRunner(cfg, rank=rank, world=world, device=device, dataset=dataset)
+    if ns.gradcam_dir:
+        from .fl.explain import check_gradcam
+
+        check_gradcam(run.model, ns.gradcam_stage, ns.gradcam_class, 1)     # before training, not after it
     if ns.checkpoint and os.path.exists(ns.checkpoint):
         run.load_checkpoint(ns.checkpoint)
         if rank == 0:
@@ -129,6 +144,12 @@ def main(argv=None) -> int:
             print(json.dumps({"test_images": len(test), "client": run.client_ids[0], **run.evaluate(test, client=0)}))
         else:
             print(json.dumps({"test_images": len(test), **run.evaluate(test)}))
+        del test
+        if ns.gradcam_dir:
+            from .fl.explain import write_explanations
+
+            print(json.dumps(write_explanations(run, ns.test_dir, ns.gradcam_dir, ns.gradcam_stage, ns.gradcam_class,
+                                                client=0 if cfg.personal_layers else None)))
     if world > 1:
         dist.barrier()
         dist.destroy_process_group()

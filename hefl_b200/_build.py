@@ -48,6 +48,7 @@ CUDA_SOURCES = [
     "nn/wgrad_gather.cu",
     "nn/wgrad0_mma.cu",
     "nn/head_cluster.cu",
+    "nn/gradcam.cu",
 ]
 HOST_SOURCES = [
     "he/host_math.cpp",

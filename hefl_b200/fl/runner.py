@@ -37,6 +37,7 @@ from ..models.cnn import MedCNN, SmallCNN
 from ..parallel import LoopbackTransport, make_transport
 from ..utils import DeviceTimer, JsonlLogger, StageTimes
 from .data import BatchFeeder, SyntheticImageDataset, dirichlet_partition, shard_range, split_train_val
+from .explain import check_gradcam, gradcam_torch
 from .server_opt import ServerOptimizer, check_server_options, reference_step
 from .trainer import LocalTrainer
 
@@ -720,6 +721,58 @@ class FederatedRunner:
             preds.append(self.model(x).float().argmax(1).cpu())
         self.model.train()
         return classification_metrics(dataset.labels.cpu(), torch.cat(preds), int(getattr(dataset, "classes", self.cfg.num_classes)))
+
+    def explain(self, images_u8: torch.Tensor, stage: int = 4, target=None, client: Optional[int] = None,
+                batch_size: Optional[int] = None):
+        """Grad-CAM of the installed model (DESIGN.md §11): ``(probs [N, C], cams [N, S, S])``, both fp32 on the CPU,
+        for uint8 NHWC scans ``images_u8`` [N, S, S, in_channels]. ``cams`` are the maps of the class score at conv
+        stage ``stage`` (1..n), upsampled to S x S and scaled to [0, 1]. ``target``: None (each scan's predicted
+        class), an int, or N class indices (-1 = predicted). ``client``: as in ``evaluate``. Runs on the hand-written
+        engine in input slot 0 when the trainer has one (in batches of its fixed batch size, the last one padded;
+        ``batch_size`` is not used there), else ``gradcam_torch`` in batches of ``batch_size``. Not to be called
+        while ``fit`` runs; the weights, optimiser state, augmentation position and RNG are left as they were."""
+        if client is not None and not 0 <= client < self.clients_per_rank:
+            raise ValueError(f"client slot {client} is not one of this rank's {self.clients_per_rank}")
+        if client is not None and self.n_personal and self.clients_per_rank > 1:
+            saved = self.pack.flat[self.n_shared:].clone()
+            self.pack.flat[self.n_shared:].copy_(self._c_head[client])
+            try:
+                return self.explain(images_u8, stage, target, None, batch_size)
+            finally:
+                self.pack.flat[self.n_shared:].copy_(saved)
+        N = int(images_u8.shape[0])
+        targets = check_gradcam(self.model, stage, target, N)
+        cfg = self.cfg
+        S, C = cfg.image_size, self.model.num_classes
+        if tuple(images_u8.shape[1:]) != (S, S, cfg.in_channels) or images_u8.dtype != torch.uint8:
+            raise ValueError(f"images must be uint8 [N, {S}, {S}, {cfg.in_channels}], got {tuple(images_u8.shape)} "
+                             f"{images_u8.dtype}")
+        probs = torch.empty(N, C, dtype=torch.float32)
+        cams = torch.empty(N, S, S, dtype=torch.float32)
+        eng = self.trainer.engine
+        if eng is None:
+            bs = batch_size or cfg.batch_size
+            for i in range(0, N, bs):
+                p, c = gradcam_torch(self.model, images_u8[i:i + bs], stage, targets[i:i + bs])
+                probs[i:i + bs], cams[i:i + bs] = p.float().cpu(), c.float().cpu()
+            return probs, cams
+        B, dev = eng.B, self.device
+        x = torch.zeros(B, S, S, cfg.in_channels, dtype=torch.uint8, device=dev)
+        tgt = torch.full((B,), -1, dtype=torch.int64, device=dev)
+        logits = torch.zeros(B, C, dtype=torch.float32, device=dev)
+        cam = torch.zeros(B, S, S, dtype=torch.float32, device=dev)
+        for i in range(0, N, B):
+            nv = min(B, N - i)
+            if nv < B:                                   # padding rows: explained, never written back
+                x.zero_()
+                tgt.fill_(-1)
+            x[:nv].copy_(images_u8[i:i + nv])
+            tgt[:nv].copy_(targets[i:i + nv])
+            eng.preprocess(x, 0, False, False)
+            eng.gradcam_staged(0, stage, tgt, logits, cam, nv)
+            probs[i:i + nv] = torch.softmax(logits[:nv].cpu(), dim=1)
+            cams[i:i + nv] = cam[:nv].cpu()
+        return probs, cams
 
     # ------------------------------------------------------------------ checkpoint / resume
     def save_checkpoint(self, path: str) -> None:

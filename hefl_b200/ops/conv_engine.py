@@ -22,6 +22,8 @@ Replaces Keras' ``model.fit`` compute path (FLPyfhelin.py:118-136, :193) for the
             tail (``opt`` hooks)
   head-only (personalised FL, ``head_step_staged``) forward convs without arg-max codes, the head kernel at the
             depth that yields the personal layers' gradients only, Adam over the personal layers
+  Grad-CAM  (``gradcam_staged``, DESIGN.md §11) forward convs (arg-max codes from the explained stage on), the head
+            seeded with a class score (head_saliency), the un-pool / dgrad chain down to that stage, gradcam
 
 All buffers are allocated once; a step is CUDA-graph capturable (one graph per input slot); every
 kernel uses programmatic dependent launch (csrc/nn/launch.cuh).
@@ -222,19 +224,20 @@ class MedCNNEngine:
         self.ops.preprocess_u8(x_u8, None, self._x0c[slot] if compact else self.X0[slot], seed, None, self.spack0,
                                compact)     # channels from x_u8
 
-    def forward_convs(self, slot: int, train: bool) -> torch.Tensor:
+    def forward_convs(self, slot: int, train: bool, codes_from: int = 0) -> torch.Tensor:
+        """The conv stack on the input of ``slot``; with ``train``, layers ``codes_from`` .. n-1 store arg-max codes."""
         x = self.X0[slot]
         for l in range(self.n):
             h = self.H[l]
+            codes = self.amax[l] if train and l >= codes_from else None
             if l < self.fwd_pair and h % 2 == 0 and (h - 2) // 2 <= 128 and self.CK[l] <= 32 and self.Co[l] <= 64:
                 compact = l == 0 and self.compact0
                 self.ops.conv_fwd_pool_pair(x if l else self.x0(slot), self._wf0c() if compact else self._wf(l),
-                                            self.bias[l], self.X[l + 1], self.amax[l] if train else None, self.B, h, h,
+                                            self.bias[l], self.X[l + 1], codes, self.B, h, h,
                                             self.CK[l], self.Co[l], self.spack0 and l == 0, self.Ci[0], compact)
                 x = self.X[l + 1]
                 continue
-            self.ops.conv_fwd_pool(x, self._wf(l), self.bias[l], self.X[l + 1],
-                                   self.amax[l] if train else None, self.B, h, h, self.CK[l], self.Co[l],
+            self.ops.conv_fwd_pool(x, self._wf(l), self.bias[l], self.X[l + 1], codes, self.B, h, h, self.CK[l], self.Co[l],
                                    self.spack0 and l == 0, self.Ci[0])
             x = self.X[l + 1]
         return self.X[self.n]
@@ -349,6 +352,35 @@ class MedCNNEngine:
             out[1] = (x.argmax(1) == y).sum()
         opt.bump()
         opt.apply(self.head_lo, self.pack.n_trainable)
+
+    def gradcam_staged(self, slot: int, stage: int, target: torch.Tensor, logits_out: torch.Tensor,
+                       cam_out: torch.Tensor, nvalid: int) -> None:
+        """Grad-CAM (DESIGN.md §11) of the batch pre-processed into ``slot`` (``preprocess(.., train=False,
+        augment=False)``): ``logits_out`` [B, C] fp32 and ``cam_out`` [>= nvalid, S, S] fp32, the first ``nvalid`` maps.
+        ``target`` int64 [B] on the device: the class whose score is explained per scan, -1 for the predicted one.
+        ``stage`` 1..n is the pooled output X[stage] the map is taken at. Runs no weight gradient, finalize, Adam or
+        relayout: only X, amax, dY, gX, dfeat and the head scratch change."""
+        if not 1 <= stage <= self.n:
+            raise ValueError(f"stage must be in 1..{self.n}, got {stage}")
+        feat_bf = self.forward_convs(slot, True, codes_from=stage)
+        if self.fused_head:
+            self.ops.head_saliency(feat_bf, self.pack.flat, self.head_offs, target, self.dfeat, self.h1_buf,
+                                   self.dh1_buf, logits_out, self.B, self.F, self.H1, self.H2, self.C)
+            g = self.dfeat.view_as(feat_bf)
+        else:
+            with torch.enable_grad():
+                feat = feat_bf.view(self.B, -1).float().requires_grad_(True)
+                logits = self._head(feat)
+                t = torch.where(target < 0, logits.argmax(1), target)
+                gf, = torch.autograd.grad(logits.gather(1, t[:, None]).sum(), feat)
+            logits_out.copy_(logits.detach())
+            g = gf.to(torch.bfloat16).view_as(feat_bf).contiguous()
+        for l in range(self.n - 1, stage - 1, -1):
+            h = self.H[l]
+            self.ops.unpool_relu(g, self.amax[l], self.X[l + 1], self.dY[l], self.B, h, h, self.Co[l])
+            self.ops.conv_dgrad(self.dY[l], self._wd(l), self.gX[l], self.B, h, h, self.Co[l], self.Ci[l])
+            g = self.gX[l]
+        self.ops.gradcam(self.X[stage], g, cam_out, self.B, self.H[stage], self.Co[stage - 1], self.H[0], nvalid)
 
     def eval_step(self, x_u8: torch.Tensor, y: torch.Tensor, out: torch.Tensor) -> None:
         self.preprocess(x_u8, 0, False, False)

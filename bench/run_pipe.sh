@@ -1,18 +1,15 @@
 #!/bin/bash
-# ResNet-18 FedAvg stage with / without the SM partition: bash bench/run_pipe.sh <N>
+# ResNet-18 FedAvg stage with its per-chunk timeline: bash bench/run_pipe.sh <N> (results under $OUT, default bench_out)
 N=${1:-2}
-mkdir -p gpurun_out
+OUT=${OUT:-bench_out}
+mkdir -p $OUT
 TR="python -m torch.distributed.run --nnodes=1 --nproc-per-node $N --master-addr 127.0.0.1"
 ARGS="bench.py --gpus $N --steps 3 --warmup 3 --model resnet18 --he-preset n8192_l4 --local-epochs 1 --steps-per-epoch 5 --val-steps 1 --no-own-baseline --skip-e2e"
-for split in default "0,0,0" "100,24,24" "92,24,32"; do
-  if [ "$split" = default ]; then unset HEFL_PIPE_SPLIT; else export HEFL_PIPE_SPLIT=$split; fi
-  tag=$(echo $split | tr ',' '_')
-  HEFL_TIMELINE=gpurun_out/fedavg_timeline_${N}gpu_$tag.json timeout 300 $TR --master-port 29711 $ARGS > gpurun_out/pipe_${N}_$tag.json 2> gpurun_out/pipe_${N}_$tag.err
-  python - <<PY
+HEFL_TIMELINE=$OUT/fedavg_timeline_${N}gpu.json timeout 300 $TR --master-port 29711 $ARGS > $OUT/pipe_${N}.json 2> $OUT/pipe_${N}.err
+python - <<PY
 import json
 try:
-    d=json.load(open("gpurun_out/pipe_${N}_$tag.json")); print("$split", d["stage_ms_last_round"], "ms/round", round(d["ms_per_step"],2))
+    d=json.load(open("$OUT/pipe_${N}.json")); print(d["stage_ms_last_round"], "ms/round", round(d["ms_per_step"],2))
 except Exception as e:
-    print("$split failed", e); print(open("gpurun_out/pipe_${N}_$tag.err").read()[-1500:])
+    print("failed", e); print(open("$OUT/pipe_${N}.err").read()[-1500:])
 PY
-done

@@ -20,6 +20,7 @@ the aggregate and broadcasts the averaged plaintext model.
 """
 from __future__ import annotations
 
+import contextlib
 import hashlib
 import json
 import math
@@ -360,6 +361,23 @@ class FederatedRunner:
         """Install the new global model (the federated part only: personal layers stay as they are)."""
         self.shared().copy_(vec.to(self.pack.flat.device, torch.float32).reshape(-1)[: self.n_shared])
 
+    @contextlib.contextmanager
+    def _client_head(self, client: Optional[int]):
+        """Install client slot ``client``'s personal layers for the block and restore the installed ones on exit (None
+        or a one-client rank, whose client's layers are the installed ones, swaps nothing)."""
+        if client is not None and not 0 <= client < self.clients_per_rank:
+            raise ValueError(f"client slot {client} is not one of this rank's {self.clients_per_rank}")
+        if client is None or not self.n_personal or self.clients_per_rank == 1:
+            yield
+            return
+        head = self.pack.flat[self.n_shared:]
+        saved = head.clone()
+        head.copy_(self._c_head[client])
+        try:
+            yield
+        finally:
+            head.copy_(saved)
+
     def _client_takes_part(self, i: int) -> bool:
         p = self.participating
         return bool(p[i] if isinstance(p, (list, tuple)) else p) or not self.cfg.allow_dropouts
@@ -440,18 +458,56 @@ class FederatedRunner:
             return buf, None, 1.0, 0, True
         return buf, torch.zeros_like(self.shared()), 1.0, self._encrypt_seed(self.num_clients + self.rank), False
 
+    def _encrypt_chunk(self, update, c0: int, c1: int, ci: int = 0) -> CtBatch:
+        """Ciphertexts ``c0 .. c1 - 1`` of the rank's update (``update``: what ``_rank_update`` returned), written
+        into the matching view of its buffer and masked with chunk index ``ci``. Each ciphertext draws its
+        randomness at its own index (``ct_offset``), so before the mask the words do not depend on the chunking."""
+        buf, flat, weight, seed, acc = update
+        ctx, vpc = self.ctx, self.ctx.values_per_ct(self.cfg.packing)
+        nv = min(self.n_shared, c1 * vpc) - c0 * vpc
+        view = buf[c0 * 2 * ctx.L * ctx.n: c1 * 2 * ctx.L * ctx.n]
+        if flat is not None:
+            ct = ctx.encrypt(flat[c0 * vpc: c0 * vpc + nv], self.pk, seed=seed, packing=self.cfg.packing, out=view,
+                             ct_offset=c0, weight=weight, accumulate=acc)
+        else:                                # every client of the rank is already in the buffer
+            ct = CtBatch(view.view(c1 - c0, 2, ctx.L, ctx.n), ctx.scale, nv, self.cfg.packing)
+        self._mask(ct.data, chunk=ci)
+        return ct
+
+    def _decode(self, agg: CtBatch, k: float, offset: int = 0, out: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """The aggregate of ``k`` clients decoded into global values ``offset .. offset + agg.nvals - 1`` of ``out``: the
+        fused server step or the plain average (nothing on a rank without sk). Returns ``out``, or without it a new
+        vector of the shared part: for the plain average the decrypt's own result, installed without a copy."""
+        if self.server_opt is not None:
+            # x_{t+1} = step(x_t, average): decoded and stepped in one launch, broadcast where the average was
+            out = torch.empty_like(self.shared()) if out is None else out
+            self.server_opt.step(self.ctx, agg, self.sk, k, self.global_flat[: self.n_shared], out, offset=offset,
+                                 avg_out=self._avg_out)
+        elif self.has_sk:
+            avg = self.ctx.decrypt(agg, self.sk, divide_by=k)
+            if out is None:
+                return avg
+            out[offset: offset + avg.numel()].copy_(avg)
+        return torch.empty_like(self.shared()) if out is None else out
+
+    def _publish(self, avg: torch.Tensor) -> None:
+        """Broadcast the new global model (and ``_avg_out`` when set) from the key holder, install it as the shared
+        part on every rank and refresh the engine's weight layouts from it."""
+        if self.key_holder >= 0:
+            avg = avg.to(self.pack.flat.dtype).contiguous()
+            dist.broadcast(avg, src=self.key_holder, group=self.group)
+            if self._avg_out is not None:
+                dist.broadcast(self._avg_out, src=self.key_holder, group=self.group)
+        self._install_shared(avg)
+        if self.trainer.engine is not None:
+            self.trainer.engine.after_restore()
+
     def encrypt_update(self) -> CtBatch:
         """The rank's ciphertext of the round: the last trained client added into the buffer its co-located clients
         were accumulated into (an encryption of zeros when none of them takes part), masked once."""
-        buf, flat, weight, seed, acc = self._rank_update()
+        update = self._rank_update()
         with self.timer.stage("encrypt"):
-            if flat is not None:
-                self.ctx.encrypt(flat, self.pk, seed=seed, packing=self.cfg.packing, out=buf, weight=weight,
-                                 accumulate=acc)
-            ct = CtBatch(buf[: self.ct_numel].view(self.n_ct, 2, self.ctx.L, self.ctx.n), self.ctx.scale,
-                         self.n_shared, self.cfg.packing)
-            self._mask(ct.data)
-            return ct
+            return self._encrypt_chunk(update, 0, self.n_ct)
 
     def aggregate(self, ct: CtBatch) -> CtBatch:
         with self.timer.stage("aggregate"):
@@ -463,117 +519,84 @@ class FederatedRunner:
             k = self._contributors()
             if k == 0:                                       # nobody took part: keep the current global model
                 return
-            if self.server_opt is not None:
-                # x_{t+1} = step(x_t, average): decoded and stepped in one launch, broadcast where the average was
-                avg = torch.empty_like(self.shared())
-                self.server_opt.step(self.ctx, agg, self.sk, float(k), self.global_flat[: self.n_shared], avg,
-                                     avg_out=self._avg_out)
-            elif self.has_sk:
-                avg = self.ctx.decrypt(agg, self.sk, divide_by=float(k))
-            else:
-                avg = torch.empty_like(self.shared())
-            if self.key_holder >= 0:
-                avg = avg.to(self.pack.flat.dtype).contiguous()
-                dist.broadcast(avg, src=self.key_holder, group=self.group)
-                if self._avg_out is not None:
-                    dist.broadcast(self._avg_out, src=self.key_holder, group=self.group)
-            self._install_shared(avg)
-            if self.trainer.engine is not None:
-                self.trainer.engine.after_restore()
+            self._publish(self._decode(agg, k))
 
     # ------------------------------------------------------------------ chunked, overlapped FedAvg
     def fedavg_pipelined(self, chunk_cts: int = 256) -> None:
-        """encode+encrypt of chunk i+1, the all-reduce of chunk i and decrypt+decode of chunk i-1
-        run concurrently on three streams (SURVEY.md §5.7: the scaling axis of this workload is
-        ciphertext volume; ResNet-18 is 1.5 GB of ciphertext per client). Result is identical to
-        the unchunked path: chunks are whole ciphertexts and every chunk uses its own seed offset."""
-        ctx, dev = self.ctx, self.device
+        """encode+encrypt of chunk i+1, the all-reduce of chunk i and decrypt+decode of chunk i-1 run concurrently on
+        three CUDA streams (SURVEY.md §5.7: the scaling axis of this workload is ciphertext volume; ResNet-18 is 1.5 GB
+        of ciphertext per client); on the CPU the chunks run in order. Result is identical to the unchunked path:
+        chunks are whole ciphertexts and every chunk uses its own seed offset."""
+        ctx, dev, n_ct = self.ctx, self.device, self.n_ct
+        cuda = dev.type == "cuda"
         vpc = ctx.values_per_ct(self.cfg.packing)
-        n_ct = self.n_ct
-        per_ct = 2 * ctx.L * ctx.n
         # the rank's other clients are already in the buffer; the last one is encrypted chunk by chunk into it
-        buf, flat, weight, seed, acc = self._rank_update()
-        out = torch.empty_like(self.shared())
+        update = self._rank_update()
         k = self._contributors()
         if k == 0:
             return
+        out = torch.empty_like(self.shared())
         if self.server_opt is not None:
             self.server_opt.ensure_state()               # on the current stream, before the three streams fork
-        # the three streams live as long as the runner: the caching allocator keeps one pool per stream, so
-        # fresh streams every round meant fresh cudaMallocs (and cudaFree stalls) every round
-        if getattr(self, "_pipe_streams", None) is None:
-            self._pipe_streams = tuple(torch.cuda.Stream(dev) for _ in range(3))
-        s_enc, s_comm, s_dec = self._pipe_streams
-        cur = torch.cuda.current_stream(dev)
-        for st in (s_enc, s_comm, s_dec):
-            st.wait_stream(cur)
+        s_enc = s_comm = s_dec = cur = None              # torch.cuda.stream(None) leaves the current stream in place
+        if cuda:
+            # the three streams live as long as the runner: the caching allocator keeps one pool per stream, so
+            # fresh streams every round meant fresh cudaMallocs (and cudaFree stalls) every round
+            if getattr(self, "_pipe_streams", None) is None:
+                self._pipe_streams = tuple(torch.cuda.Stream(dev) for _ in range(3))
+            s_enc, s_comm, s_dec = self._pipe_streams
+            cur = torch.cuda.current_stream(dev)
+            for st in (s_enc, s_comm, s_dec):
+                st.wait_stream(cur)
         # The three stages only overlap if they fit on the chip together: encrypt / decrypt are persistent
         # one-CTA-per-SM kernels and the all-reduce is a copy engine that saturates NVLink from a few SMs, so the
-        # SMs are partitioned for the duration of the pipeline (HEFL_PIPE_SPLIT overrides the default split).
+        # SMs are partitioned for the duration of the pipeline (encrypt gets what the other two leave).
         split = None
-        if self.world > 1 and dev.type == "cuda" and self.transport.name == "fused":
-            sms = torch.cuda.get_device_properties(dev).multi_processor_count
-            env = os.environ.get("HEFL_PIPE_SPLIT")
-            if env:
-                split = tuple(int(v) for v in env.split(","))
-            else:
-                ar = 24
-                dec = 28 if self.has_sk else 0
-                split = (sms - ar - dec, dec, ar)
-            if min(split[0], split[2]) >= 2 * ctx.L and split[0] + split[1] + split[2] <= sms:
-                ctx.ops.set_he_cta_limits(0, split[0], split[1])
-                saved_blocks, self.transport.blocks = self.transport.blocks, split[2]
-            else:
-                split = None
-        timeline = [] if os.environ.get("HEFL_TIMELINE") else None
+        if self.world > 1 and cuda and self.transport.name == "fused":
+            ar, dec = 24, 28 if self.has_sk else 0
+            enc = torch.cuda.get_device_properties(dev).multi_processor_count - ar - dec
+            if min(enc, ar) >= 2 * ctx.L:
+                split = (enc, dec, ar)
+                ctx.ops.set_he_cta_limits(0, enc, dec)
+                saved_blocks, self.transport.blocks = self.transport.blocks, ar
+        timeline = [] if cuda and os.environ.get("HEFL_TIMELINE") else None
 
         def mark(stream):
+            if not cuda:
+                return None
             e = torch.cuda.Event(enable_timing=timeline is not None)
             e.record(stream)
             return e
 
         with self.timer.stage("fedavg_pipelined"):
-            ev_enc, ev_comm = [], []
-            chunks = [(c0, min(n_ct, c0 + chunk_cts)) for c0 in range(0, n_ct, chunk_cts)]
             t_origin = mark(cur) if timeline is not None else None
-            for ci, (c0, c1) in enumerate(chunks):
-                nv = min(self.n_shared, c1 * vpc) - c0 * vpc
-                view = buf[c0 * per_ct: c1 * per_ct]
+            for ci, c0 in enumerate(range(0, n_ct, chunk_cts)):
                 rec = {"chunk": ci}
                 with torch.cuda.stream(s_enc):
                     if timeline is not None:
                         rec["enc0"] = mark(s_enc)
-                    if flat is not None:
-                        ct = ctx.encrypt(flat[c0 * vpc: c0 * vpc + nv], self.pk, seed=seed, packing=self.cfg.packing,
-                                         out=view, ct_offset=c0, weight=weight, accumulate=acc)
-                    else:                        # every client of the rank is already in the buffer
-                        ct = CtBatch(view.view(c1 - c0, 2, ctx.L, ctx.n), ctx.scale, nv, self.cfg.packing)
-                    self._mask(ct.data, chunk=ci)
-                    ev_enc.append(mark(s_enc))
+                    ct = self._encrypt_chunk(update, c0, min(n_ct, c0 + chunk_cts), ci)
+                    rec["enc1"] = mark(s_enc)
                 with torch.cuda.stream(s_comm):
-                    s_comm.wait_event(ev_enc[ci])
+                    if cuda:
+                        s_comm.wait_event(rec["enc1"])
                     if timeline is not None:
                         rec["ar0"] = mark(s_comm)
                     data = self.transport.allreduce(ct.data)
-                    ev_comm.append(mark(s_comm))
+                    rec["ar1"] = mark(s_comm)
                 with torch.cuda.stream(s_dec):
-                    s_dec.wait_event(ev_comm[ci])
+                    if cuda:
+                        s_dec.wait_event(rec["ar1"])
                     if timeline is not None:
                         rec["dec0"] = mark(s_dec)
-                    if self.server_opt is not None:
-                        self.server_opt.step(ctx, CtBatch(data, ct.scale, ct.nvals, ct.packing), self.sk, k,
-                                             self.global_flat[: self.n_shared], out, offset=c0 * vpc, avg_out=self._avg_out)
-                    elif self.has_sk:
-                        avg = ctx.decrypt(CtBatch(data, ct.scale, ct.nvals, ct.packing), self.sk, divide_by=k)
-                        out[c0 * vpc: c0 * vpc + avg.numel()].copy_(avg)
+                    self._decode(CtBatch(data, ct.scale, ct.nvals, ct.packing), k, offset=c0 * vpc, out=out)
                     if timeline is not None:
                         rec["dec1"] = mark(s_dec)
                 if timeline is not None:
-                    rec["enc1"], rec["ar1"] = ev_enc[ci], ev_comm[ci]
                     timeline.append(rec)
-            cur.wait_stream(s_dec)
-            cur.wait_stream(s_comm)
-            cur.wait_stream(s_enc)
+            if cuda:
+                for st in (s_dec, s_comm, s_enc):
+                    cur.wait_stream(st)
             if split is not None:
                 ctx.ops.set_he_cta_limits(0, 0, 0)
                 self.transport.blocks = saved_blocks
@@ -585,11 +608,7 @@ class FederatedRunner:
                     with open(os.environ["HEFL_TIMELINE"], "w") as f:
                         json.dump({"world": self.world, "n_ct": n_ct, "chunk_cts": chunk_cts, "sm_split_enc_dec_ar": split,
                                    "unit": "ms since the start of the FedAvg stage", "chunks": rows}, f, indent=1)
-            if self.key_holder >= 0:
-                dist.broadcast(out, src=self.key_holder, group=self.group)
-                if self._avg_out is not None:
-                    dist.broadcast(self._avg_out, src=self.key_holder, group=self.group)
-            self._install_shared(out)
+            self._publish(out)
 
     def guard_finite(self) -> None:
         """NaN/Inf guard on decoded weights (failure detection, SURVEY.md §5.3)."""
@@ -610,12 +629,8 @@ class FederatedRunner:
             pipelined = self.device.type == "cuda" and self.n_ct > 512 and self.transport.name in ("fused", "nccl", "gloo")
         if pipelined:
             self.fedavg_pipelined()
-            if self.trainer.engine is not None:
-                self.trainer.engine.after_restore()
         else:
-            ct = self.encrypt_update()
-            agg = self.aggregate(ct)
-            self.decrypt_apply(agg)
+            self.decrypt_apply(self.aggregate(self.encrypt_update()))
         if self.cfg.debug_poison:
             self.poison_buffers()
         times = self.timer.resolve()
@@ -703,23 +718,15 @@ class FederatedRunner:
         Runs the plain PyTorch forward of the model (any backend / device); not a hot path. ``client``: a local slot
         whose personal layers are installed for the evaluation (the installed ones are restored afterwards); None
         scores the installed model."""
-        if client is not None and not 0 <= client < self.clients_per_rank:
-            raise ValueError(f"client slot {client} is not one of this rank's {self.clients_per_rank}")
-        if client is not None and self.n_personal and self.clients_per_rank > 1:
-            saved = self.pack.flat[self.n_shared:].clone()
-            self.pack.flat[self.n_shared:].copy_(self._c_head[client])
-            try:
-                return self.evaluate(dataset, batch_size)
-            finally:
-                self.pack.flat[self.n_shared:].copy_(saved)
-        bs = batch_size or self.cfg.batch_size
-        self.model.eval()
-        preds = []
-        for i in range(0, len(dataset), bs):
-            x = dataset.images[i:i + bs].to(self.device, non_blocking=True)
-            x = x.permute(0, 3, 1, 2).float() * (1.0 / 255.0)
-            preds.append(self.model(x).float().argmax(1).cpu())
-        self.model.train()
+        with self._client_head(client):
+            bs = batch_size or self.cfg.batch_size
+            self.model.eval()
+            preds = []
+            for i in range(0, len(dataset), bs):
+                x = dataset.images[i:i + bs].to(self.device, non_blocking=True)
+                x = x.permute(0, 3, 1, 2).float() * (1.0 / 255.0)
+                preds.append(self.model(x).float().argmax(1).cpu())
+            self.model.train()
         return classification_metrics(dataset.labels.cpu(), torch.cat(preds), int(getattr(dataset, "classes", self.cfg.num_classes)))
 
     def explain(self, images_u8: torch.Tensor, stage: int = 4, target=None, client: Optional[int] = None,
@@ -731,48 +738,40 @@ class FederatedRunner:
         engine in input slot 0 when the trainer has one (in batches of its fixed batch size, the last one padded;
         ``batch_size`` is not used there), else ``gradcam_torch`` in batches of ``batch_size``. Not to be called
         while ``fit`` runs; the weights, optimiser state, augmentation position and RNG are left as they were."""
-        if client is not None and not 0 <= client < self.clients_per_rank:
-            raise ValueError(f"client slot {client} is not one of this rank's {self.clients_per_rank}")
-        if client is not None and self.n_personal and self.clients_per_rank > 1:
-            saved = self.pack.flat[self.n_shared:].clone()
-            self.pack.flat[self.n_shared:].copy_(self._c_head[client])
-            try:
-                return self.explain(images_u8, stage, target, None, batch_size)
-            finally:
-                self.pack.flat[self.n_shared:].copy_(saved)
-        N = int(images_u8.shape[0])
-        targets = check_gradcam(self.model, stage, target, N)
-        cfg = self.cfg
-        S, C = cfg.image_size, self.model.num_classes
-        if tuple(images_u8.shape[1:]) != (S, S, cfg.in_channels) or images_u8.dtype != torch.uint8:
-            raise ValueError(f"images must be uint8 [N, {S}, {S}, {cfg.in_channels}], got {tuple(images_u8.shape)} "
-                             f"{images_u8.dtype}")
-        probs = torch.empty(N, C, dtype=torch.float32)
-        cams = torch.empty(N, S, S, dtype=torch.float32)
-        eng = self.trainer.engine
-        if eng is None:
-            bs = batch_size or cfg.batch_size
-            for i in range(0, N, bs):
-                p, c = gradcam_torch(self.model, images_u8[i:i + bs], stage, targets[i:i + bs])
-                probs[i:i + bs], cams[i:i + bs] = p.float().cpu(), c.float().cpu()
+        with self._client_head(client):
+            N = int(images_u8.shape[0])
+            targets = check_gradcam(self.model, stage, target, N)
+            cfg = self.cfg
+            S, C = cfg.image_size, self.model.num_classes
+            if tuple(images_u8.shape[1:]) != (S, S, cfg.in_channels) or images_u8.dtype != torch.uint8:
+                raise ValueError(f"images must be uint8 [N, {S}, {S}, {cfg.in_channels}], got "
+                                 f"{tuple(images_u8.shape)} {images_u8.dtype}")
+            probs = torch.empty(N, C, dtype=torch.float32)
+            cams = torch.empty(N, S, S, dtype=torch.float32)
+            eng = self.trainer.engine
+            if eng is None:
+                bs = batch_size or cfg.batch_size
+                for i in range(0, N, bs):
+                    p, c = gradcam_torch(self.model, images_u8[i:i + bs], stage, targets[i:i + bs])
+                    probs[i:i + bs], cams[i:i + bs] = p.float().cpu(), c.float().cpu()
+                return probs, cams
+            B, dev = eng.B, self.device
+            x = torch.zeros(B, S, S, cfg.in_channels, dtype=torch.uint8, device=dev)
+            tgt = torch.full((B,), -1, dtype=torch.int64, device=dev)
+            logits = torch.zeros(B, C, dtype=torch.float32, device=dev)
+            cam = torch.zeros(B, S, S, dtype=torch.float32, device=dev)
+            for i in range(0, N, B):
+                nv = min(B, N - i)
+                if nv < B:                                   # padding rows: explained, never written back
+                    x.zero_()
+                    tgt.fill_(-1)
+                x[:nv].copy_(images_u8[i:i + nv])
+                tgt[:nv].copy_(targets[i:i + nv])
+                eng.preprocess(x, 0, False, False)
+                eng.gradcam_staged(0, stage, tgt, logits, cam, nv)
+                probs[i:i + nv] = torch.softmax(logits[:nv].cpu(), dim=1)
+                cams[i:i + nv] = cam[:nv].cpu()
             return probs, cams
-        B, dev = eng.B, self.device
-        x = torch.zeros(B, S, S, cfg.in_channels, dtype=torch.uint8, device=dev)
-        tgt = torch.full((B,), -1, dtype=torch.int64, device=dev)
-        logits = torch.zeros(B, C, dtype=torch.float32, device=dev)
-        cam = torch.zeros(B, S, S, dtype=torch.float32, device=dev)
-        for i in range(0, N, B):
-            nv = min(B, N - i)
-            if nv < B:                                   # padding rows: explained, never written back
-                x.zero_()
-                tgt.fill_(-1)
-            x[:nv].copy_(images_u8[i:i + nv])
-            tgt[:nv].copy_(targets[i:i + nv])
-            eng.preprocess(x, 0, False, False)
-            eng.gradcam_staged(0, stage, tgt, logits, cam, nv)
-            probs[i:i + nv] = torch.softmax(logits[:nv].cpu(), dim=1)
-            cams[i:i + nv] = cam[:nv].cpu()
-        return probs, cams
 
     # ------------------------------------------------------------------ checkpoint / resume
     def save_checkpoint(self, path: str) -> None:

@@ -1271,6 +1271,303 @@ void conv_wgrad(const void* X, const void* DY, float* dW32, float* ws, int B, in
   });
 }
 
+// ------------------------------------------------------------------------------------------
+// G3: fused data + weight gradient of a CK = Co = 32 layer on a wide map (layer 2 of the medical CNN).
+//
+// The weight gradient keeps wgrad_kernel<32, 32, false>'s work exactly: the same CTA columns (wgrad_plan), units,
+// filter row per blockIdx.z, ring of (X row i + 2, dY row i) stages and MMA sequence per accumulator, on the same
+// operand values. Every CTA partial, and so dW32 after reduce_partials, is the same bits as conv_wgrad's.
+// The data gradient rides on that ring. The dY box is 72 columns starting 2 before the strip (the weight gradient reads
+// its columns 2 .. 65) and dY is loaded for every step of a unit, also for its two leading steps, so at step i the
+// ring holds dY rows i, i - 1, i - 2: all that image row i of the strip needs for
+//   dX[m, :] = sum_{r,s} dY[m - r*W - s, :] * Wd[r,s]      (conv_dgrad's flat formula)
+// Columns and rows that flat indexing would take from a neighbouring row or image are the zero border of dY, which the
+// 3-D boxes read as zeros, so every MMA operand is the value tap_gemm_kernel<32, 32, false, 3> reads, in its tap,
+// k-step order: gX is the same bits as conv_dgrad's. Row i of the strip is computed by the CTA with z = i % 3 (one third
+// of the rows each), and the unit that ends at the last valid row also steps over the two border rows below it for
+// their data gradient only. The map needs strips * 64 >= W (conv_dgrad_wgrad_supported).
+//
+// Warps as wgrad_kernel: 0..7 compute, 8 the TMA producer. For a data-gradient row, warp w owns pixels 16 * (w % 4) ..
+// +15 of the strip and output channels 16 * (w / 4) .. +15. The 18 fragment loads and MMA pairs of a row are software-
+// pipelined (step j + 1's fragments are loaded before step j's MMAs).
+// ------------------------------------------------------------------------------------------
+struct DgradWgradCfg {
+  using WG = WgradCfg<32, 32, false>;
+  static constexpr int C = 32;
+  static constexpr int RB = C * 2;                        // bytes per pixel (64-byte swizzle)
+  static constexpr int X_SEG = WG::X_SEG;                 // X row segment: 72 pixels from the strip start
+  static constexpr int DY_COLS = 72;                      // dY row segment: 72 pixels from 2 before the strip start
+  static constexpr int DY_BYTES = DY_COLS * RB;
+  static constexpr int STAGE = X_SEG + ((DY_BYTES + 1023) / 1024) * 1024;
+  static constexpr int TX = WG::X_BYTES + DY_BYTES;
+  static constexpr int NSTAGE = WG::NSTAGE;
+  static constexpr int W_TAP = C * RB;
+  static constexpr int W_BYTES = 9 * W_TAP;
+  static constexpr int SCR_BYTES = 8 * 1024;              // 1 KB accumulator staging per compute warp
+  static constexpr int SMEM = NSTAGE * STAGE + W_BYTES + SCR_BYTES + 512 + 1024;
+  static constexpr int PART = (9 * C + 1) * C;            // floats of one CTA column's partial
+  static_assert(blocks_fit(SMEM, 2), "two CTAs per SM, as wgrad_kernel");
+  static_assert(NSTAGE >= 4, "ring needs 3 live stages + 1 in flight");
+};
+
+struct DgradWgradArgs {
+  WgradArgs w;          // wgrad_plan's split; w.ws = [gridDim.x][9*32 + 1][32]
+#ifdef HEFL_CONV_DEBUG
+  int dbg;              // 1 = skip TMA data, 2 = skip MMAs, 4 = skip the gX store, 8 = skip the weight-gradient MMAs
+#endif
+  __nv_bfloat16* dx;    // [B*H*W][32]
+};
+
+__global__ void __launch_bounds__(288, 2)
+dgrad_wgrad_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ CUtensorMap tmDY,
+                   const __grid_constant__ CUtensorMap tmW, const DgradWgradArgs args) {
+  using Cfg = DgradWgradCfg;
+  constexpr int CK = 32, SA = Cfg::RB, SB = Cfg::RB, NT = 4, MT = 6;
+  const WgradArgs& a = args.w;
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  uint8_t* sW = smem + Cfg::NSTAGE * Cfg::STAGE;
+  float* scr_all = reinterpret_cast<float*>(sW + Cfg::W_BYTES);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(reinterpret_cast<uint8_t*>(scr_all) + Cfg::SCR_BYTES);
+  uint64_t* full = bars;
+  uint64_t* empty = bars + Cfg::NSTAGE;
+  uint64_t* wfull = bars + 2 * Cfg::NSTAGE;
+  const int warp = threadIdx.x >> 5;
+  const int lane = threadIdx.x & 31;
+  const int fr = blockIdx.z;                                    // filter row r of the weight gradient
+  bool do_mma = true, do_wgrad = true, do_store = true;
+#ifdef HEFL_CONV_DEBUG
+  do_mma = !(args.dbg & 2);
+  do_store = !(args.dbg & 4);
+  do_wgrad = !(args.dbg & 8);
+#endif
+
+  if (warp == 8 && lane == 0) {
+    prefetch_tmap(&tmX);
+    prefetch_tmap(&tmDY);
+    prefetch_tmap(&tmW);
+    for (int s = 0; s < Cfg::NSTAGE; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 8); }
+    mbar_init(wfull, 1);
+    fence_barrier_init();
+  }
+  __syncthreads();
+  // PDL as tap_gemm_kernel: the weight tile before the wait, activations after it
+  pdl_trigger();
+  if (warp == 8 && elect_one()) {
+    mbar_expect_tx(wfull, Cfg::W_BYTES);
+    for (int tap = 0; tap < 9; ++tap) tma_load_2d(sW + tap * Cfg::W_TAP, &tmW, 0, tap * CK, wfull);
+  }
+  pdl_wait();
+  const int per_img = a.strips * a.rsplit;
+
+  if (warp == 8) {
+    if (elect_one()) {
+      int slot = 0;
+      uint32_t phase = 0;
+      for (int u = blockIdx.x; u < a.units; u += gridDim.x) {
+        const int b = u / per_img;
+        const int rem = u - b * per_img;
+        const int strip = rem / a.rsplit;
+        const int h0 = (rem - strip * a.rsplit) * a.rows_per;
+        const int h1 = min(a.Ho, h0 + a.rows_per);
+        if (h0 >= h1) continue;
+        const int h_end = h1 == a.Ho ? a.H : h1;               // + the border rows' data gradient
+        for (int i = h0 - 2; i < h_end; ++i) {
+          mbar_wait(&empty[slot], phase ^ 1u);
+          uint8_t* st = smem + slot * Cfg::STAGE;
+#ifdef HEFL_CONV_DEBUG
+          if (args.dbg & 1) {
+            mbar_arrive(&full[slot]);
+          } else
+#endif
+          {
+            mbar_expect_tx(&full[slot], Cfg::TX);
+            tma_load_3d(st, &tmX, 0, strip * 64, b * a.H + i + 2, &full[slot]);
+            tma_load_3d(st + Cfg::X_SEG, &tmDY, 0, strip * 64 - 2, b * a.H + i, &full[slot]);
+          }
+          if (++slot == Cfg::NSTAGE) { slot = 0; phase ^= 1; }
+        }
+      }
+    }
+    return;
+  }
+
+  // ===== compute warps 0..7: the weight gradient exactly as wgrad_kernel<32, 32, false>
+  float acc[2][NT][4];
+  float bacc[4] = {0.f, 0.f, 0.f, 0.f};
+#pragma unroll
+  for (int u = 0; u < 2; ++u)
+#pragma unroll
+    for (int n = 0; n < NT; ++n)
+#pragma unroll
+      for (int q = 0; q < 4; ++q) acc[u][n][q] = 0.f;
+  constexpr uint32_t kOnes = 0x3F803F80u;                       // bf16 1.0 x2
+  const uint32_t ones[4] = {kOnes, kOnes, kOnes, kOnes};
+  const int bias_nt = warp % NT;
+  const int lrow = lane & 7;
+  const int ia = lane >> 3;
+  uint32_t a_off[2];
+  int a_shift[2];
+#pragma unroll
+  for (int u = 0; u < 2; ++u) {
+    const int tile = warp + 8 * u;
+    const int s = tile / (CK / 16), ci0 = (tile % (CK / 16)) * 16;
+    a_shift[u] = s;
+    a_off[u] = (uint32_t)(ci0 * 2 + (ia & 1) * 16);
+  }
+  const uint32_t smem0 = smem_u32(smem);
+  const uint32_t w_base = smem_u32(sW);
+  float* scr = scr_all + warp * 256;
+  const int qd = warp & 3, grp = warp >> 2;                    // data gradient: pixels 16 qd .., channels 16 grp ..
+
+  auto wstep = [&](uint32_t x_tile, uint32_t dy_tile) {
+#pragma unroll
+    for (int kk = 0; kk < 4; ++kk) {
+      uint32_t bf[NT / 2][4];
+#pragma unroll
+      for (int n = 0; n < NT; n += 2)
+        ldsm_x4_t(swz<SB>(dy_tile + (uint32_t)((kk * 16 + (ia & 1) * 8 + lrow) * SB + (n + (ia >> 1)) * 16)), bf[n / 2]);
+#pragma unroll
+      for (int u = 0; u < 2; ++u) {
+        if (warp + 8 * u >= MT) break;
+        uint32_t af[4];
+        ldsm_x4_t(swz<SA>(x_tile + (uint32_t)((kk * 16 + (ia >> 1) * 8 + lrow + a_shift[u]) * SA) + a_off[u]), af);
+#pragma unroll
+        for (int n = 0; n < NT; ++n) mma_bf16(acc[u][n], af, bf[n / 2][(n & 1) * 2], bf[n / 2][(n & 1) * 2 + 1]);
+      }
+      if (fr == 0) {
+#pragma unroll
+        for (int n = 0; n < NT; ++n)
+          if (n == bias_nt) mma_bf16(bacc, ones, bf[n / 2][(n & 1) * 2], bf[n / 2][(n & 1) * 2 + 1]);
+      }
+    }
+  };
+
+  // data gradient of image row h (= b*H + h of the [B*H] row axis) of the strip; dyr[r] = dY stage of row h - r
+  auto drow = [&](const uint32_t (&dyr)[3], int row, int strip) {
+    float d[2][4];
+#pragma unroll
+    for (int i = 0; i < 2; ++i)
+#pragma unroll
+      for (int q = 0; q < 4; ++q) d[i][q] = 0.f;
+    if (do_mma) {
+      // step j = (tap j / 2, k-step j % 2), tap_gemm_kernel's order; dY column c - s is row 2 - s + c of a segment
+      auto load = [&](int j, uint32_t(&bf)[4], uint32_t(&af)[4]) {
+        const int tap = j >> 1, ks = j & 1, r = tap / 3, s = tap % 3;
+        ld_b_kmajor<Cfg::RB>(w_base + tap * Cfg::W_TAP, grp * 16, grp * 16 + 8, ks * 32, lane, bf);
+        ld_a_kmajor<Cfg::RB>(dyr[r], (2 - s) + qd * 16, ks * 32, lane, af);
+      };
+      uint32_t bf[2][4], af[2][4];
+      load(0, bf[0], af[0]);
+#pragma unroll
+      for (int j = 0; j < 18; ++j) {
+        const int c = j & 1;
+        if (j + 1 < 18) load(j + 1, bf[c ^ 1], af[c ^ 1]);
+        mma_bf16(d[0], af[c], bf[c][0], bf[c][1]);
+        mma_bf16(d[1], af[c], bf[c][2], bf[c][3]);
+      }
+    }
+    // lane L: pixel 16 qd + L % 16 of the strip, channels 16 grp + 8 (L / 16) .. +7
+    float v[8];
+    frag_rows(scr, d[0], d[1], lane, v);
+    const int w = strip * 64 + qd * 16 + (lane & 15);
+    if (do_store && w < a.W)
+      *reinterpret_cast<uint4*>(args.dx + ((size_t)row * a.W + w) * CK + grp * 16 + (lane >> 4) * 8) =
+          make_uint4(pack_bf16x2(v[0], v[1]), pack_bf16x2(v[2], v[3]), pack_bf16x2(v[4], v[5]),
+                     pack_bf16x2(v[6], v[7]));
+  };
+
+  mbar_wait(wfull, 0);
+  int slot = 0;
+  uint32_t phase = 0;
+  for (int u = blockIdx.x; u < a.units; u += gridDim.x) {
+    const int b = u / per_img;
+    const int rem = u - b * per_img;
+    const int strip = rem / a.rsplit;
+    const int h0 = (rem - strip * a.rsplit) * a.rows_per;
+    const int h1 = min(a.Ho, h0 + a.rows_per);
+    if (h0 >= h1) continue;
+    const int h_end = h1 == a.Ho ? a.H : h1;
+    for (int i = h0 - 2; i < h_end; ++i) {
+      mbar_wait(&full[slot], phase);
+      const int s1 = slot == 0 ? Cfg::NSTAGE - 1 : slot - 1;       // stage of X row h+1, dY row h-1
+      const int s0 = s1 == 0 ? Cfg::NSTAGE - 1 : s1 - 1;           // stage of X row h, dY row h-2
+      if (i >= h0) {
+        if (i < h1 && do_mma && do_wgrad) {
+          const int sx = fr == 0 ? s0 : (fr == 1 ? s1 : slot);
+          wstep(smem0 + sx * Cfg::STAGE, smem0 + slot * Cfg::STAGE + Cfg::X_SEG + 2 * SB);
+        }
+        if (i % 3 == fr) {
+          const uint32_t dyr[3] = {smem0 + slot * Cfg::STAGE + Cfg::X_SEG, smem0 + s1 * Cfg::STAGE + Cfg::X_SEG,
+                                   smem0 + s0 * Cfg::STAGE + Cfg::X_SEG};
+          drow(dyr, b * a.H + i, strip);
+        }
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&empty[s0]);                    // stage of X row h / dY row h-2 is done
+      }
+      if (++slot == Cfg::NSTAGE) { slot = 0; phase ^= 1; }
+    }
+    __syncwarp();
+    if (lane == 0) {                                               // release the last two stages of the unit
+      const int l1 = slot == 0 ? Cfg::NSTAGE - 1 : slot - 1;
+      const int l0 = l1 == 0 ? Cfg::NSTAGE - 1 : l1 - 1;
+      mbar_arrive(&empty[l0]);
+      mbar_arrive(&empty[l1]);
+    }
+  }
+  // wgrad_kernel's partial store: every CTA writes its whole share (zeros when it had no work)
+  float* part = a.ws + (size_t)blockIdx.x * (9 * CK + 1) * a.Co;
+#pragma unroll
+  for (int u = 0; u < 2; ++u) {
+    const int tile = warp + 8 * u;
+    if (tile >= MT) break;
+    const int s = tile / (CK / 16), ci0 = (tile % (CK / 16)) * 16;
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int R = (fr * 3 + s) * CK + ci0 + (lane >> 2) + 8 * h;   // dW32 row: (r*3+s)*CK + ci
+      float* dst = part + (size_t)R * a.Co + 2 * (lane & 3);
+#pragma unroll
+      for (int n = 0; n < NT; ++n)
+        *reinterpret_cast<float2*>(dst + n * 8) = make_float2(acc[u][n][2 * h], acc[u][n][2 * h + 1]);
+    }
+  }
+  if (fr == 0 && warp < NT && lane < 4)                              // bias: row 0 of the all-ones product
+    *reinterpret_cast<float2*>(part + (size_t)(9 * CK) * a.Co + bias_nt * 8 + 2 * lane) = make_float2(bacc[0], bacc[1]);
+}
+
+bool conv_dgrad_wgrad_supported(int H, int W, int CK, int Co) {
+  return CK == 32 && Co == 32 && H >= 3 && W >= 3 && (W - 2 + 63) / 64 * 64 >= W;
+}
+
+int64_t conv_dgrad_wgrad_ws_floats(int B, int H, int W) {
+  WgradArgs a;
+  return (int64_t)wgrad_plan<32, 32, false>(B, H, W, 32, a) * DgradWgradCfg::PART;
+}
+
+void conv_dgrad_wgrad(const void* X, const void* dY, const void* Wd, void* dX, float* dW32, float* ws, int B, int H,
+                      int W, int CK, int Co, cudaStream_t st) {
+  using Cfg = DgradWgradCfg;
+  if (!conv_dgrad_wgrad_supported(H, W, CK, Co))
+    throw std::runtime_error("conv_dgrad_wgrad: CK = Co = 32 and a map the 64-column strips cover");
+  DgradWgradArgs a{};
+#ifdef HEFL_CONV_DEBUG
+  a.dbg = g_dbg;
+#endif
+  const int gx = wgrad_plan<32, 32, false>(B, H, W, Co, a.w);
+  a.w.ws = ws;
+  a.dx = reinterpret_cast<__nv_bfloat16*>(dX);
+  const auto* x = reinterpret_cast<const __nv_bfloat16*>(X);
+  const auto* d = reinterpret_cast<const __nv_bfloat16*>(dY);
+  const CUtensorMap tmX = make_map_3d(x, Cfg::C, W, (uint64_t)B * H, Cfg::RB, Cfg::C, Cfg::WG::XROWS);
+  const CUtensorMap tmD = make_map_3d(d, Cfg::C, W, (uint64_t)B * H, Cfg::RB, Cfg::C, Cfg::DY_COLS);
+  const CUtensorMap tmW = make_map(Wd, Cfg::C, 9 * Cfg::C, Cfg::RB, Cfg::C, Cfg::C);
+  cudaFuncSetAttribute(dgrad_wgrad_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM);
+  launch_pdl(dgrad_wgrad_kernel, dim3(gx, 1, 3), dim3(288), Cfg::SMEM, st, tmX, tmD, tmW, a);
+  hefl::cuda::note_launch();
+  // a plain launch: starts only when every partial is written
+  reduce_partials(ws, gx, Cfg::PART, dW32, st);
+}
+
 }  // namespace nn
 }  // namespace hefl
 

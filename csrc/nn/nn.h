@@ -31,6 +31,12 @@ void conv_dgrad(const void* dY, const void* Wd, void* dX, int B, int H, int W, i
 int64_t conv_wgrad_ws_floats(int B, int H, int W, int CK, int Co);
 void conv_wgrad(const void* X, const void* DY, float* dW32, float* ws, int B, int H, int W, int CK, int Co,
                 cudaStream_t st);
+// Both gradients of a CK = Co = 32 layer from one pass over dY: the same bits as conv_dgrad(dY, Wd, dX, .., 32, 32)
+// and conv_wgrad(X, dY, dW32, .., 32, 32). ws: conv_dgrad_wgrad_ws_floats(...) floats.
+bool conv_dgrad_wgrad_supported(int H, int W, int CK, int Co);
+int64_t conv_dgrad_wgrad_ws_floats(int B, int H, int W);
+void conv_dgrad_wgrad(const void* X, const void* dY, const void* Wd, void* dX, float* dW32, float* ws, int B, int H,
+                      int W, int CK, int Co, cudaStream_t st);
 
 // Dense head (Flatten -> Dense/ReLU -> Dense/ReLU -> Dense -> softmax-CE) forward + backward. depth: 0 forward and
 // loss only, 1 every gradient and dfeat, 2 / 3 / 4 the gradients of the last 3 / 2 / 1 Dense layers and no dfeat.

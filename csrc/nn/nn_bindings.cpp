@@ -155,6 +155,24 @@ void conv_wgrad(const Tensor& X, const Tensor& DY, Tensor dW32, int64_t B, int64
                        (int)CK, (int)Co, cur());
 }
 
+bool conv_dgrad_wgrad_supported(int64_t H, int64_t W, int64_t CK, int64_t Co) {
+  return hefl::nn::conv_dgrad_wgrad_supported((int)H, (int)W, (int)CK, (int)Co);
+}
+
+void conv_dgrad_wgrad(const Tensor& X, const Tensor& dY, const Tensor& Wd, Tensor dX, Tensor dW32, int64_t B, int64_t H,
+                      int64_t W, int64_t CK, int64_t Co) {
+  chk_bf16(X, "X"); chk_bf16(dY, "dY"); chk_bf16(Wd, "Wd"); chk_bf16(dX, "dX");
+  TORCH_CHECK(hefl::nn::conv_dgrad_wgrad_supported((int)H, (int)W, (int)CK, (int)Co),
+              "conv_dgrad_wgrad: CK = Co = 32 and (W - 2) rounded up to 64 columns must cover W");
+  const int64_t P = B * H * W;
+  TORCH_CHECK(X.numel() == P * CK && dY.numel() == P * Co && dX.numel() == P * CK && Wd.numel() == 9 * CK * Co,
+              "X, dX must be [B*H*W, CK], dY [B*H*W, Co], Wd [9, CK, Co]");
+  TORCH_CHECK(dW32.is_cuda() && dW32.scalar_type() == at::kFloat && dW32.numel() >= (9 * CK + 1) * Co, "dW32 too small");
+  Tensor ws = at::empty({hefl::nn::conv_dgrad_wgrad_ws_floats((int)B, (int)H, (int)W)}, dW32.options());
+  hefl::nn::conv_dgrad_wgrad(X.data_ptr(), dY.data_ptr(), Wd.data_ptr(), dX.data_ptr(), dW32.data_ptr<float>(),
+                             ws.data_ptr<float>(), (int)B, (int)H, (int)W, (int)CK, (int)Co, cur());
+}
+
 void preprocess_u8(const Tensor& x, const c10::optional<Tensor>& theta, Tensor X, int64_t aug_seed,
                    const c10::optional<Tensor>& step, bool spack, bool compact) {
   TORCH_CHECK(x.is_cuda() && x.scalar_type() == at::kByte && x.is_contiguous() && x.dim() == 4 && (x.size(3) == 3 || x.size(3) == 1),
@@ -492,6 +510,9 @@ TORCH_LIBRARY_FRAGMENT(hefl, m) {
   m.def("conv_fwd_pool_pair(Tensor X, Tensor Wf, Tensor bias, Tensor(a!) out, Tensor(b!)? argmax, int B, int H, int W, int CK, int CO, bool spack=False, int in_channels=3, bool compact=False) -> ()", &conv_fwd_pool_pair);
   m.def("conv_dgrad(Tensor dY, Tensor Wd, Tensor(a!) dX, int B, int H, int W, int CK, int CO) -> ()", &conv_dgrad);
   m.def("conv_wgrad(Tensor X, Tensor DY, Tensor(a!) dW32, int B, int H, int W, int CK, int Co) -> ()", &conv_wgrad);
+  m.def("conv_dgrad_wgrad_supported(int H, int W, int CK, int Co) -> bool", &conv_dgrad_wgrad_supported);
+  m.def("conv_dgrad_wgrad(Tensor X, Tensor dY, Tensor Wd, Tensor(a!) dX, Tensor(b!) dW32, int B, int H, int W, int CK, "
+        "int Co) -> ()", &conv_dgrad_wgrad);
   m.def("preprocess_u8(Tensor x, Tensor? theta, Tensor(a!) X, int aug_seed, Tensor? step, bool spack=False, bool compact=False) -> ()", &preprocess_u8);
   m.def("unpool_relu(Tensor g, Tensor amax, Tensor ypool, Tensor(a!) dY, int B, int H, int W, int Co) -> ()", &unpool_relu);
   m.def("head_forward_backward(Tensor feat, Tensor flat, Tensor(a!) grad, int[] offs, Tensor y, Tensor(b!) dfeat, Tensor(c!) h1_buf, Tensor(d!) dh1_buf, Tensor(e!) out, int B, int F, int H1, int H2, int C, int depth) -> ()", &head_forward_backward);

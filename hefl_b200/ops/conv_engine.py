@@ -14,7 +14,8 @@ Replaces Keras' ``model.fit`` compute path (FLPyfhelin.py:118-136, :193) for the
                                    cluster of 8 CTAs)
   backward  unpool_relu / conv_dgrad chain on the main stream (layers 6..2),
             conv_wgrad (tensor cores, operands read in place, split-K partials added in a fixed order) on a
-            side stream,
+            side stream; layer 2 (CK = Co = 32 on the wide map): conv_dgrad_wgrad, both gradients from one pass
+            over dY on the main stream,
             layer 1: wgrad0_gather straight from the pooled gradient (no un-pool, no dY tensor): four
                      masked GEMMs on the tensor cores (wgrad0_mma.cu), FP32-pipe gather as the fallback
   update    conv_grad_finalize + Adam + conv_weight_relayout: layers 2..6 and the head on the side
@@ -93,6 +94,12 @@ class MedCNNEngine:
         self.gather_wgrad0 = (os.environ.get("HEFL_GATHER_WGRAD0", "1") != "0" and self.Co[0] == 32
                               and self.CK[0] == 16 and self.H[0] <= 256)
         self._wgrad0_mma = not os.environ.get("HEFL_WGRAD0_MMA", "1").startswith("0")     # as wgrad0_mma.cu reads it
+        # layers whose data and weight gradients come from one pass over dY on the main stream (conv_dgrad_wgrad,
+        # conv_tcgen05.cu G3): CK = Co = 32 on a map wider than 64 columns (layer 2), where the weight gradient on the
+        # side stream was the step's tail. Same bits as conv_dgrad + conv_wgrad.
+        self.dgrad_wgrad = [l > 0 and self.H[l] > 64 and self.CK[l] == 32 and self.Co[l] == 32
+                            and self.ops.conv_dgrad_wgrad_supported(self.H[l], self.H[l], 32, 32)
+                            for l in range(self.n)]
         bf = dict(dtype=torch.bfloat16, device=device)
         self.P = [B * self.H[l] * self.H[l] for l in range(self.n + 1)]
         # activations / gradients (all NHWC bf16 viewed as [pixels, channels])
@@ -301,7 +308,13 @@ class MedCNNEngine:
             if self.dY[l] is None:
                 self.dY[l] = torch.zeros(self.P[l], self.Co[l], dtype=torch.bfloat16, device=self.device)
             self.ops.unpool_relu(g, self.amax[l], self.X[l + 1], self.dY[l], self.B, h, h, self.Co[l])
-            if l > 0:
+            if l > 0 and self.dgrad_wgrad[l]:
+                # both gradients on the main stream; the side stream's finalize of this layer waits on an event
+                # recorded after it (layer 1's split below, or main.wait_stream(side) at the end)
+                self.ops.conv_dgrad_wgrad(xin, self.dY[l], self._wd(l), self.gX[l], self._dw(l), self.B, h, h,
+                                          self.CK[l], self.Co[l])
+                g = self.gX[l]
+            elif l > 0:
                 # wgrad(l) only needs X[l] and dY[l]; dgrad(l) -> unpool(l-1) -> ... proceeds meanwhile
                 self.side.wait_stream(main)
                 with torch.cuda.stream(self.side):

@@ -59,6 +59,13 @@ void head_cluster(const void* feat, const float* W1, const float* b1, const floa
 // the Hp x Hp map (0 where that maximum is 0). Scans >= nvalid are neither read nor written.
 bool gradcam_supported(int Hp, int C, int S);
 void gradcam(const void* X, const void* G, float* out, int Hp, int C, int S, int nvalid, cudaStream_t st);
+// ---- layer-1 input gradient (input_grad.cu, DESIGN.md §12) ----
+// g: bf16 [B*Hp*Hp][32], the gradient at layer 1's pooled output, Hp = (S - 2) / 2; amax: its codes (bits 0-1 arg-max
+// position, bit 2 active unit); w: layer 1's bf16 weights [32][in_channels][3][3]. acc: fp32 [nvalid][S][S]
+// [in_channels] += the full correlation of the conv-grid gradient (g at the arg-max of every active window, 0 elsewhere)
+// with w, in_channels 1 or 3. Scans >= nvalid are neither read nor written.
+void input_grad0(const void* g, const uint8_t* amax, const void* w, float* acc, int S, int Hp, int in_channels,
+                 int nvalid, cudaStream_t st);
 bool wgrad0_gather_supported(int W, int Wp, int CK, int Ci, int Co);
 // layer-1 partials: [wgrad0_parts(B, Hp)][kWgrad0Part] floats of workspace
 constexpr int kWgrad0Part = 28 * 32;

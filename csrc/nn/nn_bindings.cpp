@@ -288,6 +288,31 @@ void gradcam(const Tensor& X, const Tensor& G, Tensor out, int64_t B, int64_t Hp
   hefl::nn::gradcam(X.data_ptr(), G.data_ptr(), out.data_ptr<float>(), (int)Hp, (int)C, (int)S, (int)nvalid, cur());
 }
 
+// Layer-1 input gradient (csrc/nn/input_grad.cu): g bf16 [B*Hp*Hp, 32] at layer 1's pooled output, amax uint8 codes
+// of the same shape, w bf16 [32 * in_channels * 9] (layer 1's [Co][Ci][3][3] weights), acc fp32 with at least
+// nvalid * S * S * in_channels elements, of which the first nvalid scans are accumulated into.
+void input_grad0(const Tensor& g, const Tensor& amax, const Tensor& w, Tensor acc, int64_t B, int64_t S,
+                 int64_t in_channels, int64_t nvalid) {
+  chk_bf16(g, "g"); chk_bf16(w, "w");
+  TORCH_CHECK(in_channels == 1 || in_channels == 3, "input_grad0: in_channels must be 1 or 3, got ", in_channels);
+  const int64_t Hp = (S - 2) / 2;
+  TORCH_CHECK(S >= 4 && S <= 65534, "input_grad0: S must be in [4, 65534], got ", S);
+  TORCH_CHECK(B >= 1 && g.numel() == B * Hp * Hp * 32, "input_grad0: g must be [B*Hp*Hp, 32] with Hp = (S - 2) / 2");
+  TORCH_CHECK(amax.is_cuda() && amax.scalar_type() == at::kByte && amax.is_contiguous() && amax.numel() == g.numel(),
+              "input_grad0: amax must be contiguous uint8 like g");
+  TORCH_CHECK(w.numel() == 32 * in_channels * 9, "input_grad0: w must hold 32 x in_channels x 3 x 3 weights");
+  TORCH_CHECK(acc.is_cuda() && acc.scalar_type() == at::kFloat && acc.is_contiguous(), "acc must be contiguous float32");
+  TORCH_CHECK(g.device() == amax.device() && g.device() == w.device() && g.device() == acc.device(),
+              "g, amax, w and acc must be on one device");
+  TORCH_CHECK(reinterpret_cast<uintptr_t>(g.data_ptr()) % 16 == 0 && reinterpret_cast<uintptr_t>(amax.data_ptr()) % 16 == 0,
+              "input_grad0: g and amax must be 16-byte aligned");
+  TORCH_CHECK(nvalid >= 0 && nvalid <= B && nvalid <= 65535 && acc.numel() >= nvalid * S * S * in_channels,
+              "acc must hold nvalid <= B scans of S x S x in_channels");
+  if (nvalid == 0) return;
+  hefl::nn::input_grad0(g.data_ptr(), amax.data_ptr<uint8_t>(), w.data_ptr(), acc.data_ptr<float>(), (int)S, (int)Hp,
+                        (int)in_channels, (int)nvalid, cur());
+}
+
 void conv_set_debug(int64_t mask) { hefl::nn::conv_set_debug((int)mask); }
 
 // x, res, y: NHWC bf16 viewed as [P, C]. Returns nothing; mean/invstd/sums are caller-provided fp32 scratch.
@@ -518,6 +543,7 @@ TORCH_LIBRARY_FRAGMENT(hefl, m) {
   m.def("head_forward_backward(Tensor feat, Tensor flat, Tensor(a!) grad, int[] offs, Tensor y, Tensor(b!) dfeat, Tensor(c!) h1_buf, Tensor(d!) dh1_buf, Tensor(e!) out, int B, int F, int H1, int H2, int C, int depth) -> ()", &head_forward_backward);
   m.def("head_saliency(Tensor feat, Tensor flat, int[] offs, Tensor target, Tensor(a!) dfeat, Tensor(b!) h1_buf, Tensor(c!) dh1_buf, Tensor(d!) logits_out, int B, int F, int H1, int H2, int C) -> ()", &head_saliency);
   m.def("gradcam(Tensor X, Tensor G, Tensor(a!) out, int B, int Hp, int C, int S, int nvalid) -> ()", &gradcam);
+  m.def("input_grad0(Tensor g, Tensor amax, Tensor w, Tensor(a!) acc, int B, int S, int in_channels, int nvalid) -> ()", &input_grad0);
   m.def("conv_set_debug(int mask) -> ()", &conv_set_debug);
   m.def("wgrad0_gather(Tensor X, Tensor g, Tensor amax, Tensor(a!) dW32, int B, int H, int W, bool spack=False, int in_channels=3, bool compact=False) -> ()", &wgrad0_gather);
   m.def("fp8_quantize(Tensor x, Tensor(a!) q, Tensor scale, Tensor(b!) amax) -> ()", &fp8_quantize);

@@ -16,6 +16,8 @@
     python -m hefl_b200 --clients-per-rank 8 --dirichlet-alpha 0.3 --personal-layers 3 --personal-head-epochs 2
     # after training, class probabilities and a Grad-CAM heatmap of every test scan (DESIGN.md §11)
     python -m hefl_b200 --data-dir image/Train --test-dir image/Test --gradcam-dir cams --gradcam-stage 4
+    # after training, pixel-level Integrated Gradients of every test scan, 32 path points (DESIGN.md §12)
+    python -m hefl_b200 --data-dir image/Train --test-dir image/Test --ig-dir attributions --ig-steps 32
 
 Every ``FLConfig`` field is a flag (``--local-epochs 10``) or an environment variable
 (``HEFL_LOCAL_EPOCHS=10``); the reference hard-codes all of them (FLPyfhelin.py:31-36, notebook N:24-32).
@@ -29,6 +31,10 @@ rank 0's first client's personal model, named by ``"client"``),
 predicted, p_0 .. p_{C-1} — and one PNG per test scan blended with its Grad-CAM map, then prints
 ``{"gradcam_dir", "images", "stage"}``), ``--gradcam-stage s`` (the conv stage of the map, default 4),
 ``--gradcam-class c`` (the explained class; default each scan's predicted class),
+``--ig-dir DIR`` (needs ``--test-dir``; after the metrics, rank 0 writes ``DIR/attributions.csv`` — file, label,
+target, p_target, score, baseline_score, attribution_sum, gap — and one PNG per test scan blended with its positive
+Integrated Gradients attributions, then prints ``{"ig_dir", "images", "steps"}``), ``--ig-steps m`` (path points,
+1..1024, default 32), ``--ig-class c`` (the explained class; default each scan's predicted class),
 ``--checkpoint PATH`` (written by rank 0 after every round, resumed from if it exists),
 ``--simulate`` (all ``--clients`` in this one process through the loopback transport: the reference's own
 structure, clients as loop iterations, FLPyfhelin.py:184).
@@ -59,10 +65,15 @@ def main(argv=None) -> int:
     extra.add_argument("--gradcam-dir", default=None)
     extra.add_argument("--gradcam-stage", type=int, default=4)
     extra.add_argument("--gradcam-class", type=int, default=None)
+    extra.add_argument("--ig-dir", default=None)
+    extra.add_argument("--ig-steps", type=int, default=32)
+    extra.add_argument("--ig-class", type=int, default=None)
     extra.add_argument("-h", "--help", action="store_true")
     ns, rest = extra.parse_known_args(argv)
     if ns.gradcam_dir and not ns.test_dir:
         extra.error("--gradcam-dir explains the scans of --test-dir: give --test-dir DIR as well")
+    if ns.ig_dir and not ns.test_dir:
+        extra.error("--ig-dir attributes the scans of --test-dir: give --test-dir DIR as well")
     if ns.help:
         print(__doc__)
         print("FLConfig fields:", ", ".join(f.name for f in __import__("dataclasses").fields(FLConfig)))
@@ -117,6 +128,10 @@ def main(argv=None) -> int:
         from .fl.explain import check_gradcam
 
         check_gradcam(run.model, ns.gradcam_stage, ns.gradcam_class, 1)     # before training, not after it
+    if ns.ig_dir:
+        from .fl.explain import check_ig
+
+        check_ig(run.model, ns.ig_steps, ns.ig_class, 1)
     if ns.checkpoint and os.path.exists(ns.checkpoint):
         run.load_checkpoint(ns.checkpoint)
         if rank == 0:
@@ -149,6 +164,11 @@ def main(argv=None) -> int:
             from .fl.explain import write_explanations
 
             print(json.dumps(write_explanations(run, ns.test_dir, ns.gradcam_dir, ns.gradcam_stage, ns.gradcam_class,
+                                                client=0 if cfg.personal_layers else None)))
+        if ns.ig_dir:
+            from .fl.explain import write_attributions
+
+            print(json.dumps(write_attributions(run, ns.test_dir, ns.ig_dir, ns.ig_steps, ns.ig_class,
                                                 client=0 if cfg.personal_layers else None)))
     if world > 1:
         dist.barrier()

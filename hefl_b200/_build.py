@@ -49,6 +49,7 @@ CUDA_SOURCES = [
     "nn/wgrad0_mma.cu",
     "nn/head_cluster.cu",
     "nn/gradcam.cu",
+    "nn/input_grad.cu",
 ]
 HOST_SOURCES = [
     "he/host_math.cpp",

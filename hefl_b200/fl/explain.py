@@ -1,5 +1,5 @@
 """Grad-CAM (Selvaraju et al. 2017) for the sequential CNNs: class probabilities and a heatmap of where the model
-looked, per scan (DESIGN.md §11).
+looked, per scan (DESIGN.md §11); and pixel-level Integrated Gradients (Sundararajan et al. 2017, DESIGN.md §12).
 
 For stage s (the output X[s] of the s-th [Conv 3x3 + ReLU -> MaxPool 2x2] block, [N, C, Hp, Hp]) and a target class
 t_b per scan (-1: the predicted class, the arg-max of the logits with the lowest index on ties):
@@ -23,16 +23,17 @@ import torch.nn.functional as F
 from ..models.cnn import _SeqCNN
 
 Target = Optional[Union[int, torch.Tensor]]
+MAX_IG_STEPS = 1024
 
 
-def check_gradcam(model, stage: int, target: Target, n: int) -> torch.Tensor:
-    """Reject what Grad-CAM cannot explain and return the targets of ``n`` scans as int64 [n] (-1 = predicted class)."""
+def _check_model(model, what: str) -> None:
     if not isinstance(model, _SeqCNN):
-        raise ValueError(f"Grad-CAM supports the sequential CNNs (medcnn, cnn2), not {type(model).__name__}: the "
+        raise ValueError(f"{what} supports the sequential CNNs (medcnn, cnn2), not {type(model).__name__}: the "
                          "ResNets (resnet18, resnet50) would need a BatchNorm backward without statistics updates")
-    stages = len(model.convs)
-    if isinstance(stage, bool) or not isinstance(stage, int) or not 1 <= stage <= stages:
-        raise ValueError(f"stage must be an integer in 1..{stages} for this model, got {stage!r}")
+
+
+def check_target(model, target: Target, n: int) -> torch.Tensor:
+    """The explained class of each of ``n`` scans as int64 [n] (-1 = the predicted class); rejects classes >= C."""
     C = model.num_classes
     if target is None:
         t = torch.full((n,), -1, dtype=torch.int64)
@@ -46,6 +47,15 @@ def check_gradcam(model, stage: int, target: Target, n: int) -> torch.Tensor:
         raise ValueError(f"target classes must be in 0..{C - 1} (or -1 for the predicted class), got "
                          f"{int(t.min())}..{int(t.max())}")
     return t
+
+
+def check_gradcam(model, stage: int, target: Target, n: int) -> torch.Tensor:
+    """Reject what Grad-CAM cannot explain and return the targets of ``n`` scans as int64 [n] (-1 = predicted class)."""
+    _check_model(model, "Grad-CAM")
+    stages = len(model.convs)
+    if isinstance(stage, bool) or not isinstance(stage, int) or not 1 <= stage <= stages:
+        raise ValueError(f"stage must be an integer in 1..{stages} for this model, got {stage!r}")
+    return check_target(model, target, n)
 
 
 def gradcam_torch(model, x_u8: torch.Tensor, stage: int = 4, target: Target = None) -> Tuple[torch.Tensor, torch.Tensor]:
@@ -77,6 +87,45 @@ def gradcam_torch(model, x_u8: torch.Tensor, stage: int = 4, target: Target = No
     mx = cam.amax(dim=(1, 2))
     cams = torch.where(mx[:, None, None] > 0, up / torch.where(mx > 0, mx, 1)[:, None, None], torch.zeros_like(up))
     return torch.softmax(logits.detach(), dim=1), cams
+
+
+def check_ig(model, steps: int, target: Target, n: int) -> torch.Tensor:
+    """Reject what Integrated Gradients cannot explain and return the targets of ``n`` scans as int64 [n]."""
+    _check_model(model, "Integrated Gradients")
+    if isinstance(steps, bool) or not isinstance(steps, int) or not 1 <= steps <= MAX_IG_STEPS:
+        raise ValueError(f"steps must be an integer in 1..{MAX_IG_STEPS}, got {steps!r}")
+    return check_target(model, target, n)
+
+
+def _ig_torch(model, x_u8: torch.Tensor, steps: int, t: torch.Tensor):
+    """(probs, attr, score, baseline score, resolved targets) of the definition in ``integrated_gradients_torch``."""
+    p = next(model.parameters())
+    dtype, dev = p.dtype, p.device
+    xh = x_u8.to(dev).permute(0, 3, 1, 2).to(dtype) * (1.0 / 255.0)
+    with torch.no_grad():
+        logits = model(xh)
+        base = model(torch.zeros_like(xh))
+    t = t.to(dev)
+    t = torch.where(t < 0, logits.argmax(1), t)
+    total = torch.zeros_like(xh)
+    with torch.enable_grad():
+        for k in range(1, steps + 1):
+            xk = (xh * ((k - 0.5) / steps)).requires_grad_(True)
+            gk, = torch.autograd.grad(model(xk).gather(1, t[:, None]).sum(), xk)
+            total += gk
+    attr = (xh * total).sum(1) / steps
+    return (torch.softmax(logits, dim=1), attr, logits.gather(1, t[:, None])[:, 0],
+            base.gather(1, t[:, None])[:, 0], t)
+
+
+def integrated_gradients_torch(model, x_u8: torch.Tensor, steps: int = 32,
+                               target: Target = None) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
+    """(probs [N, C], attr [N, S, S], gap [N]) of the uint8 NHWC scans ``x_u8``, in the dtype of the model and on its
+    device: Integrated Gradients against the black image with ``steps`` midpoint-rule path points. ``target``: None
+    (each scan's predicted class), an int, or N ints (-1 = predicted)."""
+    t = check_ig(model, steps, target, x_u8.shape[0])
+    probs, attr, score, base, _ = _ig_torch(model, x_u8, steps, t)
+    return probs, attr, attr.sum((1, 2)) - (score - base)
 
 
 def heat_overlay(img_u8, cam, weight: float = 0.5):
@@ -125,3 +174,42 @@ def write_explanations(run, test_dir: str, out_dir: str, stage: int, target: Opt
                 png = f"{i + k:06d}_{os.path.splitext(os.path.basename(name))[0]}.png"
                 Image.fromarray(heat_overlay(x[k].numpy(), cams[k].numpy())).save(os.path.join(out_dir, png))
     return {"gradcam_dir": out_dir, "images": len(ds), "stage": stage}
+
+
+def write_attributions(run, test_dir: str, out_dir: str, steps: int, target: Optional[int] = None,
+                       client: Optional[int] = None, chunk: int = 256) -> dict:
+    """``out_dir/attributions.csv`` (file, label, target, p_target, score, baseline_score, attribution_sum, gap) and
+    one PNG per scan of the image folder ``test_dir`` (``<label>/<file>``): the scan blended with a heat ramp of its
+    positive Integrated Gradients attributions over their 99th percentile, clipped to [0, 1] (0 for a scan with no
+    positive attribution). The folder is decoded ``chunk`` scans at a time. Returns the JSON summary."""
+    import csv
+    import os
+
+    from PIL import Image
+
+    from .data import ImageFolderDataset
+
+    cfg = run.cfg
+    ds = ImageFolderDataset(test_dir, cfg.image_size, cfg.in_channels, shuffle_seed=None, pin=False, stream=True)
+    os.makedirs(out_dir, exist_ok=True)
+    root = os.path.abspath(test_dir)
+    buf = torch.empty(min(chunk, len(ds)), cfg.image_size, cfg.image_size, cfg.in_channels, dtype=torch.uint8)
+    with open(os.path.join(out_dir, "attributions.csv"), "w", newline="") as fh:
+        w = csv.writer(fh)
+        w.writerow(["file", "label", "target", "p_target", "score", "baseline_score", "attribution_sum", "gap"])
+        for i in range(0, len(ds), chunk):
+            n = min(chunk, len(ds) - i)
+            x = buf[:n]
+            ds.load_batch(torch.arange(i, i + n), x)
+            probs, attr, gap, t, score, base = run._attribute(x, steps, target, client)
+            for k in range(n):
+                name = os.path.relpath(ds.filenames[i + k], root)
+                tk = int(t[k])
+                w.writerow([name, int(ds.labels[i + k]), tk, repr(float(probs[k, tk])), repr(float(score[k])),
+                            repr(float(base[k])), repr(float(attr[k].double().sum())), repr(float(gap[k]))])
+                pos = attr[k].clamp_min(0)
+                q = float(torch.quantile(pos[pos > 0], 0.99)) if bool((pos > 0).any()) else 0.0
+                heat = (pos / q).clamp(0, 1) if q > 0 else torch.zeros_like(pos)
+                png = f"{i + k:06d}_{os.path.splitext(os.path.basename(name))[0]}.png"
+                Image.fromarray(heat_overlay(x[k].numpy(), heat.numpy())).save(os.path.join(out_dir, png))
+    return {"ig_dir": out_dir, "images": len(ds), "steps": steps}

@@ -38,7 +38,7 @@ from ..models.cnn import MedCNN, SmallCNN
 from ..parallel import LoopbackTransport, make_transport
 from ..utils import DeviceTimer, JsonlLogger, StageTimes
 from .data import BatchFeeder, SyntheticImageDataset, dirichlet_partition, shard_range, split_train_val
-from .explain import check_gradcam, gradcam_torch
+from .explain import _ig_torch, check_gradcam, check_ig, gradcam_torch
 from .server_opt import ServerOptimizer, check_server_options, reference_step
 from .trainer import LocalTrainer
 
@@ -741,11 +741,9 @@ class FederatedRunner:
         with self._client_head(client):
             N = int(images_u8.shape[0])
             targets = check_gradcam(self.model, stage, target, N)
+            self._check_images(images_u8)
             cfg = self.cfg
             S, C = cfg.image_size, self.model.num_classes
-            if tuple(images_u8.shape[1:]) != (S, S, cfg.in_channels) or images_u8.dtype != torch.uint8:
-                raise ValueError(f"images must be uint8 [N, {S}, {S}, {cfg.in_channels}], got "
-                                 f"{tuple(images_u8.shape)} {images_u8.dtype}")
             probs = torch.empty(N, C, dtype=torch.float32)
             cams = torch.empty(N, S, S, dtype=torch.float32)
             eng = self.trainer.engine
@@ -772,6 +770,68 @@ class FederatedRunner:
                 probs[i:i + nv] = torch.softmax(logits[:nv].cpu(), dim=1)
                 cams[i:i + nv] = cam[:nv].cpu()
             return probs, cams
+
+    def _check_images(self, images_u8: torch.Tensor) -> None:
+        S, ch = self.cfg.image_size, self.cfg.in_channels
+        if tuple(images_u8.shape[1:]) != (S, S, ch) or images_u8.dtype != torch.uint8:
+            raise ValueError(f"images must be uint8 [N, {S}, {S}, {ch}], got {tuple(images_u8.shape)} "
+                             f"{images_u8.dtype}")
+
+    def attribute(self, images_u8: torch.Tensor, steps: int = 32, target=None, client: Optional[int] = None,
+                  batch_size: Optional[int] = None):
+        """Integrated Gradients of the installed model (DESIGN.md §12): ``(probs [N, C], attr [N, S, S], gap [N])``,
+        all fp32 on the CPU, for uint8 NHWC scans ``images_u8`` [N, S, S, in_channels]. ``attr`` is the pixel-level
+        attribution of the class score against the black image, summed over the input channels, with ``steps``
+        (1..1024) midpoint-rule path points; ``gap`` is its completeness error, sum(attr) - (score - black score).
+        ``target``: None (each scan's predicted class), an int, or N class indices (-1 = predicted). ``client`` and
+        ``batch_size``: as in ``explain``; the engine uses input slots 0 and 1. Not to be called while ``fit`` runs;
+        the weights, optimiser state, augmentation position and RNG are left as they were."""
+        return self._attribute(images_u8, steps, target, client, batch_size)[:3]
+
+    def _attribute(self, images_u8, steps, target, client, batch_size=None):
+        """``attribute``'s results followed by the resolved targets, the scores and the black image's scores (int64
+        and fp32 [N], CPU)."""
+        with self._client_head(client):
+            N = int(images_u8.shape[0])
+            targets = check_ig(self.model, steps, target, N)
+            self._check_images(images_u8)
+            cfg = self.cfg
+            S, C = cfg.image_size, self.model.num_classes
+            probs = torch.empty(N, C, dtype=torch.float32)
+            attr = torch.empty(N, S, S, dtype=torch.float32)
+            tres = torch.empty(N, dtype=torch.int64)
+            score = torch.empty(N, dtype=torch.float32)
+            base = torch.empty(N, dtype=torch.float32)
+            eng = self.trainer.engine
+            if eng is None:
+                bs = batch_size or cfg.batch_size
+                for i in range(0, N, bs):
+                    r = _ig_torch(self.model, images_u8[i:i + bs], steps, targets[i:i + bs])
+                    for dst, v in zip((probs, attr, score, base, tres), r):
+                        dst[i:i + bs] = v.detach().to("cpu", dst.dtype)
+            else:
+                B, dev = eng.B, self.device
+                x = torch.zeros(B, S, S, cfg.in_channels, dtype=torch.uint8, device=dev)
+                tgt = torch.full((B,), -1, dtype=torch.int64, device=dev)
+                logits = torch.zeros(B, C, dtype=torch.float32, device=dev)
+                blog = torch.zeros(B, C, dtype=torch.float32, device=dev)
+                att = torch.zeros(B, S, S, dtype=torch.float32, device=dev)
+                for i in range(0, N, B):
+                    nv = min(B, N - i)
+                    if nv < B:                                   # padding rows: attributed, never written back
+                        x.zero_()
+                        tgt.fill_(-1)
+                    x[:nv].copy_(images_u8[i:i + nv])
+                    tgt[:nv].copy_(targets[i:i + nv])
+                    eng.preprocess(x, 1, False, False)
+                    t = eng.ig_staged(steps, tgt, logits, blog, att, nv)[:nv, None]
+                    probs[i:i + nv] = torch.softmax(logits[:nv].cpu(), dim=1)
+                    attr[i:i + nv] = att[:nv].cpu()
+                    tres[i:i + nv] = t[:, 0].cpu()
+                    score[i:i + nv] = logits[:nv].gather(1, t)[:, 0].cpu()
+                    base[i:i + nv] = blog[:nv].gather(1, t)[:, 0].cpu()
+            gap = (attr.double().sum((1, 2)) - (score.double() - base.double())).float()
+            return probs, attr, gap, tres, score, base
 
     # ------------------------------------------------------------------ checkpoint / resume
     def save_checkpoint(self, path: str) -> None:

@@ -25,6 +25,9 @@ Replaces Keras' ``model.fit`` compute path (FLPyfhelin.py:118-136, :193) for the
             depth that yields the personal layers' gradients only, Adam over the personal layers
   Grad-CAM  (``gradcam_staged``, DESIGN.md §11) forward convs (arg-max codes from the explained stage on), the head
             seeded with a class score (head_saliency), the un-pool / dgrad chain down to that stage, gradcam
+  IG        (``ig_staged``, DESIGN.md §12) per path point: the scan in slot 1 scaled into slot 0, forward convs
+            with every arg-max code, the head seeded with a class score, the un-pool / dgrad chain down to X[1],
+            input_grad0 (the layer-1 input gradient straight from the pooled gradient, into an fp32 accumulator)
 
 All buffers are allocated once; a step is CUDA-graph capturable (one graph per input slot); every
 kernel uses programmatic dependent launch (csrc/nn/launch.cuh).
@@ -162,6 +165,7 @@ class MedCNNEngine:
         self.theta = torch.zeros(B, 2, 3, dtype=torch.float32, device=device)
         self.aug_seed = (cfg.seed * 2654435761 + 12345) & 0x7FFFFFFFFFFFFFFF or 1
         self.prep_count = 0          # augmented batches pre-processed so far (keys the in-kernel Philox draw)
+        self.ig_acc = None           # Integrated Gradients: fp32 [B, S, S, Ci] sum of the path's input gradients (lazy)
         # weight gradients run on a side stream, concurrently with the dgrad / un-pool chain
         self.side = torch.cuda.Stream(device)
         self.after_restore()
@@ -366,16 +370,12 @@ class MedCNNEngine:
         opt.bump()
         opt.apply(self.head_lo, self.pack.n_trainable)
 
-    def gradcam_staged(self, slot: int, stage: int, target: torch.Tensor, logits_out: torch.Tensor,
-                       cam_out: torch.Tensor, nvalid: int) -> None:
-        """Grad-CAM (DESIGN.md §11) of the batch pre-processed into ``slot`` (``preprocess(.., train=False,
-        augment=False)``): ``logits_out`` [B, C] fp32 and ``cam_out`` [>= nvalid, S, S] fp32, the first ``nvalid`` maps.
-        ``target`` int64 [B] on the device: the class whose score is explained per scan, -1 for the predicted one.
-        ``stage`` 1..n is the pooled output X[stage] the map is taken at. Runs no weight gradient, finalize, Adam or
-        relayout: only X, amax, dY, gX, dfeat and the head scratch change."""
-        if not 1 <= stage <= self.n:
-            raise ValueError(f"stage must be in 1..{self.n}, got {stage}")
-        feat_bf = self.forward_convs(slot, True, codes_from=stage)
+    def _saliency(self, slot: int, stage: int, codes_from: int, target: torch.Tensor,
+                  logits_out: torch.Tensor) -> torch.Tensor:
+        """Forward convs on the input of ``slot`` (arg-max codes of layers ``codes_from`` .. n-1), the head seeded with
+        the class score of ``target`` (head_saliency; -1: the arg-max), ``logits_out`` [B, C] fp32, and the un-pool /
+        dgrad chain down to stage ``stage`` (1..n). Returns d logits[b, t_b] / d X[stage] (bf16, X[stage]'s shape)."""
+        feat_bf = self.forward_convs(slot, True, codes_from=codes_from)
         if self.fused_head:
             self.ops.head_saliency(feat_bf, self.pack.flat, self.head_offs, target, self.dfeat, self.h1_buf,
                                    self.dh1_buf, logits_out, self.B, self.F, self.H1, self.H2, self.C)
@@ -393,7 +393,53 @@ class MedCNNEngine:
             self.ops.unpool_relu(g, self.amax[l], self.X[l + 1], self.dY[l], self.B, h, h, self.Co[l])
             self.ops.conv_dgrad(self.dY[l], self._wd(l), self.gX[l], self.B, h, h, self.Co[l], self.Ci[l])
             g = self.gX[l]
+        return g
+
+    def gradcam_staged(self, slot: int, stage: int, target: torch.Tensor, logits_out: torch.Tensor,
+                       cam_out: torch.Tensor, nvalid: int) -> None:
+        """Grad-CAM (DESIGN.md §11) of the batch pre-processed into ``slot`` (``preprocess(.., train=False,
+        augment=False)``): ``logits_out`` [B, C] fp32 and ``cam_out`` [>= nvalid, S, S] fp32, the first ``nvalid`` maps.
+        ``target`` int64 [B] on the device: the class whose score is explained per scan, -1 for the predicted one.
+        ``stage`` 1..n is the pooled output X[stage] the map is taken at. Runs no weight gradient, finalize, Adam or
+        relayout: only X, amax, dY, gX, dfeat and the head scratch change."""
+        if not 1 <= stage <= self.n:
+            raise ValueError(f"stage must be in 1..{self.n}, got {stage}")
+        g = self._saliency(slot, stage, stage, target, logits_out)
         self.ops.gradcam(self.X[stage], g, cam_out, self.B, self.H[stage], self.Co[stage - 1], self.H[0], nvalid)
+
+    def ig_staged(self, steps: int, target: torch.Tensor, logits_out: torch.Tensor, base_out: torch.Tensor,
+                  attr_out: torch.Tensor, nvalid: int) -> torch.Tensor:
+        """Integrated Gradients (DESIGN.md §12) of the batch pre-processed into slot 1 (``preprocess(.., 1,
+        train=False, augment=False)``), black baseline, midpoint rule with ``steps`` points. ``target`` int64 [B] on
+        the device (-1: the class predicted at the scan); returns it resolved. ``logits_out`` / ``base_out`` [B, C]
+        fp32: the logits at the scan and at the black image. ``attr_out`` [>= nvalid, S, S] fp32, the first ``nvalid``
+        maps: sum over channels of x * (1/steps) sum_k d logit_t / d x at x_k = bf16(alpha_k x), alpha_k =
+        (k - 1/2) / steps; ``ig_acc`` keeps the sum over k. Path points are scaled into slot 0. Runs no weight
+        gradient, finalize, Adam or relayout: only slot 0, X, amax, dY, gX, dfeat, the head scratch and ig_acc change."""
+        if self.Co[0] != 32:
+            raise ValueError(f"input_grad0 handles a first conv of 32 filters, this model has {self.Co[0]}")
+        if not 1 <= steps <= 1024:
+            raise ValueError(f"steps must be in 1..1024, got {steps}")
+        B, S, ci, n = self.B, self.H[0], self.Ci[0], self.n
+        if self.ig_acc is None:
+            self.ig_acc = torch.zeros(B, S, S, ci, dtype=torch.float32, device=self.device)
+        x1, x0 = self.x0(1), self.x0(0)
+        self._saliency(1, n, n, target, logits_out)
+        t = torch.where(target < 0, logits_out.argmax(1), target)
+        torch.mul(x1, 0.0, out=x0)
+        self._saliency(0, n, n, t, base_out)
+        w_off = int(self.table[0, 3])
+        w0 = self.shadow[w_off: w_off + self.Co[0] * ci * 9]           # layer 1's [Co][Ci][3][3], as the forward used
+        acc = self.ig_acc
+        acc[:nvalid].zero_()
+        scratch = torch.empty_like(logits_out)
+        for k in range(1, steps + 1):
+            torch.mul(x1, (k - 0.5) / steps, out=x0)          # fp32 opmath, rounded to bf16 in every layer-1 layout
+            g = self._saliency(0, 1, 0, t, scratch)
+            self.ops.input_grad0(g, self.amax[0], w0, acc, B, S, ci, nvalid)
+        xh = x1[: self.P[0], :ci].view(B, S, S, ci)
+        attr_out[:nvalid] = (xh[:nvalid].float() * acc[:nvalid]).sum(-1) / steps
+        return t
 
     def eval_step(self, x_u8: torch.Tensor, y: torch.Tensor, out: torch.Tensor) -> None:
         self.preprocess(x_u8, 0, False, False)

@@ -18,6 +18,8 @@
 // dW3 / db3. Every early exit follows the last cluster barrier after which no CTA writes into another's shared memory.
 // depth 5 (kHeadSaliency, Grad-CAM, DESIGN.md §11) seeds the backward with the one-hot of a target class (-1: the
 // arg-max of the logits) instead of p - y, CTA 0 writes the logits, and P3-P5 skip every dW / db: dfeat only.
+// depth 6 (kHeadScore, federated evaluation, DESIGN.md §13) runs P1-P3, CTA 0 writes the logits, and the kernel exits
+// where depth 0 exits: no label is read and no loss, gradient or dfeat is written.
 // Four cluster barriers replace three kernel boundaries; nothing but parameters gradients, dfeat and the
 // two result scalars touches global memory.
 #include <cooperative_groups.h>
@@ -67,8 +69,9 @@ struct HeadClusterArgs {
   float *gW1, *gb1, *gW2, *gb2, *gW3, *gb3;
   __nv_bfloat16* dfeat;        // [B][F]
   float* out;                  // [2] loss, ncorrect
-  float* logits;               // [B][C], kHeadSaliency only
-  int B, C, depth;           // 0 eval, 1 full backward, 2 / 3 / 4 stop after dW1 / dW2 / dW3 (no dfeat), kHeadSaliency
+  float* logits;               // [B][C], kHeadSaliency and kHeadScore only
+  int B, C, depth;           // 0 eval, 1 full backward, 2 / 3 / 4 stop after dW1 / dW2 / dW3 (no dfeat), kHeadSaliency,
+                             // kHeadScore
 };
 
 __global__ void __launch_bounds__(hc::NT, 1) head_cluster_kernel(const HeadClusterArgs a) {
@@ -235,14 +238,18 @@ __global__ void __launch_bounds__(hc::NT, 1) head_cluster_kernel(const HeadClust
       for (int c = 0; c < C; ++c) if (lgS[t * CM + c] > mx) { mx = lgS[t * CM + c]; am = c; }
       float s = 0.f;
       for (int c = 0; c < C; ++c) s += __expf(lgS[t * CM + c] - mx);
-      const int yy = (int)a.y[t];
-      if (a.depth == kHeadSaliency) {                        // d logits[t, target] / d logits: one-hot
+      if (a.depth == kHeadScore) {                           // logits only: no labels, loss or backward
+        if (r == 0)
+          for (int c = 0; c < C; ++c) a.logits[t * C + c] = lgS[t * CM + c];
+      } else if (a.depth == kHeadSaliency) {                 // d logits[t, target] / d logits: one-hot
+        const int yy = (int)a.y[t];
         const int tt = yy < 0 ? am : yy;
         for (int c = 0; c < C; ++c) {
           if (r == 0) a.logits[t * C + c] = lgS[t * CM + c];
           lgS[t * CM + c] = c == tt ? 1.f : 0.f;
         }
       } else {
+        const int yy = (int)a.y[t];
         l = -(lgS[t * CM + yy] - mx - __logf(s));
         nc = am == yy ? 1.f : 0.f;
         const float invB = 1.f / B;
@@ -256,13 +263,13 @@ __global__ void __launch_bounds__(hc::NT, 1) head_cluster_kernel(const HeadClust
       l += __shfl_xor_sync(0xffffffffu, l, off);
       nc += __shfl_xor_sync(0xffffffffu, nc, off);
     }
-    if (t == 0 && r == 0 && a.depth != kHeadSaliency) {
+    if (t == 0 && r == 0 && a.depth < kHeadSaliency) {
       a.out[0] = l / B;
       a.out[1] = nc;
     }
   }
   __syncthreads();
-  if (!a.depth) return;          // nobody writes into this CTA's shared memory after the P2 barrier
+  if (!a.depth || a.depth == kHeadScore) return;   // nobody writes into this CTA's shared memory after the P2 barrier
   const bool params = a.depth != kHeadSaliency;
   if (r == 0 && params) {
     for (int o = t; o < C * H2 + C; o += NT) {

@@ -44,6 +44,9 @@ void conv_dgrad_wgrad(const void* X, const void* dY, const void* Wd, void* dX, f
 // logits [B][C] are written, the backward is seeded with d logits[b, y_b] instead of the loss and yields dfeat only:
 // no parameter gradient, no loss (gW* and out are not touched).
 constexpr int kHeadSaliency = 5;
+// kHeadScore (federated evaluation): the forward only; logits [B][C] are written, y is not read, and no loss, gradient
+// or dfeat is written.
+constexpr int kHeadScore = 6;
 void head_forward_backward(const void* feat, const float* W1, const float* b1, const float* W2, const float* b2,
                            const float* W3, const float* b3, const int64_t* y, float* gW1, float* gb1, float* gW2,
                            float* gb2, float* gW3, float* gb3, void* dfeat, float* h1_buf, float* dh1_buf,
@@ -66,6 +69,14 @@ void gradcam(const void* X, const void* G, float* out, int Hp, int C, int S, int
 // with w, in_channels 1 or 3. Scans >= nvalid are neither read nor written.
 void input_grad0(const void* g, const uint8_t* amax, const void* w, float* acc, int S, int Hp, int in_channels,
                  int nvalid, cudaStream_t st);
+// ---- federated evaluation counts (score.cu, DESIGN.md §13) ----
+// logits fp32 [B][C], labels int64 [B], *nvalid (device): rows >= nvalid are neither read nor written. probs fp32
+// [B][C] = softmax(logits). counts int32 [C*C + C*C*nbins] += the confusion matrix conf[t][argmax] and the score
+// histograms hist[t][c][min(nbins - 1, floor(p_c * nbins))]; *loss_sum (fp64) += the cross-entropy of the rows, summed
+// in a fixed order by one thread. A label outside 0..C-1 sets *err to 1 and its row adds nothing.
+constexpr int kScoreMaxClasses = 32;
+void score_stats(const float* logits, const int64_t* labels, const int* nvalid, float* probs, int* counts,
+                 double* loss_sum, int* err, int B, int C, int nbins, cudaStream_t st);
 bool wgrad0_gather_supported(int W, int Wp, int CK, int Ci, int Co);
 // layer-1 partials: [wgrad0_parts(B, Hp)][kWgrad0Part] floats of workspace
 constexpr int kWgrad0Part = 28 * 32;

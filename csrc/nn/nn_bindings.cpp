@@ -273,6 +273,60 @@ void head_saliency(const Tensor& feat, const Tensor& flat, at::IntArrayRef offs,
                                   hefl::nn::kHeadSaliency, cur());
 }
 
+// Forward of the head for federated evaluation (DESIGN.md §13): logits_out [B, C] fp32 and nothing else; no labels are
+// read and no loss, parameter gradient or dfeat is written.
+void head_logits(const Tensor& feat, const Tensor& flat, at::IntArrayRef offs, Tensor h1_buf, Tensor dh1_buf,
+                 Tensor logits_out, int64_t B, int64_t F, int64_t H1, int64_t H2, int64_t C) {
+  chk_bf16(feat, "feat");
+  TORCH_CHECK(offs.size() == 6, "need six parameter offsets");
+  TORCH_CHECK(B <= 32 && B >= 1, "the head kernels handle up to 32 samples per step");
+  TORCH_CHECK(feat.numel() == B * F, "feat must be [B,F]");
+  TORCH_CHECK(flat.is_cuda() && flat.scalar_type() == at::kFloat, "float32 parameter buffer required");
+  TORCH_CHECK(logits_out.is_cuda() && logits_out.scalar_type() == at::kFloat && logits_out.is_contiguous() &&
+              logits_out.numel() == B * C, "logits_out must be a contiguous float32 [B, C]");
+  TORCH_CHECK(h1_buf.numel() >= B * H1 && dh1_buf.numel() >= B * (H1 + H2), "scratch too small");
+  const float* p = flat.data_ptr<float>();
+  if (hefl::nn::head_cluster_supported((int)B, (int)F, (int)H1, (int)H2, (int)C)) {
+    hefl::nn::head_cluster(feat.data_ptr(), p + offs[0], p + offs[1], p + offs[2], p + offs[3], p + offs[4], p + offs[5],
+                           nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr,
+                           logits_out.data_ptr<float>(), (int)B, (int)C, hefl::nn::kHeadScore, cur());
+    return;
+  }
+  TORCH_CHECK(B % 2 == 0 && H2 % 4 == 0 && H1 % 4 == 0 && F % 8 == 0, "head dims must be even / multiples of 4 / 8");
+  hefl::nn::head_forward_backward(feat.data_ptr(), p + offs[0], p + offs[1], p + offs[2], p + offs[3], p + offs[4],
+                                  p + offs[5], nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr,
+                                  h1_buf.data_ptr<float>(), dh1_buf.data_ptr<float>(), nullptr,
+                                  logits_out.data_ptr<float>(), (int)B, (int)F, (int)H1, (int)H2, (int)C,
+                                  hefl::nn::kHeadScore, cur());
+}
+
+// One client's evaluation counts (csrc/nn/score.cu): logits fp32 [B, C], labels int64 [B], nvalid int32 [1] on the
+// device; probs_out fp32 [B, C]; counts int32 [C*C + C*C*nbins] and loss_sum fp64 [1] are added into; err int32 [1]
+// is set to 1 when a valid row's label is outside 0..C-1.
+void score_stats(const Tensor& logits, const Tensor& labels, const Tensor& nvalid, Tensor probs_out, Tensor counts,
+                 Tensor loss_sum, Tensor err, int64_t nbins) {
+  TORCH_CHECK(logits.is_cuda() && logits.scalar_type() == at::kFloat && logits.dim() == 2 && logits.is_contiguous(),
+              "logits must be a contiguous float32 [B, C] CUDA tensor");
+  const int64_t B = logits.size(0), C = logits.size(1);
+  TORCH_CHECK(C >= 1 && C <= hefl::nn::kScoreMaxClasses, "score_stats handles 1..32 classes, got ", C);
+  TORCH_CHECK(nbins >= 2 && nbins <= 1024, "nbins must be in 2..1024, got ", nbins);
+  TORCH_CHECK(B >= 1 && B <= (1 << 20), "score_stats: B must be in 1..2^20");
+  TORCH_CHECK(labels.scalar_type() == at::kLong && labels.is_contiguous() && labels.numel() == B, "labels must be int64 [B]");
+  TORCH_CHECK(nvalid.scalar_type() == at::kInt && nvalid.numel() == 1, "nvalid must be an int32 [1] device tensor");
+  TORCH_CHECK(probs_out.scalar_type() == at::kFloat && probs_out.is_contiguous() && probs_out.numel() == B * C,
+              "probs_out must be a contiguous float32 [B, C]");
+  TORCH_CHECK(counts.scalar_type() == at::kInt && counts.is_contiguous() && counts.numel() == C * C + C * C * nbins,
+              "counts must be a contiguous int32 [C*C + C*C*nbins]");
+  TORCH_CHECK(loss_sum.scalar_type() == at::kDouble && loss_sum.numel() == 1, "loss_sum must be a float64 [1]");
+  TORCH_CHECK(err.scalar_type() == at::kInt && err.numel() == 1, "err must be an int32 [1]");
+  for (const Tensor* t : {&labels, &nvalid, static_cast<const Tensor*>(&probs_out), static_cast<const Tensor*>(&counts),
+                          static_cast<const Tensor*>(&loss_sum), static_cast<const Tensor*>(&err)})
+    TORCH_CHECK(t->device() == logits.device(), "score_stats: every tensor must be on the logits' device");
+  hefl::nn::score_stats(logits.data_ptr<float>(), labels.data_ptr<int64_t>(), nvalid.data_ptr<int>(),
+                        probs_out.data_ptr<float>(), counts.data_ptr<int>(), loss_sum.data_ptr<double>(),
+                        err.data_ptr<int>(), (int)B, (int)C, (int)nbins, cur());
+}
+
 // Grad-CAM maps (csrc/nn/gradcam.cu): X, G bf16 [B*Hp*Hp, C]; out fp32 with at least nvalid * S * S elements, of which
 // the first nvalid maps are written.
 void gradcam(const Tensor& X, const Tensor& G, Tensor out, int64_t B, int64_t Hp, int64_t C, int64_t S, int64_t nvalid) {
@@ -542,6 +596,8 @@ TORCH_LIBRARY_FRAGMENT(hefl, m) {
   m.def("unpool_relu(Tensor g, Tensor amax, Tensor ypool, Tensor(a!) dY, int B, int H, int W, int Co) -> ()", &unpool_relu);
   m.def("head_forward_backward(Tensor feat, Tensor flat, Tensor(a!) grad, int[] offs, Tensor y, Tensor(b!) dfeat, Tensor(c!) h1_buf, Tensor(d!) dh1_buf, Tensor(e!) out, int B, int F, int H1, int H2, int C, int depth) -> ()", &head_forward_backward);
   m.def("head_saliency(Tensor feat, Tensor flat, int[] offs, Tensor target, Tensor(a!) dfeat, Tensor(b!) h1_buf, Tensor(c!) dh1_buf, Tensor(d!) logits_out, int B, int F, int H1, int H2, int C) -> ()", &head_saliency);
+  m.def("head_logits(Tensor feat, Tensor flat, int[] offs, Tensor(a!) h1_buf, Tensor(b!) dh1_buf, Tensor(c!) logits_out, int B, int F, int H1, int H2, int C) -> ()", &head_logits);
+  m.def("score_stats(Tensor logits, Tensor labels, Tensor nvalid, Tensor(a!) probs_out, Tensor(b!) counts, Tensor(c!) loss_sum, Tensor(d!) err, int nbins) -> ()", &score_stats);
   m.def("gradcam(Tensor X, Tensor G, Tensor(a!) out, int B, int Hp, int C, int S, int nvalid) -> ()", &gradcam);
   m.def("input_grad0(Tensor g, Tensor amax, Tensor w, Tensor(a!) acc, int B, int S, int in_channels, int nvalid) -> ()", &input_grad0);
   m.def("conv_set_debug(int mask) -> ()", &conv_set_debug);

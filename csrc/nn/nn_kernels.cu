@@ -410,7 +410,8 @@ void conv_grad_finalize(float* dW32, const ConvLayerTable& t, float* grad, int l
 //   k4  dW1, db1, dfeat (column slices of 16)                      grid F/16
 // A head-only step (depth 2 / 3 / 4, DESIGN.md §10) skips dfeat, k4, or k3 and k4 with k2's dh2. Grad-CAM
 // (kHeadSaliency, DESIGN.md §11) seeds k2's dlogits with a one-hot target, writes the logits and runs k3 and k4 without
-// their dW / db (null gradient pointers).
+// their dW / db (null gradient pointers). Federated evaluation (kHeadScore, DESIGN.md §13) runs k1 and k2 up to the
+// logits, which it writes, and nothing after them.
 // ------------------------------------------------------------------------------------------
 namespace hefl {
 namespace nn {
@@ -476,7 +477,7 @@ struct HeadMidArgs {
   float *gW3, *gb3;
   float* dh2;           // [B][H2] out
   float* out;           // [2]: loss, ncorrect
-  float* logits;        // [B][C], kHeadSaliency only
+  float* logits;        // [B][C], kHeadSaliency and kHeadScore only
   int B, H1, H2, C, depth;
 };
 
@@ -553,14 +554,17 @@ head_mid_kernel(const HeadMidArgs a) {
       for (int c = 0; c < C; ++c) if (lg[tid * C + c] > mx) { mx = lg[tid * C + c]; am = c; }
       float s = 0.f;
       for (int c = 0; c < C; ++c) s += __expf(lg[tid * C + c] - mx);
-      const int yy = (int)a.y[tid];
-      if (a.depth == kHeadSaliency) {                          // d logits[b, target] / d logits: one-hot
+      if (a.depth == kHeadScore) {                             // logits only: no labels, loss or backward
+        for (int c = 0; c < C; ++c) a.logits[tid * C + c] = lg[tid * C + c];
+      } else if (a.depth == kHeadSaliency) {                   // d logits[b, target] / d logits: one-hot
+        const int yy = (int)a.y[tid];
         const int tt = yy < 0 ? am : yy;
         for (int c = 0; c < C; ++c) {
           a.logits[tid * C + c] = lg[tid * C + c];
           lg[tid * C + c] = c == tt ? 1.f : 0.f;
         }
       } else {
+        const int yy = (int)a.y[tid];
         l = -(lg[tid * C + yy] - mx - __logf(s));
         nc = am == yy ? 1.f : 0.f;
         const float invB = 1.f / B;
@@ -574,13 +578,13 @@ head_mid_kernel(const HeadMidArgs a) {
       l += __shfl_xor_sync(0xffffffffu, l, off);
       nc += __shfl_xor_sync(0xffffffffu, nc, off);
     }
-    if (tid == 0 && a.depth != kHeadSaliency) {
+    if (tid == 0 && a.depth < kHeadSaliency) {
       a.out[0] = l / B;
       a.out[1] = nc;
     }
   }
   __syncthreads();
-  if (!a.depth) return;
+  if (!a.depth || a.depth == kHeadScore) return;
   for (int o = tid; a.depth != kHeadSaliency && o < C * H2 + C; o += nt) {   // dW3, db3
     if (o < C * H2) {
       const int c = o / H2, j = o % H2;

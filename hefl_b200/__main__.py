@@ -18,6 +18,10 @@
     python -m hefl_b200 --data-dir image/Train --test-dir image/Test --gradcam-dir cams --gradcam-stage 4
     # after training, pixel-level Integrated Gradients of every test scan, 32 path points (DESIGN.md §12)
     python -m hefl_b200 --data-dir image/Train --test-dir image/Test --ig-dir attributions --ig-steps 32
+    # federated evaluation after every round: each client scores its personal model on its shard of image/Test, only
+    # the CKKS-summed confusion matrix, ROC histograms and loss sum leave it (DESIGN.md §13)
+    python -m hefl_b200 --data-dir image/Train --fed-test-dir image/Test --clients-per-rank 4 --personal-layers 3 \\
+        --fed-eval-every 1
 
 Every ``FLConfig`` field is a flag (``--local-epochs 10``) or an environment variable
 (``HEFL_LOCAL_EPOCHS=10``); the reference hard-codes all of them (FLPyfhelin.py:31-36, notebook N:24-32).
@@ -35,6 +39,10 @@ predicted, p_0 .. p_{C-1} — and one PNG per test scan blended with its Grad-CA
 target, p_target, score, baseline_score, attribution_sum, gap — and one PNG per test scan blended with its positive
 Integrated Gradients attributions, then prints ``{"ig_dir", "images", "steps"}``), ``--ig-steps m`` (path points,
 1..1024, default 32), ``--ig-class c`` (the explained class; default each scan's predicted class),
+``--fed-test-dir DIR`` (same layout; split among the K clients as ``--data-dir`` is, IID contiguous shards or the
+Dirichlet partition under ``--dirichlet-alpha``; each client scores its deployed model on its own shard and only the
+CKKS-summed counts leave it; rank 0 prints ``{"round", "fed_eval"}`` after every evaluated round, every
+``--fed-eval-every r`` rounds or once after the last round; ``--fed-eval-bins b`` sets the ROC histogram bins),
 ``--checkpoint PATH`` (written by rank 0 after every round, resumed from if it exists),
 ``--simulate`` (all ``--clients`` in this one process through the loopback transport: the reference's own
 structure, clients as loop iterations, FLPyfhelin.py:184).
@@ -59,6 +67,7 @@ def main(argv=None) -> int:
     extra.add_argument("--checkpoint", default=None)
     extra.add_argument("--data-dir", default=None)
     extra.add_argument("--test-dir", default=None)
+    extra.add_argument("--fed-test-dir", default=None)
     extra.add_argument("--stream-decode", action="store_true",
                        help="decode images per batch (flow_from_dataframe semantics) instead of the whole shard up front")
     extra.add_argument("--simulate", action="store_true")
@@ -123,7 +132,16 @@ def main(argv=None) -> int:
                                       dirichlet_alpha=cfg.dirichlet_alpha, min_train=cfg.batch_size)
                    for cid in range(rank * M, rank * M + M)]
         cfg.num_classes = max(cfg.num_classes, dataset[0].classes)
-    run = FederatedRunner(cfg, rank=rank, world=world, device=device, dataset=dataset)
+    fed_test = None
+    if ns.fed_test_dir:
+        from .fl.data import ImageFolderDataset
+
+        # the clients' test shards, split as --data-dir is
+        fed_test = [ImageFolderDataset(ns.fed_test_dir, cfg.image_size, cfg.in_channels, index=cid,
+                                       num_clients=cfg.clients, shuffle_seed=cfg.seed, stream=ns.stream_decode,
+                                       dirichlet_alpha=cfg.dirichlet_alpha)
+                    for cid in range(rank * M, rank * M + M)]
+    run = FederatedRunner(cfg, rank=rank, world=world, device=device, dataset=dataset, test_dataset=fed_test)
     if ns.gradcam_dir:
         from .fl.explain import check_gradcam
 
@@ -147,10 +165,16 @@ def main(argv=None) -> int:
                 line["selected"] = rec["selected"]
                 line["rank0_clients"] = rec["clients"]
             print(json.dumps(line))
+            if "fed_eval" in rec:
+                print(json.dumps({"round": rec["round"], "fed_eval": _fed_line(rec["fed_eval"])}))
         if ns.checkpoint:
             run.save_checkpoint(ns.checkpoint)       # rank 0: global model; every rank: its own optimiser / RNG state
         if world > 1:
             dist.barrier()
+    if ns.fed_test_dir and not cfg.fed_eval_every:
+        fed = run.evaluate_federated()                  # a collective: every rank
+        if rank == 0:
+            print(json.dumps({"round": run.round - 1, "fed_eval": _fed_line(fed)}))
     if ns.test_dir and rank == 0:
         from .fl.data import ImageFolderDataset
 
@@ -174,6 +198,11 @@ def main(argv=None) -> int:
         dist.barrier()
         dist.destroy_process_group()
     return 0
+
+
+def _fed_line(fed: dict) -> dict:
+    """The federation's evaluation without the rank's own clients' plaintext metrics."""
+    return {k: v for k, v in fed.items() if k != "local"}
 
 
 if __name__ == "__main__":

@@ -50,6 +50,7 @@ CUDA_SOURCES = [
     "nn/head_cluster.cu",
     "nn/gradcam.cu",
     "nn/input_grad.cu",
+    "nn/score.cu",
 ]
 HOST_SOURCES = [
     "he/host_math.cpp",

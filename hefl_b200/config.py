@@ -87,6 +87,10 @@ class FLConfig:
     server_momentum: float = 0.9              # beta1
     server_beta2: float = 0.99                # beta2 (fedyogi, fedadam)
     server_tau: float = 1e-3                  # tau: adaptivity / epsilon term; v starts at tau^2
+    # federated evaluation (DESIGN.md §13): every client scores its deployed model on its own test scans, only the
+    # CKKS-summed confusion matrix, score histograms and loss sum leave it
+    fed_eval_every: int = 0                   # 0: on request only (FederatedRunner.evaluate_federated); r: every r-th round
+    fed_eval_bins: int = 100                  # score-histogram bins of the ROC AUC (2..1024)
     # HE
     he_preset: str = "n4096_l3"
     packing: str = "slots"            # slots (canonical embedding, N/2 per ct) | coeff (N per ct)

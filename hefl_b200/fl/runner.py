@@ -39,6 +39,7 @@ from ..parallel import LoopbackTransport, make_transport
 from ..utils import DeviceTimer, JsonlLogger, StageTimes
 from .data import BatchFeeder, SyntheticImageDataset, dirichlet_partition, shard_range, split_train_val
 from .explain import _ig_torch, check_gradcam, check_ig, gradcam_torch
+from .fedeval import check_fedeval_options, count_len, metrics_from_confusion, metrics_from_counts
 from .server_opt import ServerOptimizer, check_server_options, reference_step
 from .trainer import LocalTrainer
 
@@ -100,8 +101,10 @@ def check_personal_options(cfg: FLConfig) -> None:
 
 class FederatedRunner:
     def __init__(self, cfg: FLConfig, rank: int = 0, world: int = 1, group=None,
-                 device: Optional[torch.device] = None, samples_per_client: Optional[int] = None, dataset=None):
+                 device: Optional[torch.device] = None, samples_per_client: Optional[int] = None, dataset=None,
+                 test_dataset=None):
         check_noniid_options(cfg)
+        check_fedeval_options(cfg)
         check_server_options(cfg)
         check_client_options(cfg)
         check_personal_options(cfg)
@@ -175,6 +178,16 @@ class FederatedRunner:
             self.clients.append({"id": cid, "dataset": ds, "nval": nval, "per": per, "n_train": per - nval,
                                  "label_counts": counts})
         del pool
+        # federated evaluation (DESIGN.md §13): one test set per client, in id order, else its 10 % validation split
+        tests = list(test_dataset) if isinstance(test_dataset, (list, tuple)) else \
+            [test_dataset] if test_dataset is not None else None
+        if tests is not None and len(tests) != M:
+            raise ValueError(f"test_dataset: {len(tests)} datasets for {M} clients per rank (one per client, in id order)")
+        for c, t in zip(self.clients, tests or [None] * M):
+            c["test"] = (t, range(len(t))) if t is not None else (c["dataset"], range(c["nval"]))
+        self._fed_feeds: Dict[int, BatchFeeder] = {}
+        if cfg.fed_eval_every or tests is not None:
+            self._check_fedeval(tests)
         c0 = self.clients[0]
         self.dataset, self.n_train, self.label_counts = c0["dataset"], c0["n_train"], c0["label_counts"]   # n_k
         per, nval = c0["per"], c0["nval"]
@@ -631,6 +644,10 @@ class FederatedRunner:
             self.fedavg_pipelined()
         else:
             self.decrypt_apply(self.aggregate(self.encrypt_update()))
+        fed = None
+        if self.cfg.fed_eval_every and (self.round + 1) % self.cfg.fed_eval_every == 0:
+            with self.timer.stage("fed_eval"):
+                fed = self.evaluate_federated()
         if self.cfg.debug_poison:
             self.poison_buffers()
         times = self.timer.resolve()
@@ -648,6 +665,8 @@ class FederatedRunner:
             rec["val_accuracy"] = hist[-1].val_accuracy if hist else None
         if self.clients_per_rank > 1 or self.cfg.client_fraction < 1:
             rec.update(self._client_records(hists))
+        if fed is not None:
+            rec["fed_eval"] = fed
         if oracle:
             if self.world > 1:
                 dist.all_reduce(self._plain_sum, op=dist.ReduceOp.SUM, group=self.group)
@@ -770,6 +789,69 @@ class FederatedRunner:
                 probs[i:i + nv] = torch.softmax(logits[:nv].cpu(), dim=1)
                 cams[i:i + nv] = cam[:nv].cpu()
             return probs, cams
+
+    # ------------------------------------------------------------------ federated evaluation (DESIGN.md §13)
+    def _check_fedeval(self, tests=None) -> None:
+        first = self.clients[0]["dataset"]
+        check_fedeval_options(self.cfg, self.model.num_classes, self.n_ct * self.ctx.values_per_ct(self.cfg.packing),
+                              tests if tests is not None else [c["test"][0] for c in self.clients],
+                              getattr(first, "class_indices", None))
+
+    def _eval_seed(self, cid: int) -> int:
+        """Encryption randomness of client ``cid``'s count vector: never the seed of its model update."""
+        if self.cfg.deterministic_crypto:
+            h = hashlib.sha256(f"hefl-fedeval-{self.cfg.seed}-{self.round}-{cid}".encode()).digest()
+            return int.from_bytes(h[:8], "little") >> 1
+        return secrets.randbits(63)
+
+    def _fed_feed(self, i: int) -> Optional[BatchFeeder]:
+        ds, idx = self.clients[i]["test"]
+        if len(idx) == 0:
+            return None
+        if i not in self._fed_feeds:
+            self._fed_feeds[i] = BatchFeeder(ds, idx, self.cfg.batch_size, self.device, shuffle=False)
+        return self._fed_feeds[i]
+
+    @torch.no_grad()
+    def evaluate_federated(self) -> Dict:
+        """Federated evaluation of the deployed models (DESIGN.md §13); a collective that every rank must call. Every
+        local client, selected this round or not, scores the global model with its own personal layers on its test
+        set (``test_dataset``, else its 10 % validation split). Each client's count vector is encrypted with its own
+        seed and accumulated into a prefix of the rank's ciphertext buffer (weight 1: counts are sums), masked at
+        stream index round*4096 + 4095, all-reduced, decrypted by the key holder (or every rank holding sk) and
+        broadcast as float64. Returns ``metrics_from_counts`` of the sum, and under ``"local"`` this rank's clients'
+        plaintext metrics, which never leave the rank. Raises FloatingPointError if a decoded count is negative or
+        more than 0.25 from an integer. The global model, the server optimizer and the training state are untouched."""
+        self._check_fedeval()
+        cfg, ctx, dev = self.cfg, self.ctx, self.device
+        C, nb = self.model.num_classes, cfg.fed_eval_bins
+        V = count_len(C, nb)
+        rows = torch.zeros(self.clients_per_rank, V, dtype=torch.float64, device=dev)
+        for i in range(self.clients_per_rank):
+            feed = self._fed_feed(i)
+            if feed is not None:
+                with self._client_head(i):
+                    self.trainer.score(feed, rows[i])
+        n1 = ctx.num_ct(V, cfg.packing)
+        view = self.transport.buffer(self.ct_numel)[: n1 * 2 * ctx.L * ctx.n]
+        for i in range(self.clients_per_rank):        # an empty client adds an encryption of zeros
+            ct = ctx.encrypt(rows[i].float(), self.pk, seed=self._eval_seed(self.client_ids[i]), packing=cfg.packing,
+                             out=view, accumulate=i > 0)
+        self._mask(ct.data, chunk=4095)
+        data = self.transport.allreduce(ct.data)
+        vec = torch.empty(V, dtype=torch.float64, device=dev)
+        if self.has_sk:
+            vec.copy_(ctx.decrypt(CtBatch(data, ct.scale, V, cfg.packing), self.sk, divide_by=1.0).double())
+        if self.key_holder >= 0:
+            dist.broadcast(vec, src=self.key_holder, group=self.group)
+        vec = vec.cpu()
+        counts = vec[:-1].round()
+        if bool(((vec[:-1] - counts).abs() > 0.25).any()) or bool((counts < 0).any()):
+            raise FloatingPointError(f"round {self.round}: decoded evaluation counts are not non-negative integers "
+                                     f"(largest distance {float((vec[:-1] - counts).abs().max()):.3g})")
+        out = metrics_from_counts(torch.cat([counts, vec[-1:]]), C, nb)
+        out["local"] = [{"id": cid, **metrics_from_counts(rows[i].cpu(), C, nb)} for i, cid in enumerate(self.client_ids)]
+        return out
 
     def _check_images(self, images_u8: torch.Tensor) -> None:
         S, ch = self.cfg.image_size, self.cfg.in_channels
@@ -935,17 +1017,8 @@ def classification_metrics(y_true: torch.Tensor, y_pred: torch.Tensor, num_class
     y_true, y_pred = y_true.long().flatten(), y_pred.long().flatten()
     n = max(1, y_true.numel())
     num_classes = max(num_classes, int(max(y_true.max(), y_pred.max())) + 1) if y_true.numel() else num_classes
-    p_w = r_w = f_w = 0.0
-    for c in range(num_classes):
-        tp = float(((y_pred == c) & (y_true == c)).sum())
-        fp = float(((y_pred == c) & (y_true != c)).sum())
-        fn = float(((y_pred != c) & (y_true == c)).sum())
-        prec = tp / (tp + fp) if tp + fp > 0 else 0.0
-        rec = tp / (tp + fn) if tp + fn > 0 else 0.0
-        f1 = 2 * prec * rec / (prec + rec) if prec + rec > 0 else 0.0
-        w = (tp + fn) / n
-        p_w, r_w, f_w = p_w + w * prec, r_w + w * rec, f_w + w * f1
-    return {"precision": p_w, "recall": r_w, "f1": f_w, "accuracy": float((y_true == y_pred).sum()) / n}
+    conf = torch.bincount(y_true * num_classes + y_pred, minlength=num_classes * num_classes)
+    return metrics_from_confusion(conf.view(num_classes, num_classes).tolist(), n)
 
 
 def simulate_clients(cfg: FLConfig, device: Optional[torch.device] = None, rounds: int = 1,

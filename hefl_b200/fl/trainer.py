@@ -111,6 +111,9 @@ class LocalTrainer:
             self._slot_ready = [torch.cuda.Event() for _ in range(2)]
             self._slot_free = [torch.cuda.Event() for _ in range(2)]
             self._pre = None         # (feeder, train, iterator, slot) of a first batch staged ahead of its pass
+            self._score_graphs: Dict[int, torch.cuda.CUDAGraph] = {}     # captured by the first score() only
+            self._score_bufs = None  # (counts, loss, err), nvalid per slot, probs of the captured score graphs
+        self.score_launches = 0           # our kernels inside one score graph (+ the pre-process launch)
 
     # ------------------------------------------------------------------ one step (eager)
     def _prep(self, x_u8: torch.Tensor, train: bool) -> torch.Tensor:
@@ -288,6 +291,99 @@ class LocalTrainer:
         eng.after_restore()
         torch.cuda.synchronize(self.device)
 
+    def _alloc_score_bufs(self, nbins: int) -> None:
+        """(int32 counts, float64 loss sum, int32 error flag), the valid row count of each input slot, and probs."""
+        C, dev = self.model.fcs[-1].out_features, self.device
+        self._score_bufs = ((torch.zeros(C * C * (nbins + 1), dtype=torch.int32, device=dev),
+                             torch.zeros(1, dtype=torch.float64, device=dev), torch.zeros(1, dtype=torch.int32, device=dev)),
+                            [torch.zeros(1, dtype=torch.int32, device=dev) for _ in range(2)],
+                            torch.zeros(self.cfg.batch_size, C, dtype=torch.float32, device=dev))
+
+    def _score_step(self, slot: int, y: Optional[torch.Tensor] = None) -> None:
+        bufs, nv, probs = self._score_bufs
+        self.engine.score_staged(slot, self.static_y2[slot] if y is None else y, nv[slot], bufs, probs)
+
+    def _capture_score(self, nbins: int) -> None:
+        """Score graphs of the tcgen05 engine, one per input slot, captured by the first ``score`` only (and again if
+        the bin count changes), so a run that never scores captures exactly the graphs it captured before. Scoring
+        writes no parameter, gradient, optimiser state or augmentation position, so nothing needs restoring."""
+        eng, cur = self.engine, torch.cuda.current_stream(self.device)
+        self._alloc_score_bufs(nbins)
+        side = torch.cuda.Stream(self.device)
+        side.wait_stream(cur)
+        side.wait_stream(self.prep_stream)
+        with torch.cuda.stream(side):
+            for slot in range(2):
+                eng.preprocess(self.static_x, slot, False, False)
+            for _ in range(3):
+                for slot in range(2):
+                    self._score_step(slot)
+        cur.wait_stream(side)
+        torch.cuda.synchronize(self.device)
+        self._score_graphs = {}
+        for slot in range(2):
+            a = int(self.ops.launch_count())
+            g = torch.cuda.CUDAGraph()
+            with torch.cuda.graph(g):
+                self._score_step(slot)
+            self._score_graphs[slot] = g
+            if slot == 0:
+                self.score_launches = int(self.ops.launch_count()) - a + 1       # + the pre-process launch
+        torch.cuda.synchronize(self.device)
+
+    @torch.no_grad()
+    def score(self, feeder: BatchFeeder, counts_row: torch.Tensor) -> None:
+        """Federated-evaluation counts of the installed model (DESIGN.md §13) over one pass of the non-shuffled
+        ``feeder``, added into ``counts_row`` (float64 [V], ``fedeval`` layout) on the trainer's device. The tcgen05
+        engine scores on its own kernels -- graph-replayed in the ``_run_epoch`` pipeline, or eagerly without graphs;
+        the other backends run the model's forward in its dtype and ``score_counts_torch``. Weights, gradients,
+        optimiser state, the augmentation position and the RNG are left as they were. Raises ValueError if a label is
+        outside 0..C-1."""
+        from .fedeval import score_counts_torch
+
+        if feeder.shuffle:
+            raise ValueError("score needs a non-shuffled feeder (the wrapped rows of its last batch are skipped)")
+        C = self.model.fcs[-1].out_features if hasattr(self.model, "fcs") else None
+        rows, B = len(feeder.indices), feeder.bs
+        if rows == 0:
+            return
+        if self.engine is None:
+            nb = (counts_row.numel() - 1) // (C * C) - 1 if C else None
+            was = self.model.training
+            self.model.eval()
+            try:
+                for i, (x, y) in enumerate(feeder.epoch()):
+                    nv = min(B, rows - i * B)
+                    logits = self._forward(x, False).float()
+                    if nb is None:
+                        C = logits.shape[1]
+                        nb = (counts_row.numel() - 1) // (C * C) - 1
+                    if int(y[:nv].min()) < 0 or int(y[:nv].max()) >= C:
+                        raise ValueError(f"score: labels must be in 0..{C - 1}")
+                    counts_row.add_(score_counts_torch(logits[:nv], y[:nv], nb).to(counts_row.device))
+            finally:
+                self.model.train(was)
+            return
+        nbins = (counts_row.numel() - 1) // (C * C) - 1
+        graphs = self.use_graph
+        if graphs and (not self._score_graphs or self._score_bufs[0][0].numel() != counts_row.numel() - 1):
+            self._capture_score(nbins)
+        if not graphs and (self._score_bufs is None or self._score_bufs[0][0].numel() != counts_row.numel() - 1):
+            self._alloc_score_bufs(nbins)
+        (counts, loss, err), nv, _ = self._score_bufs
+        counts.zero_(); loss.zero_(); err.zero_()
+        if graphs:
+            self._run_epoch(feeder, False, None, score=True)
+        else:
+            for i, (x, y) in enumerate(feeder.epoch()):
+                self.engine.preprocess(x, 0, False, False)
+                nv[0].fill_(min(B, rows - i * B))
+                self._score_step(0, y)
+        if int(err.item()):
+            raise ValueError(f"score: labels must be in 0..{C - 1}")
+        counts_row[:-1].add_(counts.to(counts_row.device, torch.float64))
+        counts_row[-1:].add_(loss.to(counts_row.device))
+
     # ------------------------------------------------------------------ public API
     def prepare(self) -> None:
         """Capture the CUDA graphs now rather than at the first step (a rank with several clients captures once,
@@ -342,7 +438,8 @@ class LocalTrainer:
             self._eval_eager(x_u8, y)
         return self.out_eval
 
-    def _run_epoch(self, feeder, train: bool, stats: torch.Tensor, nxt=None, head: bool = False) -> None:
+    def _run_epoch(self, feeder, train: bool, stats: Optional[torch.Tensor], nxt=None, head: bool = False,
+                   score: bool = False) -> None:
         """One pass over ``feeder``; per-step [loss, ncorrect] land in ``stats`` (pinned host rows).
 
         tcgen05 engine + CUDA graphs: software pipeline over batches — batch i+1 is fetched (H2D or
@@ -350,19 +447,22 @@ class LocalTrainer:
         graph of step i runs on the main stream; events hand the slots back and forth. ``nxt`` =
         (feeder, train) of the pass that follows: its first batch is staged under this pass's last
         step, so consecutive passes (train -> validation -> next epoch) have no pipeline-fill bubble. ``head``: a
-        training pass of head-only steps (pre-processed and staged as a train pass)."""
+        training pass of head-only steps (pre-processed and staged as a train pass). ``score``: a pass of the captured
+        score graphs into ``_score_bufs`` (``stats`` unused): each slot's valid row count is set as it is staged, so
+        the rows the feeder wraps into the last batch are not counted, and nothing is read back."""
         if self.engine is None or not self.use_graph:
             for i, (x, y) in enumerate(feeder.epoch()):
                 out = self.head_step(x, y) if head else self.train_step(x, y) if train else self.eval_step(x, y)
                 stats[i].copy_(out, non_blocking=True)       # D2H of the step's loss/accuracy
             return
-        if not self._graphs:
+        if not self._graphs and not score:
             self._capture()
         if head and ("head", 0) not in self._graphs:
             self._capture_head()
         main, prep, sst = torch.cuda.current_stream(self.device), self.prep_stream, self.stats_stream
         n = feeder.steps
         outs = self.out_train2 if train else self.out_eval2
+        rows, staged = len(feeder.indices) if score else 0, [0]
 
         def stage(it, slot: int, tr: bool) -> None:
             with torch.cuda.stream(prep):
@@ -370,6 +470,9 @@ class LocalTrainer:
                 x, y = next(it)                               # feeder work (gather / wait for H2D) on prep
                 self.engine.preprocess(x, slot, tr, self.augment and tr)
                 self.static_y2[slot].copy_(y, non_blocking=True)
+                if score:
+                    self._score_bufs[1][slot].fill_(min(feeder.bs, rows - staged[0] * feeder.bs))
+                    staged[0] += 1
                 self._slot_ready[slot].record(prep)
 
         pre, self._pre = self._pre, None
@@ -392,6 +495,10 @@ class LocalTrainer:
                 stage(nit, slot ^ 1, nxt[1])
                 self._pre = (nxt[0], nxt[1], nit, slot ^ 1)
             main.wait_event(self._slot_ready[slot])
+            if score:
+                self._score_graphs[slot].replay()
+                self._slot_free[slot].record(main)
+                continue
             main.wait_event(self._stats_done[slot])           # result buffer of this slot has been read back
             self._graphs[("head" if head else train, slot)].replay()
             self._slot_free[slot].record(main)
@@ -399,7 +506,8 @@ class LocalTrainer:
                 sst.wait_event(self._slot_free[slot])
                 stats[i].copy_(outs[slot], non_blocking=True)
                 self._stats_done[slot].record(sst)
-        self.replayed_launches += n * (self.head_launches if head else self.graph_launches[0 if train else 1])
+        self.replayed_launches += n * (self.score_launches if score else self.head_launches if head
+                                       else self.graph_launches[0 if train else 1])
         with torch.cuda.stream(prep):
             for _ in it:                                      # let the feeder finish its bookkeeping
                 pass

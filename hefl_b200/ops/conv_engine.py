@@ -28,6 +28,8 @@ Replaces Keras' ``model.fit`` compute path (FLPyfhelin.py:118-136, :193) for the
   IG        (``ig_staged``, DESIGN.md §12) per path point: the scan in slot 1 scaled into slot 0, forward convs
             with every arg-max code, the head seeded with a class score, the un-pool / dgrad chain down to X[1],
             input_grad0 (the layer-1 input gradient straight from the pooled gradient, into an fp32 accumulator)
+  scoring   (``score_staged``, DESIGN.md §13) forward convs without arg-max codes, the head's logits (head_logits),
+            score_stats (confusion matrix, score histograms and loss sum of one client)
 
 All buffers are allocated once; a step is CUDA-graph capturable (one graph per input slot); every
 kernel uses programmatic dependent launch (csrc/nn/launch.cuh).
@@ -440,6 +442,27 @@ class MedCNNEngine:
         xh = x1[: self.P[0], :ci].view(B, S, S, ci)
         attr_out[:nvalid] = (xh[:nvalid].float() * acc[:nvalid]).sum(-1) / steps
         return t
+
+    def score_staged(self, slot: int, y: torch.Tensor, nvalid_dev: torch.Tensor, counts_row, probs_out: torch.Tensor) -> None:
+        """Federated-evaluation scoring (DESIGN.md §13) of the batch pre-processed into ``slot`` (``preprocess(..,
+        train=False, augment=False)``; CUDA-graph body): forward convs without arg-max codes, the head's logits
+        (head_logits; autograd-free PyTorch for heads the fused kernels do not cover) into ``score_logits``, then
+        score_stats. ``counts_row`` = (int32 counts [C*C*(nbins+1)], float64 loss sum [1], int32 error flag [1]) is
+        added into; ``probs_out`` [B, C] fp32; ``nvalid_dev`` int32 [1] on the device: rows >= it are not counted.
+        Only X, the head scratch, ``score_logits`` and the outputs change."""
+        counts, loss, err = counts_row
+        C = self.model.fcs[-1].out_features
+        nbins = counts.numel() // (C * C) - 1
+        if getattr(self, "score_logits", None) is None:
+            self.score_logits = torch.zeros(self.B, C, dtype=torch.float32, device=self.device)
+        feat_bf = self.forward_convs(slot, False)
+        if self.fused_head:
+            self.ops.head_logits(feat_bf, self.pack.flat, self.head_offs, self.h1_buf, self.dh1_buf, self.score_logits,
+                                 self.B, self.F, self.H1, self.H2, self.C)
+        else:
+            with torch.no_grad():
+                self.score_logits.copy_(self._head(feat_bf.view(self.B, -1).float()))
+        self.ops.score_stats(self.score_logits, y, nvalid_dev, probs_out, counts, loss, err, nbins)
 
     def eval_step(self, x_u8: torch.Tensor, y: torch.Tensor, out: torch.Tensor) -> None:
         self.preprocess(x_u8, 0, False, False)
